@@ -124,6 +124,11 @@ SIGNATURES = {
                                           C.c_int]),
     "dpgo_agents_host_io_async": (C.c_int, [C.POINTER(_vp), C.c_int, C.POINTER(_vp), C.POINTER(_vp), C.c_int, _vp]),
     "dpgo_agent_f_rgradnorm_resident": (C.c_int, [_vp, _dp, _dp]),
+    "dpgo_agent_set_local_trajectory": (C.c_int, [_vp, _dp, _dp]),
+    "dpgo_agent_set_align_candidates": (C.c_int, [_vp, C.c_int, _ip, _ip, _ip, _ip, _ip, _dp]),
+    "dpgo_agents_align_async": (C.c_int, [C.POINTER(_vp), C.c_int, _vp, C.c_int64, _ip, C.c_int, _vp]),
+    "dpgo_agent_align_result": (C.c_int, [_vp, _dp, _ip]),
+    "dpgo_robust_single_rotation_averaging": (C.c_int, [C.c_int, C.c_int, C.c_int, _dp, _dp, C.c_double, _dp, _ip, _ip]),
 }
 
 _lib = None

@@ -13,6 +13,7 @@ rebuilt on the device from the gathered tiles (ref PGOAgent::constructGMatrix, s
 from __future__ import annotations
 
 import ctypes as C
+import time
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -130,6 +131,44 @@ class ExchangePlan:
                 c += 1
             colour[a] = c
         return colour
+
+
+# ---------------------------------------------------------------------------------------------------
+# distributed initialisation: host tables
+# ---------------------------------------------------------------------------------------------------
+def check_private_graph_connected(agent: int, n: int, private: EdgeSet) -> None:
+    """The chordal initialisation of a private graph (odometry + private loop closures) is singular unless the graph is
+    connected; some partitions leave an agent with several pieces."""
+    if n <= 1:
+        return
+    import scipy.sparse as sp
+    from scipy.sparse.csgraph import connected_components
+    A = sp.coo_matrix((np.ones(len(private)), (private.p1, private.p2)), shape=(n, n))
+    pieces = connected_components(A, directed=False)[0]
+    if pieces != 1:
+        raise ValueError(f"agent {agent}: the private pose graph (odometry + private loop closures) has {pieces} connected "
+                         f"components, so its local chordal initialisation is singular")
+
+
+def alignment_candidates(agent: int, shared: EdgeSet, plan: ExchangePlan):
+    """Candidate table of dpgo_agent_set_align_candidates: one candidate per public pose j of a neighbour b that the agent
+    shares an edge with, grouped per neighbour in increasing id, j increasing (std::map<PoseID> order), each through the
+    FIRST shared edge touching (b, j) (ref findSharedLoopClosureWithNeighbor, src/PGOAgent.cpp:922-934)."""
+    out = shared.r1 == agent
+    nbr = np.where(out, shared.r2, shared.r1)
+    nq = np.where(out, shared.p2, shared.p1)
+    first: Dict[PoseID, int] = {}
+    for e in range(len(shared)):
+        first.setdefault((int(nbr[e]), int(nq[e])), e)
+    keys = sorted(first)
+    idx = np.array([first[key] for key in keys], dtype=np.int64)
+    groups = sorted({b for b, _ in keys})
+    ptr = np.searchsorted([b for b, _ in keys], groups + [groups[-1] + 1 if groups else 0]).astype(np.int32)
+    return dict(neighbor=np.array(groups, dtype=np.int32), ptr=ptr,
+                local=np.where(out, shared.p1, shared.p2)[idx].astype(np.int32),
+                slot=np.array([plan.slot(b, j) for b, j in keys], dtype=np.int32),
+                outgoing=out[idx].astype(np.int32),
+                T=np.ascontiguousarray(shared.homogeneous()[idx]))
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -450,8 +489,16 @@ class DistributedPGO:
                  preconditioner: int = capi.PRECOND_SPARSE_EXACT, schedule: str = "greedy",
                  owner: Optional[np.ndarray] = None, X_init: Optional[np.ndarray] = None,
                  rank: Optional[int] = None, world: Optional[int] = None, device: int = 0, dist=None,
-                 acceleration: bool = False, restart_interval: int = 30, concurrent: Optional[bool] = None):
-        """concurrent: the active agents of a round that share a GPU step side by side (each as one thread-block cluster on
+                 acceleration: bool = False, restart_interval: int = 30, concurrent: Optional[bool] = None,
+                 initialization: str = "central"):
+        """initialization: "central" -- every rank computes one chordal initialisation of the whole graph (or takes
+        X_init); "distributed" -- the reference's multi-robot protocol (ref PGOAgentParameters::multirobot_initialization,
+        include/DPGO/PGOAgent.h:129): each rank solves only its own agents' private graphs, in their own frames, on its
+        GPU; agent 0 defines the global frame and the others join it wave by wave through a robust average (GNC-TLS
+        rotation averaging, inlier translation mean) of the frame transforms their shared loop closures give with an
+        initialised neighbour (ref src/PGOAgent.cpp:369-440).  Needs X_init None; init_report / init_times describe it.
+
+        concurrent: the active agents of a round that share a GPU step side by side (each as one thread-block cluster on
         its own stream, one C call per round: dpgo_agents_round_async) instead of one after the other as full-grid kernels.
         None = automatic: on when some round has >= 2 active agents on a rank (greedy / coloured schedules, no
         acceleration).  The iterates of the two modes agree to rounding, not bitwise (different reduction trees), so
@@ -473,7 +520,12 @@ class DistributedPGO:
         self.colour = self.plan.colouring()
         self.ncolours = max(self.colour) + 1
         self.schedule = schedule
-        if X_init is None:
+        if initialization not in ("central", "distributed"):
+            raise ValueError("initialization must be 'central' or 'distributed'")
+        if initialization == "distributed" and X_init is not None:
+            raise ValueError("initialization='distributed' computes the start itself: X_init must be None")
+        self.initialization = initialization
+        if X_init is None and initialization == "central":
             X_init = pg.fixedStiefelVariable(self.d, r) @ pg.chordalInitialization(self.d, n, edges)
         per_rank = k // self.world
         self.local_ids = list(range(rank * per_rank, (rank + 1) * per_rank)) if self.distributed else list(range(k))
@@ -486,6 +538,12 @@ class DistributedPGO:
         dh = self.d + 1
         self.dev = torch.device("cuda", device)
         stream = torch.cuda.current_stream(self.dev).cuda_stream
+        YLift = np.asfortranarray(pg.fixedStiefelVariable(self.d, r))
+        self.init_times = {}
+        if initialization == "distributed":
+            for a in range(k):                             # every rank checks every agent, so all ranks raise alike
+                check_private_graph_connected(a, int(counts[a]), EdgeSet.join([parts[a][0], parts[a][1]]))
+            self.init_times["local_chordal_s"] = 0.0
         for a in self.local_ids:
             prm = PGOAgentParameters(self.d, r, k, algorithm=algorithm, preconditioner=preconditioner, device=device,
                                      cluster=self.concurrent)
@@ -493,10 +551,25 @@ class DistributedPGO:
             ag.mState = PGOAgentState.WAIT_FOR_DATA
             ag.YLift = None
             ag.setPoseGraph(*parts[a], TInit=np.zeros((self.d, dh * int(counts[a]))), n=int(counts[a]))
-            cols = (glob[a][:, None] * dh + np.arange(dh)[None, :]).ravel()
-            ag.setX(X_init[:, cols])
             ag.mProblem.set_stream(stream)
-            ag.mProblem.upload_X(ag.X)
+            if X_init is not None:
+                cols = (glob[a][:, None] * dh + np.arange(dh)[None, :]).ravel()
+                ag.setX(X_init[:, cols])
+                ag.mProblem.upload_X(ag.X)
+            else:                                          # ref localInitialization, src/PGOAgent.cpp:947-962
+                t_local = time.perf_counter()
+                priv = EdgeSet.join([parts[a][0], parts[a][1]])
+                T = pg.chordalInitializationGPU(self.d, int(counts[a]), priv, device=device) if counts[a] > 1 else \
+                    np.hstack([np.eye(self.d), np.zeros((self.d, 1))])
+                lib = ag.mProblem._lib
+                capi.check(lib.dpgo_agent_set_local_trajectory(ag.mProblem._h, capi.dptr(np.asfortranarray(T)),
+                                                               capi.dptr(YLift)))          # synchronous
+                self.init_times["local_chordal_s"] += time.perf_counter() - t_local
+                ct = alignment_candidates(a, parts[a][2], self.plan)
+                capi.check(lib.dpgo_agent_set_align_candidates(ag.mProblem._h, len(ct["neighbor"]), capi.iptr(ct["neighbor"]),
+                                                               capi.iptr(ct["ptr"]), capi.iptr(ct["local"]),
+                                                               capi.iptr(ct["slot"]), capi.iptr(ct["outgoing"]),
+                                                               capi.dptr(ct["T"])))
             ag.attach_exchange(self.plan)
             ag.opt = QuadraticOptimizer(ag.mProblem)
             ag.opt.setAlgorithm(algorithm)
@@ -519,6 +592,18 @@ class DistributedPGO:
         else:
             self.send_all = None
             self.send = {a: self.gathered[a * self.slot_elems:(a + 1) * self.slot_elems] for a in self.local_ids}
+        self._main_stream = stream if stream else 1          # 0 = torch's legacy default stream = cudaStreamLegacy (handle 1)
+        if initialization == "distributed":
+            torch.cuda.synchronize(self.dev)
+            t_waves = time.perf_counter()
+            self.init_report = self._align_waves()
+            torch.cuda.synchronize(self.dev)
+            self.init_times["waves_s"] = time.perf_counter() - t_waves
+            for a in self.local_ids:
+                self.agents[a].X = self.agents[a].mProblem.download_X()
+                self.agents[a].mState = PGOAgentState.INITIALIZED
+        else:
+            self.init_report = None
         if self.acceleration:
             # Nesterov-accelerated RBCD (ref src/PGOAgent.cpp:685-695,1040-1091): auxiliary iterates resident per agent,
             # their public tiles in a second gathered buffer (ref getAuxSharedPoseDict / updateAuxNeighborPoses)
@@ -538,8 +623,57 @@ class DistributedPGO:
         self.stats_all = torch.zeros(4 * k, dtype=torch.float64, device=self.dev)
         self.selected = [0]
         self.round = 0
-        self._main_stream = stream if stream else 1          # 0 = torch's legacy default stream = cudaStreamLegacy (handle 1)
         self._gathered_current = False       # concurrent mode: `gathered` holds every agent's current public tiles
+
+    # -- distributed initialisation: alignment waves (ref src/PGOAgent.cpp:369-440, examples/MultiRobotExample.cpp:245-256) --
+    def _align_waves(self) -> List[Dict[str, int]]:
+        """Wave w >= 1: one exchange of the public tiles; every agent that is not initialised and has a neighbour
+        initialised before the wave tries those neighbours in increasing id on the device (one call per GPU); the first
+        with a non-empty inlier set moves the agent into the global frame.  The outcome travels by one small all-gather
+        per wave.  At most k - 1 waves: a wave that initialises nobody is an error."""
+        torch, k = self.torch, self.k
+        lib = self.agents[self.local_ids[0]].mProblem._lib
+        ready = np.zeros(k, dtype=np.int32)
+        ready[0] = 1
+        report = [dict(wave=-1, neighbor=-1, candidates=0, inliers=0, iterations=0) for _ in range(k)]
+        report[0]["wave"] = 0
+        base = self.local_ids[0]
+        if self.distributed:
+            rec_local = torch.zeros(5 * len(self.local_ids), dtype=torch.float64, device=self.dev)
+            rec_all = torch.zeros(5 * k, dtype=torch.float64, device=self.dev)
+        wave = 0
+        while not ready.all():
+            wave += 1
+            self.exchange(build=False)
+            todo = [a for a in self.local_ids if not ready[a] and any(ready[b] for b in self.plan.tables[a]["neighbors"])]
+            rec = np.zeros((len(self.local_ids), 5))        # aligned, neighbour, candidates, inliers, GNC iterations
+            if todo:
+                hs = (C.c_void_p * len(todo))(*[self.agents[a].mProblem._h for a in todo])
+                capi.check(lib.dpgo_agents_align_async(hs, len(todo), C.c_void_p(self.gathered.data_ptr()),
+                                                       self.k * self.plan.pmax, capi.iptr(ready), k,
+                                                       C.c_void_p(self._main_stream)))
+                info = np.zeros(4, dtype=np.int32)
+                for a in todo:
+                    capi.check(lib.dpgo_agent_align_result(self.agents[a].mProblem._h, None, capi.iptr(info)))
+                    rec[a - base] = (1.0 if info[2] > 0 else 0.0, info[0], info[1], info[2], info[3])
+            if self.distributed:
+                rec_local.copy_(torch.from_numpy(rec.ravel()))
+                self.dist.all_gather_into_tensor(rec_all, rec_local)
+                rec = rec_all.cpu().numpy().reshape(k, 5)
+            newly = []
+            for a in range(k):
+                if rec[a, 2] > 0:
+                    report[a].update(neighbor=int(rec[a, 1]), candidates=int(rec[a, 2]), inliers=int(rec[a, 3]),
+                                     iterations=int(rec[a, 4]))
+                if rec[a, 0] > 0:
+                    report[a]["wave"] = wave
+                    newly.append(a)
+            if not newly:
+                rest = [a for a in range(k) if not ready[a]]
+                raise RuntimeError(f"distributed initialisation: agents {rest} cannot join the global frame (no initialised "
+                                   f"neighbour gives a non-empty inlier set; is the agent graph connected?)")
+            ready[newly] = 1
+        return report
 
     # -- the exchange: ONE all-gather of the padded public-pose tiles --------------------------------
     def exchange(self, build: bool = True) -> None:

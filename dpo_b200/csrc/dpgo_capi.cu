@@ -102,6 +102,17 @@ struct dpgo_problem {
   bool G_dirty = true;           // G may hold values that dpgo_agent_build_G does not overwrite
   int *d_pose_ids = nullptr, *d_pose_ptr = nullptr, *d_edge_slot = nullptr, *d_edge_out = nullptr;
   double *d_edge_T = nullptr, *d_edge_om = nullptr;
+  // distributed initialisation (dpgo_align.cu): local-frame trajectory, lift, alignment candidates, result
+  double *d_Tloc = nullptr, *d_ylift = nullptr;
+  int align_groups = 0, align_cands = 0, align_max_slot = -1, align_max_nbr = -1;
+  int *d_grp_nbr = nullptr, *d_grp_ptr = nullptr, *d_cand_local = nullptr, *d_cand_slot = nullptr, *d_cand_out = nullptr;
+  double *d_cand_T = nullptr, *d_cand_R = nullptr, *d_cand_t = nullptr, *d_cand_w = nullptr;
+  double *d_T_align = nullptr;
+  int *d_align_info = nullptr;
+  dpgo::AlignJob *d_jobs = nullptr;        // per-call tables of dpgo_agents_align_async (kept by the call's first agent)
+  int *d_ready = nullptr;
+  int jobs_cap = 0, ready_cap = 0;
+  cudaEvent_t ev_align = nullptr;          // recorded on the stream of the last dpgo_agents_align_async that aligned this agent
 
   size_t vec_bytes() const { return sizeof(double) * (size_t)r * (size_t)N; }
 };
@@ -690,12 +701,16 @@ int dpgo_problem_destroy(dpgo_problem_t *p) {
   free_dev(p->d_eT); free_dev(p->d_eom); free_dev(p->d_ew); free_dev(p->d_sblk); free_dev(p->d_eres);
   free_dev(p->d_public); free_dev(p->d_pose_ids); free_dev(p->d_pose_ptr); free_dev(p->d_edge_slot);
   free_dev(p->d_edge_out); free_dev(p->d_edge_T); free_dev(p->d_edge_om);
+  free_dev(p->d_Tloc); free_dev(p->d_ylift); free_dev(p->d_grp_nbr); free_dev(p->d_grp_ptr); free_dev(p->d_cand_local);
+  free_dev(p->d_cand_slot); free_dev(p->d_cand_out); free_dev(p->d_cand_T); free_dev(p->d_cand_R); free_dev(p->d_cand_t);
+  free_dev(p->d_cand_w); free_dev(p->d_T_align); free_dev(p->d_align_info); free_dev(p->d_jobs); free_dev(p->d_ready);
   free_nd(p);
   if (p->h_result) cudaFreeHost(p->h_result);
   for (auto &g : p->round_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   p->round_graphs.clear();
   if (p->ev_done) cudaEventDestroy(p->ev_done);
   if (p->ev_fork) cudaEventDestroy(p->ev_fork);
+  if (p->ev_align) cudaEventDestroy(p->ev_align);
   if (p->own_stream) cudaStreamDestroy(p->own_stream);
   delete p;
   return DPGO_OK;
@@ -1703,6 +1718,196 @@ int dpgo_agent_f_rgradnorm_resident(dpgo_problem_t *p, double *f_out, double *no
   DPGO_TRY(fetch_result(p));
   if (f_out) *f_out = p->h_result->f_init;
   if (norm_out) *norm_out = p->h_result->gradnorm_init;
+  return DPGO_OK;
+}
+
+
+// ---- distributed initialisation: frame alignment -------------------------------------------------------
+namespace {
+int ensure_jobs(dpgo_problem *p, int jobs, int ready) {
+  if (jobs > p->jobs_cap) {
+    free_dev(p->d_jobs);
+    DPGO_CUDA(cudaMalloc(&p->d_jobs, sizeof(dpgo::AlignJob) * jobs));
+    p->jobs_cap = jobs;
+  }
+  if (ready > p->ready_cap) {
+    free_dev(p->d_ready);
+    DPGO_CUDA(cudaMalloc(&p->d_ready, sizeof(int) * ready));
+    p->ready_cap = ready;
+  }
+  return DPGO_OK;
+}
+
+dpgo::AlignJob align_job(const dpgo_problem *p) {
+  dpgo::AlignJob J = {};
+  J.ngroups = p->align_groups;
+  J.n = p->n;
+  J.grp_nbr = p->d_grp_nbr; J.grp_ptr = p->d_grp_ptr;
+  J.cand_local = p->d_cand_local; J.cand_slot = p->d_cand_slot; J.cand_out = p->d_cand_out; J.cand_T = p->d_cand_T;
+  J.kappa = nullptr;
+  J.cand_R = p->d_cand_R; J.cand_t = p->d_cand_t; J.w = p->d_cand_w;
+  J.Tloc = p->d_Tloc; J.ylift = p->d_ylift; J.X = p->d_vec[dpgo::V_X0];
+  J.T_align = p->d_T_align; J.info = p->d_align_info;
+  return J;
+}
+}  // namespace
+
+int dpgo_agent_set_local_trajectory(dpgo_problem_t *p, const double *T_host, const double *YLift_host) {
+  DPGO_CHECK_HANDLE(p);
+  DPGO_REQUIRE(T_host && YLift_host, DPGO_ERR_INVALID_ARG, "null trajectory or lifting matrix");
+  const size_t tn = (size_t)p->d * p->dh * p->n, yn = (size_t)p->r * p->d;
+  if (!p->d_Tloc) DPGO_CUDA(cudaMalloc(&p->d_Tloc, sizeof(double) * tn));
+  if (!p->d_ylift) DPGO_CUDA(cudaMalloc(&p->d_ylift, sizeof(double) * yn));
+  DPGO_CUDA(cudaMemcpyAsync(p->d_Tloc, T_host, sizeof(double) * tn, cudaMemcpyHostToDevice, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(p->d_ylift, YLift_host, sizeof(double) * yn, cudaMemcpyHostToDevice, p->stream));
+  DPGO_TRY(ensure_jobs(p, 1, 0));
+  dpgo::AlignJob J = align_job(p);
+  J.T_align = nullptr;                     // identity: X = YLift T
+  J.info = nullptr;
+  DPGO_CUDA(cudaMemcpyAsync(p->d_jobs, &J, sizeof(J), cudaMemcpyHostToDevice, p->stream));
+  DPGO_CUDA(dpgo::launch_frame_lift(p->d, p->r, 1, p->n, p->d_jobs, p->stream));
+  DPGO_CUDA(cudaStreamSynchronize(p->stream));
+  return DPGO_OK;
+}
+
+int dpgo_agent_set_align_candidates(dpgo_problem_t *p, int num_groups, const int32_t *group_neighbor, const int32_t *group_ptr,
+                                    const int32_t *local_pose, const int32_t *nbr_slot, const int32_t *outgoing, const double *T) {
+  DPGO_CHECK_HANDLE(p);
+  DPGO_REQUIRE(num_groups >= 0 && (num_groups == 0 || (group_neighbor && group_ptr)), DPGO_ERR_INVALID_ARG, "bad candidate groups");
+  const int m = num_groups ? group_ptr[num_groups] : 0;
+  DPGO_REQUIRE(!num_groups || group_ptr[0] == 0, DPGO_ERR_INVALID_ARG, "group_ptr must start at 0");
+  for (int g = 0; g < num_groups; ++g) {
+    DPGO_REQUIRE(group_ptr[g + 1] > group_ptr[g], DPGO_ERR_INVALID_ARG, "every candidate group needs a candidate");
+    DPGO_REQUIRE(group_neighbor[g] >= 0 && (g == 0 || group_neighbor[g] > group_neighbor[g - 1]), DPGO_ERR_INVALID_ARG,
+                 "candidate groups must be in increasing neighbour id");
+  }
+  DPGO_REQUIRE(m == 0 || (local_pose && nbr_slot && outgoing && T), DPGO_ERR_INVALID_ARG, "null candidate arrays");
+  int max_slot = -1;
+  for (int q = 0; q < m; ++q) {
+    DPGO_REQUIRE(local_pose[q] >= 0 && local_pose[q] < p->n && nbr_slot[q] >= 0, DPGO_ERR_INVALID_ARG,
+                 "candidate index out of range");
+    max_slot = std::max(max_slot, (int)nbr_slot[q]);
+  }
+  free_dev(p->d_grp_nbr); free_dev(p->d_grp_ptr); free_dev(p->d_cand_local); free_dev(p->d_cand_slot); free_dev(p->d_cand_out);
+  free_dev(p->d_cand_T); free_dev(p->d_cand_R); free_dev(p->d_cand_t); free_dev(p->d_cand_w);
+  p->align_groups = num_groups;
+  p->align_cands = m;
+  p->align_max_slot = max_slot;
+  p->align_max_nbr = num_groups ? group_neighbor[num_groups - 1] : -1;
+  if (!p->d_T_align) DPGO_CUDA(cudaMalloc(&p->d_T_align, sizeof(double) * p->d * p->dh));
+  if (!p->d_align_info) DPGO_CUDA(cudaMalloc(&p->d_align_info, sizeof(int) * 4));
+  if (!num_groups) return DPGO_OK;
+  const int dh = p->dh;
+  DPGO_CUDA(cudaMalloc(&p->d_grp_nbr, sizeof(int) * num_groups));
+  DPGO_CUDA(cudaMalloc(&p->d_grp_ptr, sizeof(int) * (num_groups + 1)));
+  DPGO_CUDA(cudaMalloc(&p->d_cand_local, sizeof(int) * m));
+  DPGO_CUDA(cudaMalloc(&p->d_cand_slot, sizeof(int) * m));
+  DPGO_CUDA(cudaMalloc(&p->d_cand_out, sizeof(int) * m));
+  DPGO_CUDA(cudaMalloc(&p->d_cand_T, sizeof(double) * m * dh * dh));
+  DPGO_CUDA(cudaMalloc(&p->d_cand_R, sizeof(double) * m * p->d * p->d));
+  DPGO_CUDA(cudaMalloc(&p->d_cand_t, sizeof(double) * m * p->d));
+  DPGO_CUDA(cudaMalloc(&p->d_cand_w, sizeof(double) * m));
+  DPGO_CUDA(cudaMemcpy(p->d_grp_nbr, group_neighbor, sizeof(int) * num_groups, cudaMemcpyHostToDevice));
+  DPGO_CUDA(cudaMemcpy(p->d_grp_ptr, group_ptr, sizeof(int) * (num_groups + 1), cudaMemcpyHostToDevice));
+  DPGO_CUDA(cudaMemcpy(p->d_cand_local, local_pose, sizeof(int) * m, cudaMemcpyHostToDevice));
+  DPGO_CUDA(cudaMemcpy(p->d_cand_slot, nbr_slot, sizeof(int) * m, cudaMemcpyHostToDevice));
+  std::vector<int> outg(m);
+  for (int q = 0; q < m; ++q) outg[q] = outgoing[q] ? 1 : 0;
+  DPGO_CUDA(cudaMemcpy(p->d_cand_out, outg.data(), sizeof(int) * m, cudaMemcpyHostToDevice));
+  DPGO_CUDA(cudaMemcpy(p->d_cand_T, T, sizeof(double) * m * dh * dh, cudaMemcpyHostToDevice));
+  return DPGO_OK;
+}
+
+int dpgo_agents_align_async(dpgo_problem_t *const *agents, int count, const double *gathered_dev, int64_t num_slots,
+                            const int32_t *ready_host, int num_agents, void *stream) {
+  DPGO_REQUIRE(agents && count >= 1 && agents[0], DPGO_ERR_INVALID_ARG, "no agents to align");
+  DPGO_REQUIRE(ready_host && num_agents >= 1, DPGO_ERR_INVALID_ARG, "null ready flags");
+  dpgo_problem *lead = agents[0];
+  DPGO_CHECK_HANDLE(lead);
+  std::vector<dpgo::AlignJob> jobs((size_t)count);
+  int max_cands = 0, max_poses = 0;
+  for (int i = 0; i < count; ++i) {
+    dpgo_problem *p = agents[i];
+    DPGO_REQUIRE(p && p->device == lead->device && p->d == lead->d && p->r == lead->r, DPGO_ERR_INVALID_ARG,
+                 "the agents of one align call must share the device, d and r");
+    DPGO_REQUIRE(p->d_Tloc && p->d_T_align, DPGO_ERR_STATE,
+                 "dpgo_agent_set_local_trajectory and dpgo_agent_set_align_candidates must be called first");
+    DPGO_REQUIRE(p->align_cands == 0 || (gathered_dev && p->align_max_slot < num_slots), DPGO_ERR_INVALID_ARG,
+                 "a candidate refers to a slot beyond the gathered buffer");
+    DPGO_REQUIRE(p->align_max_nbr < num_agents, DPGO_ERR_INVALID_ARG, "a candidate group names an agent beyond the ready flags");
+    if (!p->ev_align) DPGO_CUDA(cudaEventCreateWithFlags(&p->ev_align, cudaEventDisableTiming));
+    jobs[(size_t)i] = align_job(p);
+    max_cands = std::max(max_cands, p->align_cands);
+    max_poses = std::max(max_poses, p->n);
+  }
+  cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
+  DPGO_TRY(ensure_jobs(lead, count, num_agents));
+  DPGO_CUDA(cudaMemcpyAsync(lead->d_jobs, jobs.data(), sizeof(dpgo::AlignJob) * count, cudaMemcpyHostToDevice, st));
+  DPGO_CUDA(cudaMemcpyAsync(lead->d_ready, ready_host, sizeof(int) * num_agents, cudaMemcpyHostToDevice, st));
+  DPGO_CUDA(dpgo::launch_align_candidates(lead->d, lead->r, count, max_cands, lead->d_jobs, gathered_dev, st));
+  DPGO_CUDA(dpgo::launch_robust_rotation_average(lead->d, count, lead->d_jobs, lead->d_ready, 2.0 * std::sqrt(2.0) * std::sin(0.25), st));
+  DPGO_CUDA(dpgo::launch_frame_lift(lead->d, lead->r, count, max_poses, lead->d_jobs, st));
+  for (int i = 0; i < count; ++i) DPGO_CUDA(cudaEventRecord(agents[i]->ev_align, st));   // dpgo_agent_align_result waits on it
+  return DPGO_OK;
+}
+
+int dpgo_agent_align_result(dpgo_problem_t *p, double *T_align_host, int32_t *info4) {
+  DPGO_CHECK_HANDLE(p);
+  DPGO_REQUIRE(p->d_T_align, DPGO_ERR_STATE, "dpgo_agent_set_align_candidates has not been called");
+  DPGO_REQUIRE(info4, DPGO_ERR_INVALID_ARG, "null info");
+  if (p->ev_align) DPGO_CUDA(cudaEventSynchronize(p->ev_align));     // the align call may have run on another stream
+  if (T_align_host)
+    DPGO_CUDA(cudaMemcpyAsync(T_align_host, p->d_T_align, sizeof(double) * p->d * p->dh, cudaMemcpyDeviceToHost, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(info4, p->d_align_info, sizeof(int) * 4, cudaMemcpyDeviceToHost, p->stream));
+  DPGO_CUDA(cudaStreamSynchronize(p->stream));
+  return DPGO_OK;
+}
+
+int dpgo_robust_single_rotation_averaging(int device, int d, int m, const double *R_host, const double *kappa_host,
+                                          double threshold, double *R_out, int32_t *inlier_flags, int32_t *iterations) {
+  DPGO_REQUIRE(d == 2 || d == 3, DPGO_ERR_UNSUPPORTED, "d must be 2 or 3");
+  DPGO_REQUIRE(m >= 1 && R_host && R_out, DPGO_ERR_INVALID_ARG, "need m >= 1 rotations and an output");
+  DPGO_REQUIRE(threshold > 0, DPGO_ERR_INVALID_ARG, "threshold must be positive");
+  int count = 0;
+  if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count)
+    return fail(DPGO_ERR_NO_DEVICE, "no such CUDA device: the GPU path has no CPU fallback");
+  DPGO_CUDA(cudaSetDevice(device));
+  struct Bufs {
+    double *R = nullptr, *k = nullptr, *w = nullptr, *T = nullptr;
+    int *grp = nullptr, *info = nullptr;
+    dpgo::AlignJob *job = nullptr;
+    ~Bufs() { free_dev(R); free_dev(k); free_dev(w); free_dev(T); free_dev(grp); free_dev(info); free_dev(job); }
+  } b;
+  DPGO_CUDA(cudaMalloc(&b.R, sizeof(double) * m * d * d));
+  DPGO_CUDA(cudaMalloc(&b.w, sizeof(double) * m));
+  DPGO_CUDA(cudaMalloc(&b.T, sizeof(double) * d * (d + 1)));
+  DPGO_CUDA(cudaMalloc(&b.grp, sizeof(int) * 4));
+  DPGO_CUDA(cudaMalloc(&b.info, sizeof(int) * 4));
+  DPGO_CUDA(cudaMalloc(&b.job, sizeof(dpgo::AlignJob)));
+  DPGO_CUDA(cudaMemcpy(b.R, R_host, sizeof(double) * m * d * d, cudaMemcpyHostToDevice));
+  if (kappa_host) {
+    DPGO_CUDA(cudaMalloc(&b.k, sizeof(double) * m));
+    DPGO_CUDA(cudaMemcpy(b.k, kappa_host, sizeof(double) * m, cudaMemcpyHostToDevice));
+  }
+  const int grp[4] = {0, 0, m, 1};         // neighbour 0, candidates [0, m), ready flag of neighbour 0
+  DPGO_CUDA(cudaMemcpy(b.grp, grp, sizeof(grp), cudaMemcpyHostToDevice));
+  dpgo::AlignJob J = {};
+  J.ngroups = 1;
+  J.grp_nbr = b.grp; J.grp_ptr = b.grp + 1;
+  J.kappa = b.k; J.cand_R = b.R; J.w = b.w;
+  J.T_align = b.T; J.info = b.info;
+  DPGO_CUDA(cudaMemcpy(b.job, &J, sizeof(J), cudaMemcpyHostToDevice));
+  DPGO_CUDA(dpgo::launch_robust_rotation_average(d, 1, b.job, b.grp + 3, threshold, nullptr));
+  std::vector<double> T((size_t)d * (d + 1)), w((size_t)m);
+  int info[4];
+  DPGO_CUDA(cudaMemcpy(T.data(), b.T, sizeof(double) * T.size(), cudaMemcpyDeviceToHost));
+  DPGO_CUDA(cudaMemcpy(w.data(), b.w, sizeof(double) * m, cudaMemcpyDeviceToHost));
+  DPGO_CUDA(cudaMemcpy(info, b.info, sizeof(info), cudaMemcpyDeviceToHost));
+  for (int a = 0; a < d; ++a)
+    for (int c = 0; c < d; ++c) R_out[a * d + c] = T[(size_t)c * d + a];
+  if (inlier_flags)
+    for (int q = 0; q < m; ++q) inlier_flags[q] = w[(size_t)q] > 1.0 - 1e-8 ? 1 : 0;
+  if (iterations) *iterations = info[3];
   return DPGO_OK;
 }
 

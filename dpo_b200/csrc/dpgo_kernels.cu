@@ -11,6 +11,7 @@
 //  small kernels    : Stiefel (polar) projection, public-pose packing, G assembly.
 #include "dpgo_device.cuh"
 #include "dpgo_kernels.cuh"
+#include "dpgo_rotation.cuh"
 #include <cooperative_groups.h>
 #include <algorithm>
 
@@ -1540,12 +1541,7 @@ __global__ void k_edge_weights(int64_t m, const int *__restrict__ p1, const int 
   else if (cost == 2) wt = (r < param) ? 1.0 : param / r;
   else if (cost == 3) wt = (r < param) ? 1.0 : 0.0;
   else if (cost == 4) { const double s = 1.0 + r2; wt = 1.0 / (s * s); }
-  else if (cost == 5) {
-    const double c2 = param * param;
-    if (r2 >= c2 * (mu + 1.0) / mu) wt = 0.0;
-    else if (r2 <= c2 * mu / (mu + 1.0)) wt = 1.0;
-    else wt = sqrt(c2 * mu * (mu + 1.0) / r2) - mu;
-  }
+  else if (cost == 5) wt = gnc_tls_weight(r2, mu, param);
   w[e] = wt;
 }
 

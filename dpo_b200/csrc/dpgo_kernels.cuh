@@ -123,4 +123,30 @@ cudaError_t launch_bsr_to_dense(int n, int dh, int64_t nb, const int *rowptr, co
 // dense SPD inverse in place (dense_inverse.cu); A is N x N, ld = N, symmetric positive definite
 cudaError_t dense_spd_inverse(double *A, int N, cudaStream_t stream);
 
+// ---- frame alignment of the distributed initialisation (dpgo_align.cu) ----
+// One aligning agent.  Its candidates are grouped per neighbour (group g = candidates [grp_ptr[g], grp_ptr[g+1]) against
+// agent grp_nbr[g], groups in increasing neighbour id); candidate q pairs local pose cand_local[q] with the gathered tile
+// cand_slot[q] through the shared edge cand_T[q] ((d+1) x (d+1) row-major), cand_out[q] != 0 when the agent owns its tail.
+struct AlignJob {
+  int ngroups;
+  int n;                                   // poses of the agent
+  const int *grp_nbr, *grp_ptr;
+  const int *cand_local, *cand_slot, *cand_out;
+  const double *cand_T;
+  const double *kappa;                     // per candidate rotation weight; nullptr = 1
+  double *cand_R, *cand_t, *w;             // candidate rotations (d x d row-major), translations (d; nullptr: none), weights
+  const double *Tloc;                      // d x (d+1)n local-frame trajectory, column-major
+  const double *ylift;                     // r x d, column-major
+  double *X;                               // r x (d+1)n resident iterate
+  double *T_align;                         // out: d x (d+1) column-major [R t]; nullptr in a lift job = identity
+  int *info;                               // out: neighbour used (-1: none), candidates, inliers, GNC iterations
+};
+constexpr int ALIGN_THREADS = 256;         // block of k_robust_rotation_average (one CTA per aligning agent)
+cudaError_t launch_align_candidates(int d, int r, int njobs, int max_cands, const AlignJob *jobs, const double *gathered,
+                                    cudaStream_t stream);
+cudaError_t launch_robust_rotation_average(int d, int njobs, const AlignJob *jobs, const int *ready, double cbar,
+                                           cudaStream_t stream);
+// X = YLift (T_align T) for every pose of every job whose info reports inliers (info == nullptr: always)
+cudaError_t launch_frame_lift(int d, int r, int njobs, int max_poses, const AlignJob *jobs, cudaStream_t stream);
+
 }  // namespace dpgo

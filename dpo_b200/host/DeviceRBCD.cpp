@@ -60,6 +60,13 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
   if (I.schedule != "greedy" && I.schedule != "coloured" && I.schedule != "parallel")
     throw std::runtime_error("DeviceRBCD: schedule must be greedy, coloured or parallel");
   if (I.K == 0 || n / I.K == 0) throw std::runtime_error("DeviceRBCD: more agents than poses");
+  const bool distributed = (opt.initialization == "distributed");
+  if (!distributed && opt.initialization != "central")
+    throw std::runtime_error("DeviceRBCD: initialization must be central or distributed");
+  if (distributed && XInit.size() != 0)
+    throw std::runtime_error("DeviceRBCD: the distributed initialisation computes the start itself: XInit must be empty");
+  if (!distributed && ((size_t)XInit.rows() != opt.r || (size_t)XInit.cols() != (graph[0].t.size() + 1) * n))
+    throw std::runtime_error("DeviceRBCD: XInit must be r x (d+1)n");
   if (I.K % I.N != 0) throw std::runtime_error("DeviceRBCD: the agents must divide evenly over the GPUs");
   int ndev = 0;
   check(dpgo_device_count(&ndev), "dpgo_device_count");
@@ -125,6 +132,24 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
       throw std::runtime_error("DeviceRBCD: concurrent rounds are implemented for the greedy and coloured schedules");
   }
 
+  // ---- distributed initialisation: every private graph must be connected, or its chordal initialisation is singular ----
+  if (distributed)
+    for (unsigned a = 0; a < K; ++a) {
+      std::vector<size_t> root(I.count[a]);
+      for (size_t q = 0; q < root.size(); ++q) root[q] = q;
+      auto find = [&](size_t q) { while (root[q] != q) q = root[q] = root[root[q]]; return q; };
+      size_t pieces = root.size();
+      for (const auto *set : {&odo[a], &priv[a]})
+        for (const auto &m : *set) {
+          const size_t x = find(m.p1), y = find(m.p2);
+          if (x != y) { root[x] = y; --pieces; }
+        }
+      if (pieces > 1)
+        throw std::runtime_error("DeviceRBCD: agent " + std::to_string(a) + ": the private pose graph (odometry + private loop "
+                                 "closures) has " + std::to_string(pieces) + " connected components, so its local chordal "
+                                 "initialisation is singular");
+    }
+
   // ---- streams, agents (Q on the agent's GPU), resident iterates ----
   I.stream.assign(I.N, nullptr);
   for (unsigned g = 0; g < I.N; ++g) check(dpgo_stream_create((int)g, &I.stream[g]), "dpgo_stream_create");
@@ -141,17 +166,42 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
     I.agents.emplace_back(new PGOAgent(a, prm));
     if (a == 0) I.agents[0]->getLiftingMatrix(lift);
     else I.agents[a]->setLiftingMatrix(lift);
-    // a zero trajectory of the right shape skips the agent's own chordal initialisation: X comes from XInit
+    // a zero trajectory of the right shape skips the agent's own host chordal initialisation: X comes from XInit, or from
+    // the GPU chordal initialisation and the alignment waves
     I.agents[a]->setPoseGraph(odo[a], priv[a], shared[a], Matrix::Zero(d, dh * I.count[a]));
-    Matrix Xa0(r, dh * I.count[a]);
-    for (size_t q = 0; q < I.count[a]; ++q) Xa0.block(0, q * dh, r, dh) = Matrix(XInit).block(0, I.globalOf[a][q] * dh, r, dh);
-    I.agents[a]->setX(Xa0);
     I.h[a] = I.agents[a]->problem()->handle();
     if (!I.h[a]) throw std::runtime_error("DeviceRBCD: agent without a device problem");
     check(dpgo_problem_set_stream(I.h[a], I.stream[(size_t)I.gpuOf[a]]), "dpgo_problem_set_stream");
-    Matrix Xa;
-    I.agents[a]->getX(Xa);
-    check(dpgo_problem_upload_X(I.h[a], Xa.data()), "dpgo_problem_upload_X");
+    if (!distributed) {
+      Matrix Xa0(r, dh * I.count[a]);
+      for (size_t q = 0; q < I.count[a]; ++q) Xa0.block(0, q * dh, r, dh) = Matrix(XInit).block(0, I.globalOf[a][q] * dh, r, dh);
+      I.agents[a]->setX(Xa0);
+      Matrix Xa;
+      I.agents[a]->getX(Xa);
+      check(dpgo_problem_upload_X(I.h[a], Xa.data()), "dpgo_problem_upload_X");
+      continue;
+    }
+    // ref localInitialization, src/PGOAgent.cpp:947-962: chordal initialisation of the private graph on the agent's GPU
+    const size_t na = I.count[a];
+    Matrix T = Matrix::Zero(d, dh * na);
+    for (unsigned k = 0; k < d; ++k) T(k, k) = 1.0;
+    if (na > 1) {
+      std::vector<int32_t> p1, p2;
+      std::vector<double> R, t, kap, tau;
+      for (const auto *set : {&odo[a], &priv[a]})
+        for (const auto &m : *set) {
+          p1.push_back((int32_t)m.p1); p2.push_back((int32_t)m.p2);
+          for (unsigned i = 0; i < d; ++i) {
+            for (unsigned j = 0; j < d; ++j) R.push_back(m.R(i, j));
+            t.push_back(m.t(i));
+          }
+          kap.push_back(m.weight * m.kappa); tau.push_back(m.weight * m.tau);
+        }
+      if (dpgo_chordal_initialization((int)na, (int)d, (int64_t)p1.size(), p1.data(), p2.data(), R.data(), t.data(), kap.data(),
+                                      tau.data(), I.gpuOf[a], 0.0, 0, T.data(), nullptr) != DPGO_OK)
+        throw std::runtime_error(std::string("dpgo_chordal_initialization: ") + dpgo_chordal_last_error());
+    }
+    check(dpgo_agent_set_local_trajectory(I.h[a], T.data(), lift.data()), "dpgo_agent_set_local_trajectory");
   }
 
   // ---- exchange plan: public poses, padded slots, per-agent edge tables ----
@@ -208,6 +258,39 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
     I.comm.assign(I.N, nullptr);
     checkNccl(ncclCommInitAll(I.comm.data(), (int)I.N, devs.data()), "ncclCommInitAll");
   }
+  if (distributed) {
+    // candidate tables (ref computeNeighborTransform / findSharedLoopClosureWithNeighbor, src/PGOAgent.cpp:250-288,922-934):
+    // one candidate per public pose (b, j) of a neighbour the agent shares an edge with, through the FIRST such edge,
+    // grouped per neighbour in increasing id, j increasing (std::map order)
+    for (unsigned a = 0; a < K; ++a) {
+      std::map<std::pair<unsigned, int32_t>, size_t> first;
+      for (size_t e = 0; e < shared[a].size(); ++e) {
+        const RelativeSEMeasurement &s = shared[a][e];
+        const bool out = (s.r1 == a);
+        first.emplace(std::make_pair((unsigned)(out ? s.r2 : s.r1), (int32_t)(out ? s.p2 : s.p1)), e);
+      }
+      std::vector<int32_t> grp, ptr, loc, slot, outg;
+      std::vector<double> T;
+      for (const auto &kv : first) {
+        const unsigned b = kv.first.first;
+        if (grp.empty() || grp.back() != (int32_t)b) { grp.push_back((int32_t)b); ptr.push_back((int32_t)loc.size()); }
+        const RelativeSEMeasurement &s = shared[a][kv.second];
+        const bool out = (s.r1 == a);
+        loc.push_back((int32_t)(out ? s.p1 : s.p2));
+        const auto it = std::lower_bound(pub[b].begin(), pub[b].end(), kv.first.second);
+        slot.push_back((int32_t)(b * I.pmax + (unsigned)(it - pub[b].begin())));
+        outg.push_back(out ? 1 : 0);
+        for (unsigned i = 0; i <= d; ++i)
+          for (unsigned j = 0; j <= d; ++j)
+            T.push_back(i < d ? (j < d ? s.R(i, j) : s.t(i)) : (j == d ? 1.0 : 0.0));
+      }
+      ptr.push_back((int32_t)loc.size());
+      check(dpgo_agent_set_align_candidates(I.h[a], (int)grp.size(), grp.data(), ptr.data(), loc.data(), slot.data(), outg.data(),
+                                            T.data()),
+            "dpgo_agent_set_align_candidates");
+    }
+    alignWaves();
+  }
   dpgo_opt_params_default(&I.prm);
   I.prm.algorithm = (opt.algorithm == ROPTALG::RTR) ? DPGO_ALG_RTR : DPGO_ALG_RGD;
   I.prm.precond = (int)opt.preconditioner;
@@ -228,6 +311,57 @@ DeviceRBCD::~DeviceRBCD() {
     if (I.N > 1 && I.send[g]) dpgo_device_free((int)g, I.send[g]);
     if (I.gathered[g]) dpgo_device_free((int)g, I.gathered[g]);
     if (I.stream[g]) dpgo_stream_destroy((int)g, I.stream[g]);
+  }
+}
+
+// Wave w >= 1 (ref src/PGOAgent.cpp:369-440, examples/MultiRobotExample.cpp:245-256): one exchange of the public tiles;
+// every agent that is not initialised and has a neighbour initialised before the wave tries those neighbours in increasing
+// id, all such agents of a GPU in one dpgo_agents_align_async call; the first neighbour with inliers wins.  At most K - 1
+// waves: a wave that initialises nobody is an error.
+void DeviceRBCD::alignWaves() {
+  Impl &I = *impl;
+  std::vector<int32_t> ready(I.K, 0);
+  ready[0] = 1;
+  mInitReport.assign(I.K, DeviceRBCDInitRecord());
+  mInitReport[0].wave = 0;
+  for (int wave = 1; std::find(ready.begin(), ready.end(), 0) != ready.end(); ++wave) {
+    exchange();
+    std::vector<unsigned> todo;
+    for (unsigned a = 0; a < I.K; ++a) {
+      if (ready[a]) continue;
+      for (unsigned b : I.neighbors[a])
+        if (ready[b]) { todo.push_back(a); break; }
+    }
+    for (unsigned g = 0; g < I.N; ++g) {
+      std::vector<dpgo_problem *> hs;
+      for (unsigned a : todo)
+        if ((unsigned)I.gpuOf[a] == g) hs.push_back(I.h[a]);
+      if (!hs.empty())
+        check(dpgo_agents_align_async(hs.data(), (int)hs.size(), I.gathered[g], (int64_t)I.K * I.pmax, ready.data(), (int)I.K,
+                                      I.stream[g]),
+              "dpgo_agents_align_async");
+    }
+    std::vector<unsigned> newly;
+    for (unsigned a : todo) {
+      int32_t info[4];
+      check(dpgo_agent_align_result(I.h[a], nullptr, info), "dpgo_agent_align_result");
+      DeviceRBCDInitRecord &rec = mInitReport[a];
+      rec.neighbor = info[0]; rec.candidates = info[1]; rec.inliers = info[2]; rec.iterations = info[3];
+      if (info[2] > 0) { rec.wave = wave; newly.push_back(a); }
+    }
+    if (newly.empty()) {
+      std::string rest;
+      for (unsigned a = 0; a < I.K; ++a)
+        if (!ready[a]) rest += (rest.empty() ? "" : ", ") + std::to_string(a);
+      throw std::runtime_error("DeviceRBCD: distributed initialisation: agents [" + rest + "] cannot join the global frame "
+                               "(no initialised neighbour gives a non-empty inlier set; is the agent graph connected?)");
+    }
+    for (unsigned a : newly) ready[a] = 1;
+  }
+  for (unsigned a = 0; a < I.K; ++a) {                 // the host copy of every agent's iterate, as setX leaves it
+    Matrix Xa(I.r, I.dh * I.count[a]);
+    check(dpgo_problem_download_X(I.h[a], Xa.data()), "dpgo_problem_download_X");
+    I.agents[a]->setX(Xa);
   }
 }
 

@@ -2,11 +2,13 @@
 //
 //   MultiAgentPGO <file.g2o> [--robots K] [--iters N] [--stop GRADNORM] [--accel] [--rgd] [--jacobi]
 //                 [--rank R] [--trace out.csv] [--resident [--gpus N] [--schedule greedy|coloured|parallel] [--bench ROUNDS]
-//                                                           [--partition FILE]]
+//                                                           [--partition FILE] [--init central|distributed]]
 //
 // --resident runs the device-resident multi-GPU runner (DPGO::DeviceRBCD): iterates stay in HBM, K agents over N GPUs
 // of this node, ONE ncclAllGather of the public poses per round; --bench times ROUNDS rounds without the central
-// evaluation.
+// evaluation.  --init distributed starts it from the reference's multi-robot initialisation (per-agent chordal
+// initialisation on the GPUs, then frame-alignment waves) instead of the centralised chordal relaxation, and prints one
+// "init <agent> <wave> <neighbour> <candidates> <inliers> <GNC iterations>" line per agent.
 //
 // Splits the pose graph into K contiguous agents, initialises every agent from the centralised chordal
 // relaxation lifted to rank R, then runs synchronous Riemannian block-coordinate descent with greedy agent
@@ -30,7 +32,7 @@ struct Options {
   double stop = 0.1;
   bool accel = false, rgd = false, jacobi = false, resident = false;
   unsigned gpus = 1, bench = 0;
-  std::string schedule = "greedy", partition;
+  std::string schedule = "greedy", partition, init = "central";
 };
 
 static Options parse(int argc, char **argv) {
@@ -51,6 +53,7 @@ static Options parse(int argc, char **argv) {
     else if (a == "--schedule") o.schedule = next();
     else if (a == "--bench") o.bench = (unsigned)std::stoul(next());
     else if (a == "--partition") o.partition = next();
+    else if (a == "--init") o.init = next();
     else if (a.rfind("--", 0) == 0) { std::cerr << "unknown option " << a << std::endl; std::exit(2); }
     else o.file = a;
   }
@@ -85,8 +88,14 @@ int main(int argc, char **argv) {
         if (!line.empty()) ro.owner.push_back((unsigned)std::stoul(line));
       if (ro.owner.size() != n) { std::cerr << "partition file: " << ro.owner.size() << " lines for " << n << " poses" << std::endl; return 1; }
     }
-    const Matrix lifted0 = fixedStiefelVariable(d, r) * chordalInitialization(d, n, graph);
+    ro.initialization = opt.init;
+    const Matrix lifted0 = (opt.init == "distributed") ? Matrix() : Matrix(fixedStiefelVariable(d, r) * chordalInitialization(d, n, graph));
     DeviceRBCD run(graph, n, K, lifted0, ro);
+    for (size_t a = 0; a < run.initReport().size(); ++a) {
+      const DeviceRBCDInitRecord &rec = run.initReport()[a];
+      std::cout << "init " << a << " " << rec.wave << " " << rec.neighbor << " " << rec.candidates << " " << rec.inliers << " "
+                << rec.iterations << std::endl;
+    }
     std::ofstream tr;
     if (!opt.trace.empty()) tr.open(opt.trace);
     const auto t0 = std::chrono::steady_clock::now();

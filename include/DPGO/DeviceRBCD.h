@@ -40,6 +40,17 @@ struct DeviceRBCDOptions {
   // the active agents of a round that share a GPU step side by side, each as one thread-block cluster on its own stream
   // (dpgo_agents_round_async; greedy / coloured schedules): -1 = when some GPU hosts >= 2 agents of one colour class
   int concurrent = -1;
+  // "central": the caller's XInit (r x (d+1)n); "distributed": the reference's multi-robot initialisation
+  // (PGOAgentParameters::multirobot_initialization, ref include/DPGO/PGOAgent.h:129) on the GPUs -- every agent's chordal
+  // initialisation of its private graph in its own frame, then frame-alignment waves (robust average of the frame
+  // transforms its shared loop closures give with an initialised neighbour, ref src/PGOAgent.cpp:369-440); XInit empty
+  std::string initialization = "central";
+};
+
+// per agent: the wave it joined the global frame in (agent 0: 0), the neighbour it aligned to (-1 for agent 0), the
+// candidate and inlier counts and the GNC iterations of that alignment
+struct DeviceRBCDInitRecord {
+  int wave = -1, neighbor = -1, candidates = 0, inliers = 0, iterations = 0;
 };
 
 struct DeviceRBCDStats {
@@ -50,7 +61,8 @@ struct DeviceRBCDStats {
 
 class DeviceRBCD {
  public:
-  // graph: the global pose graph (global pose ids); XInit: r x (d+1)n lifted initial iterate
+  // graph: the global pose graph (global pose ids); XInit: r x (d+1)n lifted initial iterate (empty with
+  // options.initialization == "distributed")
   DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n, unsigned numAgents, const Matrix &XInit,
              const DeviceRBCDOptions &options);
   ~DeviceRBCD();
@@ -67,10 +79,13 @@ class DeviceRBCD {
   const std::vector<unsigned> &colours() const { return mColour; }
   unsigned round() const { return mRound; }
   size_t allGatherBytesPerGpu() const;
+  const std::vector<DeviceRBCDInitRecord> &initReport() const { return mInitReport; }   // empty for "central"
 
  private:
   struct Impl;
   void roundConcurrent(const std::vector<unsigned> &active);
+  void alignWaves();
+  std::vector<DeviceRBCDInitRecord> mInitReport;
   std::unique_ptr<Impl> impl;
   unsigned mNumColours = 1, mRound = 0;
   std::vector<unsigned> mColour;

@@ -321,6 +321,36 @@ DPGO_API int dpgo_agents_host_io_async(dpgo_problem_t *const *agents, int count,
 /* per-agent Riemannian gradient norm / cost of the resident iterate (greedy selection input) */
 DPGO_API int dpgo_agent_f_rgradnorm_resident(dpgo_problem_t *p, double *f_out, double *norm_out);
 
+/* ---- distributed initialisation: every agent starts from the chordal initialisation of its private graph, in its own
+ *      frame, and joins the global frame through a robust average of the frame transforms its shared loop closures give
+ *      with an initialised neighbour.  ref: PGOAgent::initializeInGlobalFrame, src/PGOAgent.cpp:369-440 ------------- */
+/* ref PGOAgent::setPoseGraph, src/PGOAgent.cpp:182-185: the agent's local-frame trajectory T (d x (d+1)n column-major,
+ * [R_i t_i] per pose) and the lifting matrix YLift (r x d column-major) stay resident; X = YLift T (agent 0's start). */
+DPGO_API int dpgo_agent_set_local_trajectory(dpgo_problem_t *p, const double *T_host, const double *YLift_host);
+/* ref computeNeighborTransform / findSharedLoopClosureWithNeighbor, src/PGOAgent.cpp:250-288,922-934: the candidate table.
+ * Group g (neighbours in increasing id group_neighbor[g]) holds candidates [group_ptr[g], group_ptr[g+1]), one per public
+ * pose of that neighbour the agent shares an edge with, in increasing pose id.  Candidate q: local pose local_pose[q],
+ * the neighbour's tile nbr_slot[q] of the gathered buffer, the shared edge's T ((d+1) x (d+1) row-major) and
+ * outgoing[q] != 0 when the agent owns the edge tail. */
+DPGO_API int dpgo_agent_set_align_candidates(dpgo_problem_t *p, int num_groups, const int32_t *group_neighbor,
+                                             const int32_t *group_ptr, const int32_t *local_pose, const int32_t *nbr_slot,
+                                             const int32_t *outgoing, const double *T);
+/* ref updateNeighborPoses -> initializeInGlobalFrame -> computeRobustNeighborTransformTwoStage, src/PGOAgent.cpp:290-331,
+ * 369-440: one call per GPU and wave aligns `count` agents of one device against the gathered public tiles.  Per agent
+ * the groups whose neighbour has ready_host[neighbour] != 0 are tried in order (GNC-TLS rotation averaging at the
+ * threshold 2 sqrt(2) sin(0.25), ~30 degrees, then the mean translation of the inliers); the first with inliers moves
+ * the trajectory into the global frame: X = YLift (T_align T).  Asynchronous on `stream` (NULL: the first agent's). */
+DPGO_API int dpgo_agents_align_async(dpgo_problem_t *const *agents, int count, const double *gathered_dev, int64_t num_slots,
+                                     const int32_t *ready_host, int num_agents, void *stream);
+/* the agent's last alignment (waits for the stream of the align call that included the agent): T_align (d x (d+1) column-major, nullable) and info4 =
+ * {neighbour used (-1: no ready neighbour), candidates, inliers (0: not aligned), GNC iterations} */
+DPGO_API int dpgo_agent_align_result(dpgo_problem_t *p, double *T_align_host, int32_t *info4);
+/* ref robustSingleRotationAveraging, src/DPGO_utils.cpp:567-629: the same kernel on m host rotations R_host (m x d x d
+ * row-major), kappa_host (m, NULL = 1), GNC-TLS threshold `threshold` (chordal).  R_out: d x d row-major; inlier_flags
+ * (m, nullable); iterations (nullable): GNC iterations run (0: GNC skipped, every residual small).  Synchronous. */
+DPGO_API int dpgo_robust_single_rotation_averaging(int device, int d, int m, const double *R_host, const double *kappa_host,
+                                                   double threshold, double *R_out, int32_t *inlier_flags, int32_t *iterations);
+
 #ifdef __cplusplus
 }
 #endif

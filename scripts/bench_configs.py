@@ -8,6 +8,9 @@ synthetic grid / 8 agents) with k agents spread over N = WORLD_SIZE GPUs (k % N 
 Prints ONE JSON line on rank 0: rounds/s and agent-steps/s over --rounds timed rounds (CUDA events, max over
 ranks), then the convergence record of a fresh run to central gradient norm < --stop (rounds, wall time, final
 2f against the reference's f* where known).  Parity of the same paths is covered by tests/test_gpu_agents.py.
+--init distributed starts from the reference's multi-robot initialisation instead of one central chordal solve (per-agent
+chordal solves on each rank, then frame-alignment waves; tests/test_gpu_dist_init.py) and records its wall time, split into
+the local chordal solves and the waves (host clock after a device synchronise, rank 0), the waves and the inlier counts.
 """
 from __future__ import annotations
 
@@ -37,6 +40,9 @@ def main():
     ap.add_argument("--stop", type=float, default=0.1)
     ap.add_argument("--max-rounds", type=int, default=3000)
     ap.add_argument("--grid", default="100,100,10", help="synthetic grid dims when --dataset synthetic")
+    ap.add_argument("--init", default="central", choices=["central", "distributed"],
+                    help="start: one chordal solve of the whole graph (synthetic grid: perturbed ground truth), or the "
+                         "distributed initialisation from the measurements alone")
     ap.add_argument("--partition", default="blocks", choices=["blocks", "ranges"],
                     help="synthetic grid: kx*ky*kz lattice blocks (public poses only at the block faces) or the reference's "
                          "contiguous id ranges (1.25-layer slabs: every pose public)")
@@ -69,17 +75,18 @@ def main():
         owner = pg.grid_block_owner(*dims, args.agents) if args.partition == "blocks" else None
     else:
         edges, n = pg.read_g2o_file(os.path.join(ROOT, "data", args.dataset + ".g2o"))
-        T0 = pg.chordalInitialization(edges.d, n, edges)
+        T0 = pg.chordalInitialization(edges.d, n, edges) if args.init == "central" else None
         label = f"{args.dataset}.g2o = {n} poses / {len(edges)} edges"
         owner = None
     r = 5
-    X0 = pg.fixedStiefelVariable(edges.d, r) @ T0
+    X0 = pg.fixedStiefelVariable(edges.d, r) @ T0 if args.init == "central" else None
     precond = dp.PRECOND_SPARSE_EXACT if args.precond == "exact" else dp.PRECOND_BLOCK_JACOBI
     alg = dp.ROPTALG.RTR if args.alg == "rtr" else dp.ROPTALG.RGD
 
     def make():
         return DistributedPGO(edges, n, args.agents, r=r, algorithm=alg, preconditioner=precond, schedule=args.schedule,
-                              X_init=X0, rank=rank, world=world, device=local_rank, dist=dist, owner=owner)
+                              X_init=X0, rank=rank, world=world, device=local_rank, dist=dist, owner=owner,
+                              initialization=args.init)
 
     def barrier():
         if world > 1:
@@ -135,6 +142,12 @@ def main():
                                "final_cost_2f": st.cost if st else None, "final_gradnorm": st.gradnorm if st else None,
                                "fstar_reference": FSTAR.get(args.dataset)},
                "trace_head": hist[:5], "trace_tail": hist[-3:]}
+        if args.init == "distributed":
+            rep = run.init_report
+            out["init"] = {"mode": "distributed", **run.init_times, "waves": max(a["wave"] for a in rep),
+                           "per_agent": [[a["wave"], a["neighbor"], a["candidates"], a["inliers"], a["iterations"]]
+                                         for a in rep],
+                           "per_agent_fields": ["wave", "neighbor", "candidates", "inliers", "gnc_iterations"]}
         print(json.dumps(out))
     if world > 1:
         dist.destroy_process_group()
