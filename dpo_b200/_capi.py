@@ -14,6 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libdpgo_b200.so")
 
 OK = 0
+STATUS_DOUBLES = 5            # DPGO_STATUS_DOUBLES: quad, lin, |rgrad|^2, relative change, optimising calls
 ALG_RTR, ALG_RGD = 0, 1
 PRECOND_NONE, PRECOND_BLOCK_JACOBI, PRECOND_DENSE_EXACT, PRECOND_SPARSE_EXACT = 0, 1, 2, 3
 TCG_NAMES = {0: "NEGCURVTURE", 1: "EXCREGION", 2: "LCON", 3: "SCON", 4: "MAXITER", -1: "NOT_RUN"}
@@ -129,6 +130,11 @@ SIGNATURES = {
     "dpgo_agents_align_async": (C.c_int, [C.POINTER(_vp), C.c_int, _vp, C.c_int64, _ip, C.c_int, _vp]),
     "dpgo_agent_align_result": (C.c_int, [_vp, _dp, _ip]),
     "dpgo_robust_single_rotation_averaging": (C.c_int, [C.c_int, C.c_int, C.c_int, _dp, _dp, C.c_double, _dp, _ip, _ip]),
+    "dpgo_agents_status_async": (C.c_int, [C.POINTER(_vp), C.c_int, _ip, _vp, _vp]),
+    "dpgo_agent_trajectory_global": (C.c_int, [_vp, _dp, _dp]),
+    "dpgo_host_alloc_pinned": (C.c_int, [C.c_size_t, C.POINTER(_vp)]),
+    "dpgo_host_free_pinned": (C.c_int, [_vp]),
+    "dpgo_copy_to_host_async": (C.c_int, [C.c_int, _vp, _vp, C.c_size_t, _vp]),
 }
 
 _lib = None

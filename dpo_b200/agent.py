@@ -461,6 +461,60 @@ class RoundStats:
     selected: List[int]
 
 
+@dataclass
+class TeamStatus:
+    records: np.ndarray    # (k, capi.STATUS_DOUBLES): <XQ,X>, <X,G>, |rgrad|^2, last relative change, optimising calls
+    cost: float            # 2 f_central = sum(<XQ,X> + <X,G>)
+    gradnorm: float        # |grad_central|
+
+
+@dataclass
+class SolveReport:
+    rounds: int
+    reason: str            # "gradnorm", "team" or "max_rounds"
+    cost: float
+    gradnorm: float
+    relative_change: np.ndarray    # per agent, of its last optimising call
+
+
+def team_status(records: np.ndarray) -> TeamStatus:
+    records = np.asarray(records, dtype=np.float64)
+    return TeamStatus(records, float(np.sum(records[:, 0] + records[:, 1])), float(np.sqrt(np.sum(records[:, 2]))))
+
+
+def stop_reason(records: np.ndarray, calls_at_start: np.ndarray, rounds: int, max_rounds: int, gradnorm_tol: float,
+                rel_change_tol: float) -> Optional[str]:
+    """Stop rule of DistributedPGO.solve / DeviceRBCD::solve as a function of the team's status records: the central
+    gradient norm below gradnorm_tol (ref examples/MultiRobotExample.cpp:302-305); every agent ready to terminate, i.e.
+    optimised since the solve began with its last relative change <= rel_change_tol (ref PGOAgent::shouldTerminate,
+    src/PGOAgent.cpp:703-716,1007-1031); the round cap.  A tolerance of 0 disables its rule."""
+    st = team_status(records)
+    if gradnorm_tol > 0 and st.gradnorm < gradnorm_tol:
+        return "gradnorm"
+    if rel_change_tol > 0 and np.all(st.records[:, 4] > np.asarray(calls_at_start)) and \
+            np.all(st.records[:, 3] <= rel_change_tol):
+        return "team"
+    if rounds >= max_rounds:
+        return "max_rounds"
+    return None
+
+
+def greedy_selection(selected: int, agent_gradnorms: np.ndarray, has_neighbours: bool) -> int:
+    """The next agent of the greedy schedule (ref examples/MultiRobotExample.cpp:308-325): the largest per-agent gradient
+    norm, except that an agent without neighbours stays selected."""
+    return int(np.argmax(agent_gradnorms)) if has_neighbours else int(selected)
+
+
+def check_solve_arguments(schedule: str, acceleration: bool, max_rounds: int, check_every: int) -> None:
+    if acceleration:
+        raise ValueError("solve() does not support acceleration=True: the accelerated iterate's relative change is "
+                         "measured against the Nesterov step's XPrev; drive it with step()")
+    if max_rounds < 1 or check_every < 1:
+        raise ValueError("max_rounds and check_every must be >= 1")
+    if schedule == "greedy" and check_every != 1:
+        raise ValueError("the greedy schedule selects the next agent from every round's status: check_every must be 1")
+
+
 def auto_concurrent(colour: Sequence[int], k: int, world: int, schedule: str, acceleration: bool) -> bool:
     """Default launch mode of a k-agent run over `world` ranks (contiguous blocks of k/world agents per rank): the agents of
     a round step side by side (thread-block clusters, dpgo_agents_round_async) when some rank hosts >= 2 agents of one
@@ -936,3 +990,120 @@ class DistributedPGO:
             cols = (self.glob[a][:, None] * dh + np.arange(dh)[None, :]).ravel()
             X[:, cols] = self.agents[a].mProblem.download_X()
         return X
+
+    # -- running to convergence: team status, stop rule, trajectory -------------------------------------------------
+    def status(self) -> TeamStatus:
+        """Every agent's status record (capi.STATUS_DOUBLES each) with the central 2f and |grad|: one exchange (skipped
+        when the gathered tiles are already current), one status launch for the agents of this GPU, one copy to the host
+        (distributed: one all-gather of the records first).  All of it is ordered on the runner's stream, whichever torch
+        stream is current."""
+        with self.torch.cuda.stream(self._runner_stream()):
+            return self._status()
+
+    def _runner_stream(self):
+        """The torch stream the runner's work is issued on (the current stream when it was built)."""
+        if not hasattr(self, "_torch_stream"):
+            torch = self.torch
+            self._torch_stream = torch.cuda.default_stream(self.dev) if self._main_stream == 1 else \
+                torch.cuda.ExternalStream(self._main_stream, device=self.dev)
+        return self._torch_stream
+
+    def _refresh_G(self) -> None:
+        """Every local agent's G from the current public tiles: one exchange, or only the G rebuild when the gathered tiles
+        are current (concurrent rounds keep them so)."""
+        if self.concurrent and self._gathered_current:
+            for a in self.local_ids:
+                self.agents[a].build_G(self.gathered.data_ptr(), self.k * self.plan.pmax)
+        else:
+            self.exchange()
+            if self.concurrent:
+                self._gathered_current = True
+
+    def _status(self) -> TeamStatus:
+        self._refresh_G()
+        torch, S = self.torch, capi.STATUS_DOUBLES
+        if not hasattr(self, "_status_local"):
+            self._status_local = torch.zeros(S * len(self.local_ids), dtype=torch.float64, device=self.dev)
+            self._status_all = torch.zeros(S * self.k, dtype=torch.float64, device=self.dev) if self.distributed \
+                else self._status_local
+            self._status_handles = (C.c_void_p * len(self.local_ids))(*[self.agents[a].mProblem._h for a in self.local_ids])
+            self._status_slots = np.arange(len(self.local_ids), dtype=np.int32)      # agent order within the rank
+        lib = self.agents[self.local_ids[0]].mProblem._lib
+        capi.check(lib.dpgo_agents_status_async(self._status_handles, len(self.local_ids), capi.iptr(self._status_slots),
+                                                C.c_void_p(self._status_local.data_ptr()), C.c_void_p(self._main_stream)))
+        if self.distributed:
+            self.dist.all_gather_into_tensor(self._status_all, self._status_local)
+        return team_status(self._status_all.cpu().numpy().reshape(self.k, S))
+
+    def _solve_round(self, fresh: bool) -> None:
+        """One round without evaluation, as step(evaluate=False) issues it; fresh: every agent's G was built from the
+        current tiles by the status just taken, so the round does not repeat that exchange."""
+        active = self._active()
+        if self.concurrent:
+            if not self._gathered_current:
+                self.exchange(build=False)
+                self._gathered_current = True
+            self._round_concurrent(active)
+        else:
+            if not fresh:
+                self.exchange()
+            for a in self.local_ids:
+                if a in active:
+                    self.agents[a].opt.optimize_resident_async()
+        for a in self.local_ids:
+            if a in active:
+                self.agents[a].mIterationNumber += 1
+        self.round += 1
+
+    def solve(self, max_rounds: int = 500, gradnorm_tol: float = 0.1, rel_change_tol: float = 5e-3, check_every: int = 1,
+              callback=None) -> SolveReport:
+        """Run rounds until the stop rule holds (see stop_reason): the status is taken after every check_every-th round
+        and after the last one; the rounds in between are issued without a host synchronisation.  callback(round, cost,
+        gradnorm) sees every check.  The greedy schedule selects the next agent from each round's status, as step() does,
+        so it needs check_every = 1."""
+        check_solve_arguments(self.schedule, self.acceleration, max_rounds, check_every)
+        with self.torch.cuda.stream(self._runner_stream()):
+            return self._solve(max_rounds, gradnorm_tol, rel_change_tol, check_every, callback)
+
+    def _solve(self, max_rounds, gradnorm_tol, rel_change_tol, check_every, callback) -> SolveReport:
+        calls_at_start = self.status().records[:, 4].copy()
+        rounds, fresh = 0, True
+        while True:
+            self._solve_round(fresh)
+            rounds += 1
+            fresh = False
+            if rounds % check_every != 0 and rounds < max_rounds:
+                continue
+            st = self.status()
+            fresh = True
+            if callback is not None:
+                callback(rounds, st.cost, st.gradnorm)
+            if self.schedule == "greedy":
+                cur = self.selected[0]
+                self.selected = [greedy_selection(cur, np.sqrt(st.records[:, 2]), bool(self.plan.tables[cur]["neighbors"]))]
+            reason = stop_reason(st.records, calls_at_start, rounds, max_rounds, gradnorm_tol, rel_change_tol)
+            if reason is not None:
+                return SolveReport(rounds, reason, st.cost, st.gradnorm, st.records[:, 3].copy())
+
+    def trajectory(self) -> np.ndarray:
+        """The d x (d+1)n trajectory in global pose order, rounded on the device (ref getTrajectoryInGlobalFrame,
+        src/PGOAgent.cpp:500-519) against agent 0's local pose 0 (ref examples/MultiRobotExample.cpp:328-333).
+        Distributed: the anchor is broadcast from agent 0's rank and only this rank's columns are filled."""
+        d, dh, r = self.d, self.d + 1, self.r
+        anchor = np.zeros((r, dh), order="F")
+        if 0 in self.agents:
+            anchor[...] = self.agents[0].mProblem.download_X()[:, :dh]
+        if self.distributed:
+            torch = self.torch
+            with torch.cuda.stream(self._runner_stream()):
+                buf = torch.from_numpy(anchor.ravel(order="F")).to(self.dev)
+                self.dist.broadcast(buf, src=0)
+                anchor = np.asfortranarray(buf.cpu().numpy().reshape(r, dh, order="F"))
+        T = np.zeros((d, dh * self.n))
+        for a in self.local_ids:
+            ag = self.agents[a]
+            out = np.zeros((d, dh * ag.n), order="F")
+            capi.check(ag.mProblem._lib.dpgo_agent_trajectory_global(ag.mProblem._h, capi.dptr(anchor), capi.dptr(out)))
+            cols = (self.glob[a][:, None] * dh + np.arange(dh)[None, :]).ravel()
+            T[:, cols] = out
+        return T

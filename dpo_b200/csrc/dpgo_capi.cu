@@ -113,6 +113,12 @@ struct dpgo_problem {
   int *d_ready = nullptr;
   int jobs_cap = 0, ready_cap = 0;
   cudaEvent_t ev_align = nullptr;          // recorded on the stream of the last dpgo_agents_align_async that aligned this agent
+  // team status (dpgo_status.cu): last optimising call's relative change + count, per-CTA partials, ticket of the last CTA
+  double *d_opt_record = nullptr, *d_status_part = nullptr;
+  unsigned *d_status_ticket = nullptr;
+  struct StatusTable { std::vector<uint64_t> key; dpgo::StatusJob *d_jobs = nullptr; int ctas = 0; };
+  std::vector<StatusTable> status_tables;  // job tables of dpgo_agents_status_async, kept by the call's first agent
+  double *d_anchor = nullptr, *d_traj = nullptr;   // dpgo_agent_trajectory_global
 
   size_t vec_bytes() const { return sizeof(double) * (size_t)r * (size_t)N; }
 };
@@ -154,6 +160,7 @@ void fill_kparams(const dpgo_problem *p, dpgo::KParams &kp, int op, const dpgo_o
   kp.cluster = p->cluster ? 1 : 0;
   kp.smem_doubles = 0;
   kp.phase_ns = p->d_phase_ns;
+  kp.opt_record = p->d_opt_record;
   kp.prm = prm;
   kp.result = p->d_result;
 }
@@ -677,6 +684,12 @@ int dpgo_problem_create(int n, int d, int r, int device, dpgo_problem_t **out) {
   if (cudaMalloc(&p->d_bar, 2 * sizeof(unsigned)) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed");
   cudaMemsetAsync(p->d_bar, 0, 2 * sizeof(unsigned), p->stream);
   if (cudaMalloc(&p->d_result, sizeof(dpgo_opt_result_t)) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed");
+  if (cudaMalloc(&p->d_opt_record, 2 * sizeof(double)) != cudaSuccess ||
+      cudaMalloc(&p->d_status_part, sizeof(double) * 3 * (size_t)dpgo::status_ctas(n)) != cudaSuccess ||
+      cudaMalloc(&p->d_status_ticket, sizeof(unsigned)) != cudaSuccess)
+    return bail(DPGO_ERR_ALLOC, "device allocation failed (status)");
+  cudaMemsetAsync(p->d_opt_record, 0, 2 * sizeof(double), p->stream);
+  cudaMemsetAsync(p->d_status_ticket, 0, sizeof(unsigned), p->stream);
   if (cudaMallocHost(&p->h_result, sizeof(dpgo_opt_result_t)) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "pinned allocation failed");
   if (cudaStreamSynchronize(p->stream) != cudaSuccess) return bail(DPGO_ERR_CUDA, "device initialisation failed");
   // empty Q (ref: ctor calls setQ(SparseMatrix(N,N)), src/QuadraticProblem.cpp:23)
@@ -704,6 +717,8 @@ int dpgo_problem_destroy(dpgo_problem_t *p) {
   free_dev(p->d_Tloc); free_dev(p->d_ylift); free_dev(p->d_grp_nbr); free_dev(p->d_grp_ptr); free_dev(p->d_cand_local);
   free_dev(p->d_cand_slot); free_dev(p->d_cand_out); free_dev(p->d_cand_T); free_dev(p->d_cand_R); free_dev(p->d_cand_t);
   free_dev(p->d_cand_w); free_dev(p->d_T_align); free_dev(p->d_align_info); free_dev(p->d_jobs); free_dev(p->d_ready);
+  free_dev(p->d_opt_record); free_dev(p->d_status_part); free_dev(p->d_status_ticket); free_dev(p->d_anchor); free_dev(p->d_traj);
+  for (auto &t : p->status_tables) free_dev(t.d_jobs);
   free_nd(p);
   if (p->h_result) cudaFreeHost(p->h_result);
   for (auto &g : p->round_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
@@ -1908,6 +1923,119 @@ int dpgo_robust_single_rotation_averaging(int device, int d, int m, const double
   if (inlier_flags)
     for (int q = 0; q < m; ++q) inlier_flags[q] = w[(size_t)q] > 1.0 - 1e-8 ? 1 : 0;
   if (iterations) *iterations = info[3];
+  return DPGO_OK;
+}
+
+}  // extern "C"
+
+// ---- team status and rounding (dpgo_status.cu) ---------------------------------------------------------------------------
+namespace {
+int require_device() {
+  int count = 0;
+  if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
+    cudaGetLastError();
+    return fail(DPGO_ERR_NO_DEVICE, "no CUDA device available: the GPU path has no CPU fallback");
+  }
+  return DPGO_OK;
+}
+constexpr size_t STATUS_TABLES_MAX = 32;
+}  // namespace
+
+extern "C" {
+
+int dpgo_agents_status_async(dpgo_problem_t *const *agents, int count, const int32_t *slot, double *status_dev, void *stream) {
+  DPGO_TRY(require_device());
+  DPGO_REQUIRE(agents && slot && status_dev, DPGO_ERR_INVALID_ARG, "null agents, slots or status buffer");
+  DPGO_REQUIRE(count > 0, DPGO_ERR_INVALID_ARG, "count must be positive");
+  dpgo_problem *lead = agents[0];
+  DPGO_REQUIRE(lead, DPGO_ERR_INVALID_ARG, "null problem handle");
+  std::vector<int32_t> sorted(slot, slot + count);
+  std::sort(sorted.begin(), sorted.end());
+  DPGO_REQUIRE(sorted[0] >= 0, DPGO_ERR_INVALID_ARG, "negative status slot");
+  DPGO_REQUIRE(std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end(), DPGO_ERR_INVALID_ARG, "duplicate status slot");
+  std::vector<uint64_t> key;
+  key.reserve(3 * (size_t)count + 1);
+  for (int i = 0; i < count; ++i) {
+    const dpgo_problem *p = agents[i];
+    DPGO_REQUIRE(p, DPGO_ERR_INVALID_ARG, "null problem handle");
+    DPGO_REQUIRE(p->device == lead->device && p->d == lead->d && p->r == lead->r, DPGO_ERR_INVALID_ARG,
+                 "the agents of one status call must share the device, d and r");
+    key.push_back((uint64_t)(uintptr_t)p);
+    key.push_back(p->generation);
+    key.push_back((uint64_t)slot[i]);
+  }
+  key.push_back((uint64_t)(uintptr_t)status_dev);
+  DPGO_CUDA(cudaSetDevice(lead->device));
+  cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
+  // The job table of an agent list is uploaded once (stream-ordered) and kept; a repeated call is one kernel launch
+  // and nothing else, so it can be captured into a CUDA graph.
+  dpgo_problem::StatusTable *tab = nullptr;
+  for (auto &t : lead->status_tables)
+    if (t.key == key) { tab = &t; break; }
+  if (!tab) {
+    if (lead->status_tables.size() >= STATUS_TABLES_MAX) {     // a table may still be read by a launch in flight
+      DPGO_CUDA(cudaDeviceSynchronize());
+      free_dev(lead->status_tables.front().d_jobs);
+      lead->status_tables.erase(lead->status_tables.begin());
+    }
+    std::vector<dpgo::StatusJob> jobs((size_t)count);
+    int ctas = 0;
+    for (int i = 0; i < count; ++i) {
+      const dpgo_problem *p = agents[i];
+      dpgo::StatusJob &J = jobs[(size_t)i];
+      J.n = p->n;
+      J.cta0 = ctas;
+      J.rowptr = p->d_rowptr; J.bcol = p->d_bcol; J.bval = p->d_bval;
+      J.X = p->d_vec[dpgo::V_X0]; J.G = p->d_G;
+      J.opt_record = p->d_opt_record;
+      J.partials = p->d_status_part;
+      J.ticket = p->d_status_ticket;
+      J.out = status_dev + (size_t)slot[i] * DPGO_STATUS_DOUBLES;
+      ctas += dpgo::status_ctas(p->n);
+    }
+    dpgo::StatusJob *d_jobs = nullptr;
+    DPGO_CUDA(cudaMalloc(&d_jobs, sizeof(dpgo::StatusJob) * (size_t)count));
+    DPGO_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(dpgo::StatusJob) * (size_t)count, cudaMemcpyHostToDevice, st));
+    lead->status_tables.emplace_back();
+    tab = &lead->status_tables.back();
+    tab->key = key;
+    tab->d_jobs = d_jobs;
+    tab->ctas = ctas;
+  }
+  DPGO_CUDA(dpgo::launch_agents_status(lead->r, lead->dh, count, tab->ctas, tab->d_jobs, st));
+  return DPGO_OK;
+}
+
+int dpgo_agent_trajectory_global(dpgo_problem_t *p, const double *anchor_host, double *T_host) {
+  DPGO_TRY(require_device());
+  DPGO_REQUIRE(anchor_host && T_host, DPGO_ERR_INVALID_ARG, "null anchor or trajectory");
+  DPGO_CHECK_HANDLE(p);
+  if (!p->d_anchor) DPGO_CUDA(cudaMalloc(&p->d_anchor, sizeof(double) * p->ts));
+  if (!p->d_traj) DPGO_CUDA(cudaMalloc(&p->d_traj, sizeof(double) * (size_t)p->d * p->N));
+  DPGO_CUDA(cudaMemcpyAsync(p->d_anchor, anchor_host, sizeof(double) * p->ts, cudaMemcpyHostToDevice, p->stream));
+  DPGO_CUDA(dpgo::launch_trajectory_global(p->r, p->dh, p->n, p->d_anchor, p->d_vec[dpgo::V_X0], p->d_traj, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(T_host, p->d_traj, sizeof(double) * (size_t)p->d * p->N, cudaMemcpyDeviceToHost, p->stream));
+  DPGO_CUDA(cudaStreamSynchronize(p->stream));
+  return DPGO_OK;
+}
+
+int dpgo_host_alloc_pinned(size_t bytes, void **ptr) {
+  DPGO_TRY(require_device());
+  DPGO_REQUIRE(ptr && bytes > 0, DPGO_ERR_INVALID_ARG, "null output or zero size");
+  DPGO_CUDA(cudaMallocHost(ptr, bytes));
+  return DPGO_OK;
+}
+
+int dpgo_host_free_pinned(void *ptr) {
+  if (ptr) DPGO_CUDA(cudaFreeHost(ptr));
+  return DPGO_OK;
+}
+
+int dpgo_copy_to_host_async(int device, void *dst_host, const void *src_dev, size_t bytes, void *stream) {
+  DPGO_TRY(require_device());
+  DPGO_REQUIRE(dst_host && src_dev, DPGO_ERR_INVALID_ARG, "null buffer");
+  DPGO_CUDA(cudaSetDevice(device));
+  DPGO_CUDA(cudaMemcpyAsync(dst_host, src_dev, bytes, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   return DPGO_OK;
 }
 

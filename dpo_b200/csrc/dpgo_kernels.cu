@@ -1312,7 +1312,12 @@ template <int R, int DH> __global__ void __launch_bounds__(OPT_THREADS, 1) k_opt
   tick(6);
   res.relative_change = sqrt(acc[0] / (double)kp.n);
   res.success = 1;
-  if (blockIdx.x == 0 && threadIdx.x == 0) { *kp.result = res; *kp.bar_epoch = bc.epoch; }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    *kp.result = res;
+    *kp.bar_epoch = bc.epoch;
+    // the team status reads the relative change from here: the result record is overwritten by every OP_EVAL
+    if (kp.opt_record) { kp.opt_record[0] = res.relative_change; kp.opt_record[1] += 1.0; }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1643,25 +1648,6 @@ template <int R, int DH> static int max_grid_t(int device) {
   if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
   return per_sm > 0 ? sms : 0;      // one CTA per SM
 }
-
-#define DPGO_DISPATCH(R_, DH_, ...)                                    \
-  do {                                                                   \
-    if ((DH_) == 4) {                                                    \
-      switch (R_) {                                                      \
-        case 3: { constexpr int R = 3, DH = 4; __VA_ARGS__; } break;     \
-        case 4: { constexpr int R = 4, DH = 4; __VA_ARGS__; } break;     \
-        case 5: { constexpr int R = 5, DH = 4; __VA_ARGS__; } break;     \
-        default: break;                                                  \
-      }                                                                  \
-    } else if ((DH_) == 3) {                                             \
-      switch (R_) {                                                      \
-        case 2: { constexpr int R = 2, DH = 3; __VA_ARGS__; } break;     \
-        case 3: { constexpr int R = 3, DH = 3; __VA_ARGS__; } break;     \
-        case 5: { constexpr int R = 5, DH = 3; __VA_ARGS__; } break;     \
-        default: break;                                                  \
-      }                                                                  \
-    }                                                                    \
-  } while (0)
 
 cudaError_t launch_optimize(int r, int dh, const KParams &kp, cudaStream_t stream) {
   cudaError_t e = cudaErrorInvalidValue;

@@ -92,7 +92,28 @@ struct KParams {
   int strict_acquire;    // 1: the grid barrier polls with ld.acquire (L1 invalidated every phase); 0: relaxed poll (default)
   int smem_doubles;      // dynamic shared memory of this launch, in doubles
   unsigned long long *phase_ns; // diagnostic (nullable): per phase kind, ns seen by CTA 0 (dpgo_debug_phase_times)
+  double *opt_record;    // 2 doubles: relative change of the last optimising call, optimising calls so far (OP_OPTIMIZE only)
 };
+
+// Instantiations of the compiled (r, d+1) pairs (every pair dpgo_problem_create accepts); R and DH are constexpr in the body.
+#define DPGO_DISPATCH(R_, DH_, ...)                                    \
+  do {                                                                   \
+    if ((DH_) == 4) {                                                    \
+      switch (R_) {                                                      \
+        case 3: { constexpr int R = 3, DH = 4; __VA_ARGS__; } break;     \
+        case 4: { constexpr int R = 4, DH = 4; __VA_ARGS__; } break;     \
+        case 5: { constexpr int R = 5, DH = 4; __VA_ARGS__; } break;     \
+        default: break;                                                  \
+      }                                                                  \
+    } else if ((DH_) == 3) {                                             \
+      switch (R_) {                                                      \
+        case 2: { constexpr int R = 2, DH = 3; __VA_ARGS__; } break;     \
+        case 3: { constexpr int R = 3, DH = 3; __VA_ARGS__; } break;     \
+        case 5: { constexpr int R = 5, DH = 3; __VA_ARGS__; } break;     \
+        default: break;                                                  \
+      }                                                                  \
+    }                                                                    \
+  } while (0)
 
 // launchers (dpgo_kernels.cu)
 cudaError_t launch_optimize(int r, int dh, const KParams &kp, cudaStream_t stream);
@@ -148,5 +169,23 @@ cudaError_t launch_robust_rotation_average(int d, int njobs, const AlignJob *job
                                            cudaStream_t stream);
 // X = YLift (T_align T) for every pose of every job whose info reports inliers (info == nullptr: always)
 cudaError_t launch_frame_lift(int d, int r, int njobs, int max_poses, const AlignJob *jobs, cudaStream_t stream);
+
+// ---- team status and rounding (dpgo_status.cu) ----
+// One agent of a status launch: CTAs [cta0, cta0 + status_ctas(n)) own STATUS_ROWS consecutive rows of its block-CSR Q each.
+struct StatusJob {
+  int n, cta0;
+  const int *rowptr, *bcol;
+  const double *bval, *X, *G;
+  const double *opt_record;                // KParams::opt_record of the agent
+  double *partials;                        // status_ctas(n) x 3 per-CTA partial sums
+  unsigned *ticket;                        // CTAs of the agent done in this launch (the last one resets it to 0)
+  double *out;                             // DPGO_STATUS_DOUBLES
+};
+constexpr int STATUS_THREADS = 256;
+constexpr int STATUS_ROWS = 32;
+__host__ __device__ inline int status_ctas(int n) { return (n + STATUS_ROWS - 1) / STATUS_ROWS; }
+cudaError_t launch_agents_status(int r, int dh, int njobs, int total_ctas, const StatusJob *jobs, cudaStream_t stream);
+// T = [proj_SO(d)(Ya^T X_i R-block), Ya^T X_i t - Ya^T pa] per pose (d x (d+1)n column-major); anchor = [Ya pa], r x (d+1)
+cudaError_t launch_trajectory_global(int r, int dh, int n, const double *anchor, const double *X, double *T, cudaStream_t stream);
 
 }  // namespace dpgo

@@ -42,6 +42,8 @@ struct DeviceRBCD::Impl {
   unsigned selected = 0;
   bool concurrent = false;         // active agents of a GPU side by side (cluster launches, own streams)
   bool gatheredCurrent = false;    // concurrent mode: the gathered buffers hold every agent's current public tiles
+  std::vector<double *> statusDev; // per GPU: its agents' status records
+  double *statusHost = nullptr;    // pinned, all agents' records in agent order
 };
 
 DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n, unsigned numAgents, const Matrix &XInit,
@@ -310,8 +312,10 @@ DeviceRBCD::~DeviceRBCD() {
   for (unsigned g = 0; g < I.N; ++g) {
     if (I.N > 1 && I.send[g]) dpgo_device_free((int)g, I.send[g]);
     if (I.gathered[g]) dpgo_device_free((int)g, I.gathered[g]);
+    if (g < I.statusDev.size() && I.statusDev[g]) dpgo_device_free((int)g, I.statusDev[g]);
     if (I.stream[g]) dpgo_stream_destroy((int)g, I.stream[g]);
   }
+  dpgo_host_free_pinned(I.statusHost);
 }
 
 // Wave w >= 1 (ref src/PGOAgent.cpp:369-440, examples/MultiRobotExample.cpp:245-256): one exchange of the public tiles;
@@ -489,6 +493,119 @@ Matrix DeviceRBCD::assemble() {
     for (size_t q = 0; q < I.count[a]; ++q) X.block(0, I.globalOf[a][q] * I.dh, I.r, I.dh) = Xa.block(0, q * I.dh, I.r, I.dh);
   }
   return X;
+}
+
+// ---- running to convergence -------------------------------------------------------------------------------------------
+DeviceRBCDStatus DeviceRBCD::status() {
+  Impl &I = *impl;
+  constexpr unsigned S = DPGO_STATUS_DOUBLES;
+  if (I.concurrent && I.gatheredCurrent) {
+    for (unsigned a = 0; a < I.K; ++a)
+      check(dpgo_agent_build_G(I.h[a], I.gathered[(size_t)I.gpuOf[a]], (int64_t)I.K * I.pmax), "dpgo_agent_build_G");
+  } else {
+    exchange();
+    if (I.concurrent) I.gatheredCurrent = true;
+  }
+  if (I.statusDev.empty()) {
+    I.statusDev.assign(I.N, nullptr);
+    for (unsigned g = 0; g < I.N; ++g) {
+      void *p = nullptr;
+      check(dpgo_device_malloc((int)g, sizeof(double) * S * I.perGpu, &p), "dpgo_device_malloc");
+      I.statusDev[g] = static_cast<double *>(p);
+    }
+    void *hp = nullptr;
+    check(dpgo_host_alloc_pinned(sizeof(double) * S * I.K, &hp), "dpgo_host_alloc_pinned");
+    I.statusHost = static_cast<double *>(hp);
+  }
+  std::vector<int32_t> slots(I.perGpu);
+  for (unsigned i = 0; i < I.perGpu; ++i) slots[i] = (int32_t)i;
+  for (unsigned g = 0; g < I.N; ++g) {                  // a GPU hosts the contiguous block of agents g * perGpu ...
+    std::vector<dpgo_problem *> hs(I.h.begin() + (size_t)g * I.perGpu, I.h.begin() + (size_t)(g + 1) * I.perGpu);
+    check(dpgo_agents_status_async(hs.data(), (int)hs.size(), slots.data(), I.statusDev[g], I.stream[g]),
+          "dpgo_agents_status_async");
+    check(dpgo_copy_to_host_async((int)g, I.statusHost + (size_t)g * I.perGpu * S, I.statusDev[g], sizeof(double) * S * I.perGpu,
+                                  I.stream[g]),
+          "dpgo_copy_to_host_async");
+  }
+  sync();
+  DeviceRBCDStatus st;
+  st.records.assign(I.statusHost, I.statusHost + (size_t)S * I.K);
+  double gn2 = 0;
+  for (unsigned a = 0; a < I.K; ++a) {
+    st.cost += st.at(a, 0) + st.at(a, 1);
+    gn2 += st.at(a, 2);
+  }
+  st.gradnorm = std::sqrt(gn2);
+  return st;
+}
+
+// one round without evaluation, as runRounds issues it; fresh: the status just taken built every agent's G from the
+// current tiles, so the round does not repeat that exchange
+void DeviceRBCD::solveRound(bool fresh) {
+  Impl &I = *impl;
+  const std::vector<unsigned> act = activeSet(I.schedule, I.K, I.selected, mRound, mColour, mNumColours);
+  if (I.concurrent) {
+    if (!I.gatheredCurrent) { exchange(); I.gatheredCurrent = true; }
+    roundConcurrent(act);
+  } else {
+    if (!fresh) exchange();
+    for (unsigned a : act) check(dpgo_optimize_resident_async(I.h[a], &I.prm), "dpgo_optimize_resident_async");
+  }
+  ++mRound;
+}
+
+DeviceRBCDSolveReport DeviceRBCD::solve(const DeviceRBCDSolveOptions &o) {
+  Impl &I = *impl;
+  if (o.maxRounds < 1 || o.checkEvery < 1) throw std::invalid_argument("DeviceRBCD::solve: maxRounds and checkEvery must be >= 1");
+  if (I.schedule == "greedy" && o.checkEvery != 1)
+    throw std::invalid_argument("DeviceRBCD::solve: the greedy schedule selects the next agent from every round's status: "
+                                "checkEvery must be 1");
+  const DeviceRBCDStatus st0 = status();
+  std::vector<double> callsAtStart(I.K);
+  for (unsigned a = 0; a < I.K; ++a) callsAtStart[a] = st0.at(a, 4);
+  DeviceRBCDSolveReport rep;
+  bool fresh = true;
+  while (true) {
+    solveRound(fresh);
+    ++rep.rounds;
+    fresh = false;
+    if (rep.rounds % o.checkEvery != 0 && rep.rounds < o.maxRounds) continue;
+    const DeviceRBCDStatus st = status();
+    fresh = true;
+    if (o.callback) o.callback(rep.rounds, st.cost, st.gradnorm);
+    if (I.schedule == "greedy" && !I.neighbors[I.selected].empty()) {   // ref examples/MultiRobotExample.cpp:308-325
+      unsigned arg = 0;
+      for (unsigned a = 1; a < I.K; ++a)
+        if (std::sqrt(st.at(a, 2)) > std::sqrt(st.at(arg, 2))) arg = a;
+      I.selected = arg;
+    }
+    bool team = o.relChangeTol > 0;
+    for (unsigned a = 0; a < I.K && team; ++a) team = st.at(a, 4) > callsAtStart[a] && st.at(a, 3) <= o.relChangeTol;
+    if (o.gradnormTol > 0 && st.gradnorm < o.gradnormTol) rep.reason = "gradnorm";
+    else if (team) rep.reason = "team";
+    else if (rep.rounds >= o.maxRounds) rep.reason = "max_rounds";
+    if (!rep.reason.empty()) {
+      rep.cost = st.cost;
+      rep.gradnorm = st.gradnorm;
+      rep.relativeChange.resize(I.K);
+      for (unsigned a = 0; a < I.K; ++a) rep.relativeChange[a] = st.at(a, 3);
+      return rep;
+    }
+  }
+}
+
+Matrix DeviceRBCD::trajectory() {
+  Impl &I = *impl;
+  Matrix X0(I.r, I.dh * I.count[0]);
+  check(dpgo_problem_download_X(I.h[0], X0.data()), "dpgo_problem_download_X");
+  std::vector<double> anchor(X0.data(), X0.data() + (size_t)I.r * I.dh);    // agent 0's pose 0, r x (d+1) column-major
+  Matrix T(I.d, I.dh * I.n);
+  for (unsigned a = 0; a < I.K; ++a) {
+    Matrix Ta(I.d, I.dh * I.count[a]);
+    check(dpgo_agent_trajectory_global(I.h[a], anchor.data(), Ta.data()), "dpgo_agent_trajectory_global");
+    for (size_t q = 0; q < I.count[a]; ++q) T.block(0, I.globalOf[a][q] * I.dh, I.d, I.dh) = Ta.block(0, q * I.dh, I.d, I.dh);
+  }
+  return T;
 }
 
 }  // namespace DPGO

@@ -22,6 +22,7 @@
 #include <DPGO/PGOAgent.h>
 #include <DPGO/RelativeSEMeasurement.h>
 
+#include <functional>
 #include <memory>
 #include <string>
 #include <vector>
@@ -59,6 +60,34 @@ struct DeviceRBCDStats {
   std::vector<unsigned> active;
 };
 
+// Every agent's status record (DPGO_STATUS_DOUBLES = 5 doubles each, agent-major): <XQ, X>, <X, G>, |rgrad|^2, the
+// relative change of its last optimising call, its optimising calls so far (dpgo_agents_status_async)
+struct DeviceRBCDStatus {
+  std::vector<double> records;
+  double cost = 0;        // 2 f_central = sum of <XQ, X> + <X, G>
+  double gradnorm = 0;    // |grad_central|
+  double at(unsigned agent, unsigned field) const { return records[(size_t)agent * 5 + field]; }
+};
+
+// Stop rules of DeviceRBCD::solve (a tolerance of 0 disables its rule): the central gradient norm below gradnormTol
+// (ref examples/MultiRobotExample.cpp:302-305); every agent optimised since the solve began with its last relative change
+// <= relChangeTol (ref PGOAgent::shouldTerminate, src/PGOAgent.cpp:703-716,1007-1031); maxRounds rounds.  The status is
+// taken after every checkEvery-th round and after the last; the greedy schedule needs checkEvery == 1.
+struct DeviceRBCDSolveOptions {
+  unsigned maxRounds = 500;
+  double gradnormTol = 0.1;
+  double relChangeTol = 5e-3;
+  unsigned checkEvery = 1;
+  std::function<void(unsigned round, double cost, double gradnorm)> callback;   // every check
+};
+
+struct DeviceRBCDSolveReport {
+  unsigned rounds = 0;
+  std::string reason;                 // "gradnorm", "team" or "max_rounds"
+  double cost = 0, gradnorm = 0;
+  std::vector<double> relativeChange; // per agent, of its last optimising call
+};
+
 class DeviceRBCD {
  public:
   // graph: the global pose graph (global pose ids); XInit: r x (d+1)n lifted initial iterate (empty with
@@ -80,10 +109,18 @@ class DeviceRBCD {
   unsigned round() const { return mRound; }
   size_t allGatherBytesPerGpu() const;
   const std::vector<DeviceRBCDInitRecord> &initReport() const { return mInitReport; }   // empty for "central"
+  // one exchange (none when the gathered tiles are current), one status launch per GPU, one copy per GPU into pinned
+  // host memory, one synchronisation per GPU
+  DeviceRBCDStatus status();
+  DeviceRBCDSolveReport solve(const DeviceRBCDSolveOptions &options = DeviceRBCDSolveOptions());
+  // d x (d+1)n trajectory in global pose order, rounded on the device against agent 0's pose 0
+  // (ref getTrajectoryInGlobalFrame, src/PGOAgent.cpp:500-519)
+  Matrix trajectory();
 
  private:
   struct Impl;
   void roundConcurrent(const std::vector<unsigned> &active);
+  void solveRound(bool fresh);
   void alignWaves();
   std::vector<DeviceRBCDInitRecord> mInitReport;
   std::unique_ptr<Impl> impl;

@@ -351,6 +351,32 @@ DPGO_API int dpgo_agent_align_result(dpgo_problem_t *p, double *T_align_host, in
 DPGO_API int dpgo_robust_single_rotation_averaging(int device, int d, int m, const double *R_host, const double *kappa_host,
                                                    double threshold, double *R_out, int32_t *inlier_flags, int32_t *iterations);
 
+/* ---- team status and rounding of the device runners (ref PGOAgentStatus / shouldTerminate, src/PGOAgent.cpp:703-716,
+ *      1007-1031; getTrajectoryInGlobalFrame, :500-519) ------------------------------------------------------------ */
+/* doubles per agent record of dpgo_agents_status_async:
+ *   [0] <XQ, X>   [1] <X, G>   [2] |P_X(XQ + G)|^2 (the same quantities as quad_init, lin_init, gradnorm_init^2 of an
+ *   evaluation)   [3] relative change sqrt(|X - XPrev|^2 / n) of the agent's most recent optimising call (RTR or RGD;
+ *   evaluations leave it alone)   [4] optimising calls since the handle was created */
+#define DPGO_STATUS_DOUBLES 5
+/* One launch for every listed agent (all on one device, one d and r): agent i's record goes to
+ * status_dev + slot[i] * DPGO_STATUS_DOUBLES (device memory; slots distinct).  An agent's record depends only on that
+ * agent (fixed work split and reduction order), bit for bit.  Asynchronous on `stream` (NULL: the first agent's).
+ * Each agent has one partial-sum buffer and one ticket counter: two status calls that include the same agent must be
+ * ordered (one stream, or an event between them), as the round calls of one agent must be.
+ * The first call with a given agent list (and status_dev) uploads its job table and keeps it with the first agent; a
+ * repeated call is a single kernel launch, which a CUDA graph can capture.  A first call cannot be captured.  Up to 32
+ * tables are kept per first agent; a 33rd list synchronises the device and frees the oldest table, so a graph that
+ * captured a status call stays valid only while its agent list is among the last 32 used with that first agent. */
+DPGO_API int dpgo_agents_status_async(dpgo_problem_t *const *agents, int count, const int32_t *slot, double *status_dev,
+                                      void *stream);
+/* ref getTrajectoryInGlobalFrame: anchor_host = [Ya pa] (r x (d+1) column-major, the driver broadcasts agent 0's pose 0);
+ * T_host (d x (d+1)n column-major) gets, per pose, [proj_SO(d)(Ya^T Y_i)  Ya^T p_i - Ya^T pa].  Synchronous. */
+DPGO_API int dpgo_agent_trajectory_global(dpgo_problem_t *p, const double *anchor_host, double *T_host);
+/* page-locked host memory (the destination of the status records of a C++ host) and a stream-ordered copy into it */
+DPGO_API int dpgo_host_alloc_pinned(size_t bytes, void **ptr);
+DPGO_API int dpgo_host_free_pinned(void *ptr);
+DPGO_API int dpgo_copy_to_host_async(int device, void *dst_host, const void *src_dev, size_t bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
