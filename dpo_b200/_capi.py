@@ -123,6 +123,10 @@ SIGNATURES = {
     "dpgo_optimize_resident_from_aux_async": (C.c_int, [_vp, C.POINTER(OptParams)]),
     "dpgo_agents_round_async": (C.c_int, [C.POINTER(_vp), C.c_int, C.POINTER(OptParams), _vp, C.c_int64, C.POINTER(_vp), _vp,
                                           C.c_int]),
+    "dpgo_agents_accel_begin_async": (C.c_int, [C.POINTER(_vp), C.c_int, _ip, C.c_double, C.c_int, C.POINTER(_vp),
+                                                C.POINTER(_vp), _vp]),
+    "dpgo_agents_accel_round_async": (C.c_int, [C.POINTER(_vp), C.c_int, C.POINTER(OptParams), _vp, _vp, C.c_int64, _vp]),
+    "dpgo_agent_accel_state": (C.c_int, [_vp, _dp]),
     "dpgo_agents_host_io_async": (C.c_int, [C.POINTER(_vp), C.c_int, C.POINTER(_vp), C.POINTER(_vp), C.c_int, _vp]),
     "dpgo_agent_f_rgradnorm_resident": (C.c_int, [_vp, _dp, _dp]),
     "dpgo_agent_set_local_trajectory": (C.c_int, [_vp, _dp, _dp]),

@@ -86,6 +86,14 @@ struct dpgo_problem {
   // vectors
   double *d_G = nullptr;
   double *d_acc[3] = {nullptr, nullptr, nullptr};   // Nesterov acceleration: Y, V, XPrev (allocated by accel_init)
+  // accelerated rounds (dpgo_accel.cu): momentum record + ticket on the device; the host's count of begun rounds and the
+  // restart rule of the last begin, which decide whether the agent's next dpgo_agents_accel_round_async restarts
+  double *d_acc_state = nullptr;
+  unsigned *d_acc_ticket = nullptr;
+  long long acc_rounds = 0;
+  bool acc_restart_due = false;
+  struct AccelTable { std::vector<uint64_t> key; dpgo::AccelJob *d_jobs = nullptr; int ctas = 0; };
+  std::vector<AccelTable> accel_tables;    // job tables of dpgo_agents_accel_begin_async, kept by the call's first agent
   double *d_vec[dpgo::V_COUNT] = {};
   double *d_S[2] = {nullptr, nullptr};
   double *d_partials = nullptr;
@@ -98,6 +106,8 @@ struct dpgo_problem {
   // exchange
   int num_public = 0;
   int *d_public = nullptr;
+  int *d_pub_slot = nullptr;     // n: public slot of each pose, -1 when the pose is not public
+  bool pub_slot_unique = true;   // no pose is listed twice (the accelerated rounds pack through d_pub_slot)
   int num_edges = 0, num_shared_poses = 0, max_slot = -1;
   bool G_dirty = true;           // G may hold values that dpgo_agent_build_G does not overwrite
   int *d_pose_ids = nullptr, *d_pose_ptr = nullptr, *d_edge_slot = nullptr, *d_edge_out = nullptr;
@@ -719,6 +729,8 @@ int dpgo_problem_destroy(dpgo_problem_t *p) {
   free_dev(p->d_cand_w); free_dev(p->d_T_align); free_dev(p->d_align_info); free_dev(p->d_jobs); free_dev(p->d_ready);
   free_dev(p->d_opt_record); free_dev(p->d_status_part); free_dev(p->d_status_ticket); free_dev(p->d_anchor); free_dev(p->d_traj);
   for (auto &t : p->status_tables) free_dev(t.d_jobs);
+  free_dev(p->d_acc_state); free_dev(p->d_acc_ticket); free_dev(p->d_pub_slot);
+  for (auto &t : p->accel_tables) free_dev(t.d_jobs);
   free_nd(p);
   if (p->h_result) cudaFreeHost(p->h_result);
   for (auto &g : p->round_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
@@ -1393,12 +1405,20 @@ int dpgo_agent_set_public_poses(dpgo_problem_t *p, int num_public, const int32_t
   DPGO_REQUIRE(num_public >= 0 && (num_public == 0 || public_pose), DPGO_ERR_INVALID_ARG, "bad public pose list");
   for (int s = 0; s < num_public; ++s)
     if (public_pose[s] < 0 || public_pose[s] >= p->n) return fail(DPGO_ERR_INVALID_ARG, "public pose index out of range");
+  std::vector<int> pub_slot((size_t)p->n, -1);
+  p->pub_slot_unique = true;
+  for (int s = 0; s < num_public; ++s) {
+    if (pub_slot[(size_t)public_pose[s]] >= 0) p->pub_slot_unique = false;
+    else pub_slot[(size_t)public_pose[s]] = s;
+  }
   free_dev(p->d_public);
   p->num_public = num_public;
   if (num_public) {
     DPGO_CUDA(cudaMalloc(&p->d_public, sizeof(int) * num_public));
     DPGO_CUDA(cudaMemcpy(p->d_public, public_pose, sizeof(int) * num_public, cudaMemcpyHostToDevice));
   }
+  if (!p->d_pub_slot) DPGO_CUDA(cudaMalloc(&p->d_pub_slot, sizeof(int) * (size_t)p->n));
+  DPGO_CUDA(cudaMemcpy(p->d_pub_slot, pub_slot.data(), sizeof(int) * (size_t)p->n, cudaMemcpyHostToDevice));
   return DPGO_OK;
 }
 
@@ -1486,6 +1506,12 @@ int dpgo_agent_accel_init(dpgo_problem_t *p) {
     if (!p->d_acc[i]) DPGO_CUDA(cudaMalloc(&p->d_acc[i], p->vec_bytes()));
     DPGO_CUDA(cudaMemcpyAsync(p->d_acc[i], p->d_vec[dpgo::V_X0], p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
   }
+  if (!p->d_acc_state) DPGO_CUDA(cudaMalloc(&p->d_acc_state, sizeof(double) * dpgo::ACCEL_STATE_DOUBLES));
+  if (!p->d_acc_ticket) DPGO_CUDA(cudaMalloc(&p->d_acc_ticket, sizeof(unsigned)));
+  DPGO_CUDA(cudaMemsetAsync(p->d_acc_state, 0, sizeof(double) * dpgo::ACCEL_STATE_DOUBLES, p->stream));
+  DPGO_CUDA(cudaMemsetAsync(p->d_acc_ticket, 0, sizeof(unsigned), p->stream));
+  p->acc_rounds = 0;
+  p->acc_restart_due = false;
   return DPGO_OK;
 }
 int dpgo_agent_accel_begin(dpgo_problem_t *p, double alpha) {
@@ -2036,6 +2062,165 @@ int dpgo_copy_to_host_async(int device, void *dst_host, const void *src_dev, siz
   DPGO_REQUIRE(dst_host && src_dev, DPGO_ERR_INVALID_ARG, "null buffer");
   DPGO_CUDA(cudaSetDevice(device));
   DPGO_CUDA(cudaMemcpyAsync(dst_host, src_dev, bytes, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  return DPGO_OK;
+}
+
+// ---- accelerated rounds (dpgo_accel.cu) ------------------------------------------------------------------------------------
+int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, const int32_t *active_flags, double momentum_N,
+                                  int restart_interval, double *const *send_dev, double *const *send_aux_dev, void *stream) {
+  DPGO_TRY(require_device());
+  DPGO_REQUIRE(agents && active_flags && send_dev && send_aux_dev, DPGO_ERR_INVALID_ARG,
+               "null agents, active flags or send buffers");
+  DPGO_REQUIRE(count > 0, DPGO_ERR_INVALID_ARG, "count must be positive");
+  DPGO_REQUIRE(momentum_N >= 1.0 && restart_interval >= 1, DPGO_ERR_INVALID_ARG,
+               "momentum_N must be >= 1 and restart_interval >= 1");
+  dpgo_problem *lead = agents[0];
+  DPGO_REQUIRE(lead, DPGO_ERR_INVALID_ARG, "null problem handle");
+  std::vector<uint64_t> key;
+  key.reserve(5 * (size_t)count);
+  for (int i = 0; i < count; ++i) {
+    const dpgo_problem *p = agents[i];
+    DPGO_REQUIRE(p, DPGO_ERR_INVALID_ARG, "null problem handle");
+    DPGO_REQUIRE(p->device == lead->device && p->d == lead->d && p->r == lead->r, DPGO_ERR_INVALID_ARG,
+                 "the agents of one accelerated call must share the device, d and r");
+    DPGO_ACC_READY(p);
+    DPGO_REQUIRE(p->d_pub_slot && p->pub_slot_unique, DPGO_ERR_STATE,
+                 "the agent needs a public pose list without duplicates (dpgo_agent_set_public_poses)");
+    DPGO_REQUIRE(p->num_public == 0 || (send_dev[i] && send_aux_dev[i]), DPGO_ERR_INVALID_ARG, "null send buffer");
+    key.push_back((uint64_t)(uintptr_t)p);
+    key.push_back(p->generation);
+    key.push_back((uint64_t)(active_flags[i] != 0));
+    key.push_back((uint64_t)(uintptr_t)send_dev[i]);
+    key.push_back((uint64_t)(uintptr_t)send_aux_dev[i]);
+  }
+  DPGO_CUDA(cudaSetDevice(lead->device));
+  cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
+  // as in dpgo_agents_status_async: the job table of an agent list and active set is uploaded once and kept
+  dpgo_problem::AccelTable *tab = nullptr;
+  for (auto &t : lead->accel_tables)
+    if (t.key == key) { tab = &t; break; }
+  if (!tab) {
+    if (lead->accel_tables.size() >= STATUS_TABLES_MAX) {      // a table may still be read by a launch in flight
+      DPGO_CUDA(cudaDeviceSynchronize());
+      free_dev(lead->accel_tables.front().d_jobs);
+      lead->accel_tables.erase(lead->accel_tables.begin());
+    }
+    std::vector<dpgo::AccelJob> jobs((size_t)count);
+    int ctas = 0;
+    for (int i = 0; i < count; ++i) {
+      const dpgo_problem *p = agents[i];
+      dpgo::AccelJob &J = jobs[(size_t)i];
+      J.n = p->n;
+      J.cta0 = ctas;
+      J.active = active_flags[i] != 0;
+      J.X = p->d_vec[dpgo::V_X0]; J.Y = p->d_acc[0]; J.V = p->d_acc[1]; J.XP = p->d_acc[2];
+      J.state = p->d_acc_state;
+      J.pub_slot = p->d_pub_slot;
+      J.send_x = send_dev[i]; J.send_y = send_aux_dev[i];
+      J.ticket = p->d_acc_ticket;
+      ctas += dpgo::accel_ctas(p->n);
+    }
+    dpgo::AccelJob *d_jobs = nullptr;
+    DPGO_CUDA(cudaMalloc(&d_jobs, sizeof(dpgo::AccelJob) * (size_t)count));
+    DPGO_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(dpgo::AccelJob) * (size_t)count, cudaMemcpyHostToDevice, st));
+    lead->accel_tables.emplace_back();
+    tab = &lead->accel_tables.back();
+    tab->key = key;
+    tab->d_jobs = d_jobs;
+    tab->ctas = ctas;
+  }
+  DPGO_CUDA(dpgo::launch_accel_agents(lead->r, lead->dh, count, tab->ctas, tab->d_jobs, momentum_N, restart_interval, st));
+  for (int i = 0; i < count; ++i) {
+    dpgo_problem *p = agents[i];
+    ++p->acc_rounds;
+    p->acc_restart_due = (p->acc_rounds + 1) % restart_interval == 0;
+  }
+  return DPGO_OK;
+}
+
+static int issue_accel_round(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
+                             const double *gathered_dev, const double *gathered_aux_dev, int64_t num_slots, cudaStream_t main) {
+  dpgo_problem *lead = agents[0];
+  DPGO_CUDA(cudaEventRecord(lead->ev_fork, main));
+  for (int i = 0; i < num_active; ++i) {
+    dpgo_problem *p = agents[i];
+    StreamSwap swap(p, p->cluster ? p->own_stream : main);   // cluster steps side by side, full-grid steps in order
+    double *X = p->d_vec[dpgo::V_X0], *Y = p->d_acc[0], *V = p->d_acc[1], *XP = p->d_acc[2];
+    if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork, 0));
+    DPGO_TRY(dpgo_agent_build_G(p, gathered_aux_dev, num_slots));
+    DPGO_CUDA(cudaMemcpyAsync(X, Y, p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
+    DPGO_TRY(dpgo_optimize_resident_async(p, params));
+    DPGO_CUDA(dpgo::launch_accel_finish(p->r, p->dh, p->n, X, Y, V, XP, p->d_acc_state,
+                                        p->acc_restart_due ? dpgo::ACCEL_FINISH_V_RESTART : dpgo::ACCEL_FINISH_V, p->stream));
+    if (p->acc_restart_due) {
+      DPGO_TRY(dpgo_agent_build_G(p, gathered_dev, num_slots));
+      DPGO_TRY(dpgo_optimize_resident_async(p, params));
+      DPGO_CUDA(dpgo::launch_accel_finish(p->r, p->dh, p->n, X, Y, V, XP, p->d_acc_state, dpgo::ACCEL_FINISH_RESTART_END,
+                                          p->stream));
+    }
+    if (p->stream != main) {
+      DPGO_CUDA(cudaEventRecord(p->ev_done, p->stream));
+      DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done, 0));
+    }
+  }
+  return DPGO_OK;
+}
+
+int dpgo_agents_accel_round_async(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
+                                  const double *gathered_dev, const double *gathered_aux_dev, int64_t num_slots,
+                                  void *main_stream) {
+  DPGO_TRY(require_device());
+  DPGO_REQUIRE(num_active >= 0 && (num_active == 0 || agents) && params, DPGO_ERR_INVALID_ARG, "bad arguments");
+  if (num_active == 0) return DPGO_OK;
+  bool graphable = true;
+  for (int i = 0; i < num_active; ++i) {
+    DPGO_CHECK_HANDLE(agents[i]);
+    DPGO_REQUIRE(agents[i]->device == agents[0]->device, DPGO_ERR_INVALID_ARG, "the agents of a round must live on one device");
+    DPGO_ACC_READY(agents[i]);
+    DPGO_REQUIRE(agents[i]->d_acc_state && agents[i]->acc_rounds > 0, DPGO_ERR_STATE,
+                 "dpgo_agents_accel_begin_async has not been called");
+    DPGO_REQUIRE(gathered_aux_dev || agents[i]->num_edges == 0, DPGO_ERR_INVALID_ARG, "null gathered buffer");
+    DPGO_TRY(check_params(agents[i], params));
+    if (!agents[i]->ev_done) DPGO_CUDA(cudaEventCreateWithFlags(&agents[i]->ev_done, cudaEventDisableTiming));
+    if (!agents[i]->cluster || agents[i]->G_dirty || agents[i]->d_phase_ns ||
+        ((agents[i]->precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)) && !agents[i]->nd_ready))
+      graphable = false;
+  }
+  dpgo_problem *lead = agents[0];
+  cudaStream_t main = main_stream ? (cudaStream_t)main_stream : lead->stream;
+  DPGO_CUDA(cudaSetDevice(lead->device));
+  if (!lead->ev_fork) DPGO_CUDA(cudaEventCreateWithFlags(&lead->ev_fork, cudaEventDisableTiming));
+  static const bool use_graph = [] { const char *e = std::getenv("DPGO_ROUND_GRAPH"); return !e || std::atoi(e) != 0; }();
+  if (main == cudaStreamLegacy || main == nullptr) graphable = false;
+  auto issue = [&]() { return issue_accel_round(agents, num_active, params, gathered_dev, gathered_aux_dev, num_slots, main); };
+  if (!use_graph || !graphable) return issue();
+  std::vector<uint64_t> key;
+  key.reserve(3 * (size_t)num_active + 6 + sizeof(*params) / 8 + 1);
+  key.push_back(0x6163630000ull);                           // "acc": never equal to a plain round key (those start with a pointer)
+  for (int i = 0; i < num_active; ++i) {
+    key.push_back((uint64_t)(uintptr_t)agents[i]);
+    key.push_back(agents[i]->generation);
+    key.push_back((uint64_t)agents[i]->acc_restart_due);    // two variants per active set: plain and restart rounds
+  }
+  key.push_back((uint64_t)(uintptr_t)gathered_dev);
+  key.push_back((uint64_t)(uintptr_t)gathered_aux_dev);
+  key.push_back((uint64_t)num_slots);
+  key.push_back((uint64_t)(uintptr_t)main);
+  {
+    uint64_t w[(sizeof(*params) + 7) / 8] = {};
+    std::memcpy(w, params, sizeof(*params));
+    key.insert(key.end(), w, w + sizeof(w) / 8);
+  }
+  return replay_or_issue(lead, key, main, issue);
+}
+
+int dpgo_agent_accel_state(dpgo_problem_t *p, double *out3) {
+  DPGO_TRY(require_device());
+  DPGO_REQUIRE(out3, DPGO_ERR_INVALID_ARG, "null output");
+  DPGO_CHECK_HANDLE(p);
+  DPGO_REQUIRE(p->d_acc_state, DPGO_ERR_STATE, "dpgo_agent_accel_init has not been called");
+  DPGO_CUDA(cudaDeviceSynchronize());                       // the record is written on the stream of the begin calls
+  DPGO_CUDA(cudaMemcpy(out3, p->d_acc_state, 3 * sizeof(double), cudaMemcpyDeviceToHost));
   return DPGO_OK;
 }
 

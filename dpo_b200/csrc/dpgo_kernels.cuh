@@ -188,4 +188,25 @@ cudaError_t launch_agents_status(int r, int dh, int njobs, int total_ctas, const
 // T = [proj_SO(d)(Ya^T X_i R-block), Ya^T X_i t - Ya^T pa] per pose (d x (d+1)n column-major); anchor = [Ya pa], r x (d+1)
 cudaError_t launch_trajectory_global(int r, int dh, int n, const double *anchor, const double *X, double *T, cudaStream_t stream);
 
+// ---- accelerated rounds (dpgo_accel.cu) ----
+// Momentum record of an agent: {gamma, alpha, iterations, gamma of the last round}; the last slot is the gamma the round's
+// V update uses, which a restart has already cleared from slot 0.
+constexpr int ACCEL_STATE_DOUBLES = 4;
+// One agent of an accelerated begin launch: CTAs [cta0, cta0 + accel_ctas(n)) own ACCEL_THREADS consecutive poses each.
+struct AccelJob {
+  int n, cta0, active;
+  double *X, *Y, *V, *XP;
+  double *state;                           // ACCEL_STATE_DOUBLES
+  const int *pub_slot;                     // n: public slot of the pose, -1 when it is not public
+  double *send_x, *send_y;                 // the agent's public tiles of X and of Y
+  unsigned *ticket;                        // CTAs of the agent done in this launch (the last one resets it to 0)
+};
+constexpr int ACCEL_THREADS = 128;
+__host__ __device__ inline int accel_ctas(int n) { return (n + ACCEL_THREADS - 1) / ACCEL_THREADS; }
+cudaError_t launch_accel_agents(int r, int dh, int njobs, int total_ctas, const AccelJob *jobs, double momentum_n,
+                                int restart_interval, cudaStream_t stream);
+enum AccelFinish { ACCEL_FINISH_V = 0, ACCEL_FINISH_V_RESTART = 1, ACCEL_FINISH_RESTART_END = 2 };
+cudaError_t launch_accel_finish(int r, int dh, int n, double *X, double *Y, double *V, const double *XP, const double *state,
+                                int mode, cudaStream_t stream);
+
 }  // namespace dpgo

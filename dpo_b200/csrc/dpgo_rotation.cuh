@@ -54,6 +54,80 @@ template <int D> __device__ __forceinline__ void project_to_rotation(const doubl
       for (int c = 0; c < D; ++c) Rm[a][c] -= 2.0 * y[imin][a] * V[imin][c];
 }
 
+// Stiefel (polar-factor) projection of one pose tile, ref: LiftedSEManifold::project, src/manifold/LiftedSEManifold.cpp:34-45 +
+// projectToStiefelManifold, src/DPGO_utils.cpp:479-485 (U V^T of the thin SVD = polar factor): one-sided (Hestenes) Jacobi
+// SVD of the r x d block -- columns are rotated until mutually orthogonal (Y V = U Sigma), which keeps high relative accuracy
+// for ill-conditioned blocks -- then U V^T; the translation column passes through.  in(e) gives element e = c R + a of the
+// input tile, out(e, v) stores element e of the result.  Every rotation element is read before the first store and the
+// translation is read after the rotation stores, so `out` may write the buffer `in` reads.
+template <int R, int DH, class In, class Out> __device__ __forceinline__ void stiefel_project_tile(const In &in, const Out &out) {
+  constexpr int D = DH - 1;
+  double y[D][R];
+  double V[D][D];
+#pragma unroll
+  for (int c = 0; c < D; ++c) {
+#pragma unroll
+    for (int a = 0; a < R; ++a) y[c][a] = in(c * R + a);
+#pragma unroll
+    for (int q = 0; q < D; ++q) V[c][q] = (c == q) ? 1.0 : 0.0;     // V[c] = column c of V
+  }
+  for (int sweep = 0; sweep < 30; ++sweep) {
+    bool rotated = false;
+#pragma unroll
+    for (int p = 0; p < D; ++p)
+#pragma unroll
+      for (int q = p + 1; q < D; ++q) {
+        double alpha = 0, beta = 0, gamma = 0;
+#pragma unroll
+        for (int a = 0; a < R; ++a) {
+          alpha = fma(y[p][a], y[p][a], alpha);
+          beta = fma(y[q][a], y[q][a], beta);
+          gamma = fma(y[p][a], y[q][a], gamma);
+        }
+        if (fabs(gamma) <= 1e-17 * sqrt(alpha * beta) || gamma == 0.0) continue;
+        rotated = true;
+        const double zeta = (beta - alpha) / (2.0 * gamma);
+        const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+        const double cs = 1.0 / sqrt(1.0 + t * t), sn = cs * t;
+#pragma unroll
+        for (int a = 0; a < R; ++a) {
+          const double yp = y[p][a], yq = y[q][a];
+          y[p][a] = cs * yp - sn * yq;
+          y[q][a] = sn * yp + cs * yq;
+        }
+#pragma unroll
+        for (int k = 0; k < D; ++k) {
+          const double vp = V[p][k], vq = V[q][k];
+          V[p][k] = cs * vp - sn * vq;
+          V[q][k] = sn * vp + cs * vq;
+        }
+      }
+    if (!rotated) break;
+  }
+  // normalise the rotated columns: U = (Y V) Sigma^-1
+#pragma unroll
+  for (int c = 0; c < D; ++c) {
+    double s = 0;
+#pragma unroll
+    for (int a = 0; a < R; ++a) s = fma(y[c][a], y[c][a], s);
+    const double inv = (s > 0.0) ? 1.0 / sqrt(s) : 0.0;
+#pragma unroll
+    for (int a = 0; a < R; ++a) y[c][a] *= inv;
+  }
+  // out = U V^T : out[a, c] = sum_k U[a,k] V[c,k]   (V[k][c'] holds entry c' of column k)
+#pragma unroll
+  for (int c = 0; c < D; ++c)
+#pragma unroll
+    for (int a = 0; a < R; ++a) {
+      double s = 0;
+#pragma unroll
+      for (int k = 0; k < D; ++k) s = fma(y[k][a], V[k][c], s);
+      out(c * R + a, s);
+    }
+#pragma unroll
+  for (int a = 0; a < R; ++a) out(D * R + a, in(D * R + a));
+}
+
 // GNC-TLS weight of a squared residual r2 at control parameter mu and threshold cbar (Yang et al., eq. 14; ref
 // RobustCost::weight, src/DPGO_robust.cpp:49-61): 0 above (mu+1)/mu cbar^2, 1 below mu/(mu+1) cbar^2, in between
 // cbar sqrt(mu (mu+1)) / r - mu.

@@ -36,6 +36,10 @@ struct DeviceRBCD::Impl {
   std::vector<int> gpuOf;
   std::vector<void *> stream;
   std::vector<double *> send, gathered;
+  std::vector<double *> sendAux, gatheredAux;      // accelerated rounds: the public tiles of Y
+  bool acceleration = false;
+  unsigned restartInterval = 30;
+  double momentumN = 1;
   std::vector<ncclComm_t> comm;
   std::vector<std::vector<unsigned>> neighbors;
   dpgo_opt_params_t prm;
@@ -70,6 +74,13 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
   if (!distributed && ((size_t)XInit.rows() != opt.r || (size_t)XInit.cols() != (graph[0].t.size() + 1) * n))
     throw std::runtime_error("DeviceRBCD: XInit must be r x (d+1)n");
   if (I.K % I.N != 0) throw std::runtime_error("DeviceRBCD: the agents must divide evenly over the GPUs");
+  if (opt.momentumBlocks != "agents" && opt.momentumBlocks != "colours")
+    throw std::invalid_argument("DeviceRBCD: momentumBlocks must be agents or colours");
+  if (opt.momentumBlocks == "colours" && I.schedule != "coloured")
+    throw std::invalid_argument("DeviceRBCD: momentumBlocks = colours counts the colour classes of the coloured schedule");
+  if (opt.acceleration && opt.restartInterval < 1) throw std::invalid_argument("DeviceRBCD: restartInterval must be >= 1");
+  I.acceleration = opt.acceleration;
+  I.restartInterval = opt.restartInterval;
   int ndev = 0;
   check(dpgo_device_count(&ndev), "dpgo_device_count");
   if ((int)I.N > ndev) throw std::runtime_error("DeviceRBCD: fewer CUDA devices than requested GPUs");
@@ -129,7 +140,8 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
           for (unsigned a = g * I.perGpu; a < (g + 1) * I.perGpu; ++a) cnt += (mColour[a] == c);
           most = std::max(most, cnt);
         }
-    I.concurrent = opt.concurrent < 0 ? (most >= 2) : (opt.concurrent != 0);
+    const bool agentMomentum = opt.acceleration && opt.momentumBlocks == "agents";
+    I.concurrent = opt.concurrent < 0 ? (most >= 2 && !agentMomentum) : (opt.concurrent != 0);
     if (I.concurrent && I.schedule == "parallel")
       throw std::runtime_error("DeviceRBCD: concurrent rounds are implemented for the greedy and coloured schedules");
   }
@@ -293,6 +305,23 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
     }
     alignWaves();
   }
+  if (I.acceleration) {
+    I.momentumN = opt.momentumBlocks == "colours" ? (double)mNumColours : (double)K;
+    for (unsigned a = 0; a < K; ++a) check(dpgo_agent_accel_init(I.h[a]), "dpgo_agent_accel_init");
+    I.sendAux.assign(I.N, nullptr);
+    I.gatheredAux.assign(I.N, nullptr);
+    for (unsigned g = 0; g < I.N; ++g) {
+      void *p = nullptr;
+      check(dpgo_device_malloc((int)g, sizeof(double) * K * slotElems, &p), "dpgo_device_malloc");
+      I.gatheredAux[g] = static_cast<double *>(p);
+      if (I.N == 1) {
+        I.sendAux[g] = I.gatheredAux[g];
+      } else {
+        check(dpgo_device_malloc((int)g, sizeof(double) * I.perGpu * slotElems, &p), "dpgo_device_malloc");
+        I.sendAux[g] = static_cast<double *>(p);
+      }
+    }
+  }
   dpgo_opt_params_default(&I.prm);
   I.prm.algorithm = (opt.algorithm == ROPTALG::RTR) ? DPGO_ALG_RTR : DPGO_ALG_RGD;
   I.prm.precond = (int)opt.preconditioner;
@@ -312,6 +341,10 @@ DeviceRBCD::~DeviceRBCD() {
   for (unsigned g = 0; g < I.N; ++g) {
     if (I.N > 1 && I.send[g]) dpgo_device_free((int)g, I.send[g]);
     if (I.gathered[g]) dpgo_device_free((int)g, I.gathered[g]);
+    if (g < I.gatheredAux.size()) {
+      if (I.N > 1 && I.sendAux[g]) dpgo_device_free((int)g, I.sendAux[g]);
+      if (I.gatheredAux[g]) dpgo_device_free((int)g, I.gatheredAux[g]);
+    }
     if (g < I.statusDev.size() && I.statusDev[g]) dpgo_device_free((int)g, I.statusDev[g]);
     if (I.stream[g]) dpgo_stream_destroy((int)g, I.stream[g]);
   }
@@ -437,11 +470,56 @@ void DeviceRBCD::roundConcurrent(const std::vector<unsigned> &active) {
   }
 }
 
+// one accelerated round: per GPU one begin call (momentum, Y, the idle agents' iterate(false), packs of the X and Y tiles),
+// one all-gather group per buffer, per GPU one call for the active agents (G from the Y tiles, step from Y, V, restart)
+void DeviceRBCD::roundAccelerated(const std::vector<unsigned> &active) {
+  Impl &I = *impl;
+  const size_t slotElems = (size_t)I.pmax * I.ts;
+  for (unsigned g = 0; g < I.N; ++g) {
+    std::vector<dpgo_problem *> hs;
+    std::vector<int32_t> flags;
+    std::vector<double *> sx, sy;
+    for (unsigned a = g * I.perGpu; a < (g + 1) * I.perGpu; ++a) {
+      const size_t off = (I.N == 1 ? a : a % I.perGpu) * slotElems;
+      hs.push_back(I.h[a]);
+      flags.push_back(std::find(active.begin(), active.end(), a) != active.end() ? 1 : 0);
+      sx.push_back(I.send[g] + off);
+      sy.push_back(I.sendAux[g] + off);
+    }
+    check(dpgo_agents_accel_begin_async(hs.data(), (int)hs.size(), flags.data(), I.momentumN, (int)I.restartInterval, sx.data(),
+                                        sy.data(), I.stream[g]),
+          "dpgo_agents_accel_begin_async");
+  }
+  if (I.N > 1)
+    for (const auto *bufs : {&I.send, &I.sendAux}) {
+      const std::vector<double *> &dst = (bufs == &I.send) ? I.gathered : I.gatheredAux;
+      checkNccl(ncclGroupStart(), "ncclGroupStart");
+      for (unsigned g = 0; g < I.N; ++g) {
+        check(dpgo_device_set((int)g), "dpgo_device_set");
+        checkNccl(ncclAllGather((*bufs)[g], dst[g], I.perGpu * slotElems, ncclDouble, I.comm[g], (cudaStream_t)I.stream[g]),
+                  "ncclAllGather");
+      }
+      checkNccl(ncclGroupEnd(), "ncclGroupEnd");
+    }
+  for (unsigned g = 0; g < I.N; ++g) {
+    std::vector<dpgo_problem *> hs;
+    for (unsigned a : active)
+      if ((unsigned)I.gpuOf[a] == g) hs.push_back(I.h[a]);
+    if (hs.empty()) continue;
+    check(dpgo_agents_accel_round_async(hs.data(), (int)hs.size(), &I.prm, I.gathered[g], I.gatheredAux[g], (int64_t)I.K * I.pmax,
+                                        I.stream[g]),
+          "dpgo_agents_accel_round_async");
+  }
+  I.gatheredCurrent = false;                           // the gathered X tiles predate the active agents' steps
+}
+
 void DeviceRBCD::runRounds(unsigned rounds) {
   Impl &I = *impl;
   for (unsigned it = 0; it < rounds; ++it) {
     const std::vector<unsigned> act = activeSet(I.schedule, I.K, I.selected, mRound, mColour, mNumColours);
-    if (I.concurrent) {
+    if (I.acceleration) {
+      roundAccelerated(act);
+    } else if (I.concurrent) {
       if (!I.gatheredCurrent) { exchange(); I.gatheredCurrent = true; }
       roundConcurrent(act);
     } else {
@@ -457,7 +535,9 @@ DeviceRBCDStats DeviceRBCD::step(bool evaluate) {
   DeviceRBCDStats st;
   st.active = activeSet(I.schedule, I.K, I.selected, mRound, mColour, mNumColours);
   dpgo_opt_result_t res;
-  if (I.concurrent) {
+  if (I.acceleration) {
+    roundAccelerated(st.active);
+  } else if (I.concurrent) {
     if (!I.gatheredCurrent) { exchange(); I.gatheredCurrent = true; }
     roundConcurrent(st.active);
   } else {
@@ -556,6 +636,9 @@ void DeviceRBCD::solveRound(bool fresh) {
 
 DeviceRBCDSolveReport DeviceRBCD::solve(const DeviceRBCDSolveOptions &o) {
   Impl &I = *impl;
+  if (I.acceleration)
+    throw std::invalid_argument("DeviceRBCD::solve: acceleration is not supported: the accelerated iterate's relative change "
+                                "is measured against the Nesterov step's XPrev; drive it with step()");
   if (o.maxRounds < 1 || o.checkEvery < 1) throw std::invalid_argument("DeviceRBCD::solve: maxRounds and checkEvery must be >= 1");
   if (I.schedule == "greedy" && o.checkEvery != 1)
     throw std::invalid_argument("DeviceRBCD::solve: the greedy schedule selects the next agent from every round's status: "

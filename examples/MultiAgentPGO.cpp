@@ -32,7 +32,7 @@ struct Options {
   double stop = 0.1;
   bool accel = false, rgd = false, jacobi = false, resident = false;
   unsigned gpus = 1, bench = 0;
-  std::string schedule = "greedy", partition, init = "central";
+  std::string schedule = "greedy", partition, init = "central", momentum = "agents";
 };
 
 static Options parse(int argc, char **argv) {
@@ -54,12 +54,14 @@ static Options parse(int argc, char **argv) {
     else if (a == "--bench") o.bench = (unsigned)std::stoul(next());
     else if (a == "--partition") o.partition = next();
     else if (a == "--init") o.init = next();
+    else if (a == "--momentum") o.momentum = next();
     else if (a.rfind("--", 0) == 0) { std::cerr << "unknown option " << a << std::endl; std::exit(2); }
     else o.file = a;
   }
   if (o.file.empty()) {
     std::cerr << "usage: MultiAgentPGO <file.g2o> [--robots K] [--iters N] [--stop G] [--accel] [--rgd] [--jacobi] "
-                 "[--rank R] [--trace out.csv]" << std::endl;
+                 "[--rank R] [--trace out.csv] [--resident [--gpus N] [--schedule greedy|coloured|parallel] [--momentum agents|colours]]"
+              << std::endl;
     std::exit(2);
   }
   return o;
@@ -89,6 +91,8 @@ int main(int argc, char **argv) {
       if (ro.owner.size() != n) { std::cerr << "partition file: " << ro.owner.size() << " lines for " << n << " poses" << std::endl; return 1; }
     }
     ro.initialization = opt.init;
+    ro.acceleration = opt.accel;
+    ro.momentumBlocks = opt.momentum;
     const Matrix lifted0 = (opt.init == "distributed") ? Matrix() : Matrix(fixedStiefelVariable(d, r) * chordalInitialization(d, n, graph));
     DeviceRBCD run(graph, n, K, lifted0, ro);
     for (size_t a = 0; a < run.initReport().size(); ++a) {

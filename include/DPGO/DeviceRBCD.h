@@ -46,6 +46,14 @@ struct DeviceRBCDOptions {
   // initialisation of its private graph in its own frame, then frame-alignment waves (robust average of the frame
   // transforms its shared loop closures give with an initialised neighbour, ref src/PGOAgent.cpp:369-440); XInit empty
   std::string initialization = "central";
+  // Nesterov-accelerated rounds (ref src/PGOAgent.cpp:685-695,1033-1091) in the reference driver's order: the idle agents
+  // finish iterate(false), the X and Y tiles are exchanged (one ncclAllGather group per buffer), the active agents step
+  // from Y.  momentumBlocks is the N of the recurrence: "agents" = the number of agents (the reference's), "colours" = the
+  // number of colour classes (schedule "coloured" only: a coloured round is one exact block update).  With "agents" the
+  // automatic launch mode is one agent at a time.  solve() rejects acceleration.
+  bool acceleration = false;
+  unsigned restartInterval = 30;
+  std::string momentumBlocks = "agents";
 };
 
 // per agent: the wave it joined the global frame in (agent 0: 0), the neighbour it aligned to (-1 for agent 0), the
@@ -120,6 +128,7 @@ class DeviceRBCD {
  private:
   struct Impl;
   void roundConcurrent(const std::vector<unsigned> &active);
+  void roundAccelerated(const std::vector<unsigned> &active);
   void solveRound(bool fresh);
   void alignWaves();
   std::vector<DeviceRBCDInitRecord> mInitReport;

@@ -318,6 +318,30 @@ DPGO_API int dpgo_agents_round_async(dpgo_problem_t *const *agents, int num_acti
  * stream the first handle is set to); a repeated call is replayed as a CUDA graph. */
 DPGO_API int dpgo_agents_host_io_async(dpgo_problem_t *const *agents, int count, double *const *X_host,
                               double *const *send_dev, int direction, void *stream);
+/* ---- accelerated rounds with one call per GPU (ref src/PGOAgent.cpp:685-695,1033-1091; examples/MultiRobotExample.cpp:
+ *      236-279): the momentum record {gamma, alpha, iterations} of each agent lives on the device ---------------------- */
+/* Begins a round for `count` agents of one device (after dpgo_agent_accel_init and dpgo_agent_set_public_poses): advances
+ * every agent's record, gamma' = (1 + sqrt(1 + ((4 N) N) (gamma gamma))) / (2 N), alpha = 1 / (gamma' N) with N = momentum_N,
+ * bit for bit in this operation order; XPrev = X; Y = proj((1 - alpha) X + alpha V).  An agent with active_flags[i] == 0
+ * finishes its iterate(false): X = Y, V = proj(V + gamma (X - Y)), and on a restart round ((iterations + 1) %
+ * restart_interval == 0) X = XPrev, V = Y = X, gamma = alpha = 0.  Then every agent's public tiles of X and Y go to
+ * send_dev[i] and send_aux_dev[i].  One launch on `stream` (NULL: the first agent's).  Calls that share an agent must be
+ * ordered (one ticket counter per agent).  Job tables are kept per agent list and active set, as for
+ * dpgo_agents_status_async. */
+DPGO_API int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, const int32_t *active_flags,
+                                           double momentum_N, int restart_interval, double *const *send_dev,
+                                           double *const *send_aux_dev, void *stream);
+/* The active agents' part of the round begun by dpgo_agents_accel_begin_async, once the X tiles are in gathered_dev and
+ * the Y tiles in gathered_aux_dev.  Per agent: G from the Y tiles -> X = Y -> one step (thread-block cluster agents on
+ * their own streams between a fork from and a join into main_stream, full-grid agents in order on main_stream) ->
+ * V = proj(V + gamma (X - Y)); on a restart round then X = XPrev -> G from the X tiles -> one plain step -> V = Y = X.
+ * Nothing is packed.  A repeated round is replayed as a CUDA graph (two variants per active set: plain and restart);
+ * DPGO_ROUND_GRAPH=0 keeps the eager launches. */
+DPGO_API int dpgo_agents_accel_round_async(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
+                                           const double *gathered_dev, const double *gathered_aux_dev, int64_t num_slots,
+                                           void *main_stream);
+/* the agent's momentum record {gamma, alpha, iterations} after every call issued so far (synchronises the device) */
+DPGO_API int dpgo_agent_accel_state(dpgo_problem_t *p, double *out3);
 /* per-agent Riemannian gradient norm / cost of the resident iterate (greedy selection input) */
 DPGO_API int dpgo_agent_f_rgradnorm_resident(dpgo_problem_t *p, double *f_out, double *norm_out);
 
