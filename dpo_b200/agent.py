@@ -543,8 +543,9 @@ class DistributedPGO:
                             gradient norm; examples/MultiRobotExample.cpp:229-334) -- parity mode;
              = "coloured" : all agents of one colour class per round (concurrent, same RBCD semantics);
              = "parallel" : every agent every round on the neighbours' previous poses.
-    Per round: pack public poses -> ONE all-gather -> device-side G rebuild -> local optimise ->
-    3-scalar all-gather for the central cost / gradient norm / selection.
+    Per round: G rebuild from the gathered public poses -> local optimise -> pack -> ONE all-gather; with evaluation, the
+    team status (one status launch per GPU, one all-gather of the records) gives the central cost / gradient norm /
+    selection.
     """
 
     def __init__(self, edges: EdgeSet, n: int, k: int, r: int = 5, algorithm: int = ROPTALG.RTR,
@@ -688,11 +689,9 @@ class DistributedPGO:
             self.momentum_N = float(self.ncolours if momentum_blocks == "colours" else k)
             for a in self.local_ids:
                 capi.check(self.agents[a].mProblem._lib.dpgo_agent_accel_init(self.agents[a].mProblem._h))
-        self.stats_local = torch.zeros(4 * len(self.local_ids), dtype=torch.float64, device=self.dev)
-        self.stats_all = torch.zeros(4 * k, dtype=torch.float64, device=self.dev)
         self.selected = [0]
         self.round = 0
-        self._gathered_current = False       # concurrent mode: `gathered` holds every agent's current public tiles
+        self._gathered_current = False       # `gathered` holds every agent's current public tiles
 
     # -- distributed initialisation: alignment waves (ref src/PGOAgent.cpp:369-440, examples/MultiRobotExample.cpp:245-256) --
     def _align_waves(self) -> List[Dict[str, int]]:
@@ -754,9 +753,10 @@ class DistributedPGO:
             for a in self.local_ids:
                 self.agents[a].build_G(self.gathered.data_ptr(), self.k * self.plan.pmax)
 
-    def _round_concurrent(self, active: List[int], publish: bool = True) -> None:
-        """G rebuild -> RTR step -> pack for every active local agent, each on its own stream, with one C call; then the
-        all-gather that publishes the new public tiles.  Asynchronous (no host synchronisation)."""
+    def _round(self, active: List[int], publish: bool = True) -> None:
+        """G rebuild -> RTR step -> pack for every active local agent with one C call (thread-block cluster agents side by
+        side on their own streams, full-grid agents one after the other); then, with publish, the all-gather of the new
+        public tiles.  The gathered tiles must be current.  Asynchronous (no host synchronisation)."""
         mine = [a for a in self.local_ids if a in active]
         lib = self.agents[self.local_ids[0]].mProblem._lib
         if mine:
@@ -764,9 +764,11 @@ class DistributedPGO:
             sd = (C.c_void_p * len(mine))(*[C.c_void_p(self.send[a].data_ptr()) for a in mine])
             capi.check(lib.dpgo_agents_round_async(hs, len(mine), C.byref(self.agents[mine[0]].opt._p),
                                                    C.c_void_p(self.gathered.data_ptr()), self.k * self.plan.pmax, sd,
-                                                   C.c_void_p(self._main_stream), 0))
+                                                   C.c_void_p(self._main_stream), int(self.schedule == "parallel")))
         if self.distributed and publish:
             self.dist.all_gather_into_tensor(self.gathered, self.send_all)
+
+    _round_concurrent = _round               # bench.py times its rounds through this name
 
     def _active(self) -> List[int]:
         if self.schedule == "greedy":
@@ -775,22 +777,6 @@ class DistributedPGO:
             c = self.round % self.ncolours
             return [a for a in range(self.k) if self.colour[a] == c]
         return list(range(self.k))
-
-    def evaluate(self) -> Tuple[float, float, np.ndarray]:
-        """Central cost 2f, |grad|, per-agent gradient norms from per-agent (quad, lin, |g|^2)."""
-        vals = np.zeros((self.k, 4))
-        for a in self.local_ids:
-            res = self.agents[a].opt.problem_stats()
-            vals[a] = res
-        if self.distributed:
-            t = self.torch
-            mine = np.ascontiguousarray(vals[self.local_ids[0]:self.local_ids[-1] + 1]).ravel()
-            self.stats_local.copy_(t.from_numpy(mine))
-            self.dist.all_gather_into_tensor(self.stats_all, self.stats_local)
-            vals = self.stats_all.cpu().numpy().reshape(self.k, 4)
-        cost = float(np.sum(vals[:, 0] + vals[:, 1]))          # 2 f_central = sum(<XQ,X> + <X,G>)
-        gn2 = vals[:, 2]
-        return cost, float(np.sqrt(np.sum(gn2))), np.sqrt(gn2)
 
     def _step_accelerated(self) -> List[int]:
         """One round of the accelerated schedule, in the reference driver's order (examples/MultiRobotExample.cpp:236-279):
@@ -831,46 +817,24 @@ class DistributedPGO:
         return active
 
     def step(self, evaluate: bool = True) -> Optional[RoundStats]:
-        """One round: exchange, active agents optimise, (optionally) exchange again + evaluate + select."""
+        """One round, then (optionally) the team status: central cost, gradient norm and the greedy selection."""
         if self.acceleration:
             active = self._step_accelerated()
-            self.round += 1
-            if not evaluate:
-                return None
-            self.exchange()
-            cost, gn, per_agent = self.evaluate()
-            if self.schedule == "greedy" and self.plan.tables[self.selected[0]]["neighbors"]:
-                self.selected = [int(np.argmax(per_agent))]
-            return RoundStats(cost, gn, active)
-        active = self._active()
-        if self.concurrent:
+        else:
+            active = self._active()
             if not self._gathered_current:
                 self.exchange(build=False)
                 self._gathered_current = True
-            self._round_concurrent(active)
+            self._round(active)
             for a in self.local_ids:
                 if a in active:
-                    self.agents[a].mIterationNumber += 1
-        else:
-            self.exchange()
-            for a in self.local_ids:
-                if a in active:
-                    self.agents[a].opt.optimize_resident_async()
-            for a in self.local_ids:
-                if a in active:
-                    if evaluate:
-                        self.agents[a].lastResult = self.agents[a].opt.fetch_result()
                     self.agents[a].mIterationNumber += 1
         self.round += 1
         if not evaluate:
             return None
-        self.exchange()                                   # fresh neighbour poses for the central gradient
-        cost, gn, per_agent = self.evaluate()
-        if self.schedule == "greedy":
-            cur = self.selected[0]
-            if self.plan.tables[cur]["neighbors"]:
-                self.selected = [int(np.argmax(per_agent))]           # ref :308-325
-        return RoundStats(cost, gn, active)
+        st = self.status()
+        self._select(st)
+        return RoundStats(st.cost, st.gradnorm, active)
 
     # -- one round with host buffers in and out (the public host-level call of the runner) ---------------------------
     def _host_buffers(self):
@@ -886,57 +850,40 @@ class DistributedPGO:
         return self._hx
 
     def step_host(self) -> None:
-        """One round with every iterate crossing the host boundary: per local agent X is uploaded from pinned host
-        memory, the public poses are exchanged (pack -> one all-gather -> G rebuild, on the device), the active agents
-        optimise, and their iterates are read back to the host.  ag.X (host) is the state between rounds."""
+        """One round with every iterate crossing the host boundary: one call uploads every local agent's X from pinned host
+        memory and packs its public tiles, the all-gather publishes them, one call steps the active agents, one call reads
+        their iterates back, then one synchronisation (the calls are replayed as CUDA graphs when they can be).  ag.X (host)
+        is the state between rounds."""
         hx = self._host_buffers()
         for a in self.local_ids:
             if hx[a] is not self.agents[a].X:
                 hx[a][...] = self.agents[a].X
-            if not self.concurrent:
-                self.agents[a].mProblem.upload_X_async(hx[a])
         active = self._active()
-        if self.concurrent:
-            # one call per direction for the host boundary (uploads + packs / downloads, replayed as CUDA graphs), one
-            # for the round, one synchronisation
-            mine = [a for a in self.local_ids if a in active]
-            lib = self.agents[self.local_ids[0]].mProblem._lib
-            if not hasattr(self, "_io"):
-                self._io = {}
-            def arrays(ids, with_send):
-                key = (tuple(ids), with_send)
-                if key not in self._io:
-                    hs = (C.c_void_p * len(ids))(*[self.agents[a].mProblem._h for a in ids])
-                    hp = (C.c_void_p * len(ids))(*[C.c_void_p(self._hx_keep[a].data_ptr()) for a in ids])
-                    sd = (C.c_void_p * len(ids))(*[C.c_void_p(self.send[a].data_ptr()) for a in ids]) if with_send else None
-                    self._io[key] = (hs, hp, sd)
-                return self._io[key]
-            hs, hp, sd = arrays(self.local_ids, True)
-            capi.check(lib.dpgo_agents_host_io_async(hs, len(self.local_ids), hp, sd, 0, C.c_void_p(self._main_stream)))
-            if self.distributed:
-                self.dist.all_gather_into_tensor(self.gathered, self.send_all)
-            self._round_concurrent(active, publish=False)    # the next host round re-publishes every agent's tiles
-            self._gathered_current = False
-            if mine:
-                hs, hp, _ = arrays(mine, False)
-                capi.check(lib.dpgo_agents_host_io_async(hs, len(mine), hp, None, 1, C.c_void_p(self._main_stream)))
-                self.agents[mine[0]].mProblem.sync()
-            for a in mine:
-                self.agents[a].X = hx[a]
-                self.agents[a].mIterationNumber += 1
-            self.round += 1
-            return
-        else:
-            self.exchange()
-            for a in self.local_ids:
-                if a in active:
-                    self.agents[a].opt.optimize_resident_async()
-                    self.agents[a].mProblem.download_X_async(hx[a])
-        for a in self.local_ids:
-            if a in active:
-                self.agents[a].mProblem.sync()
-                self.agents[a].X = hx[a]
-                self.agents[a].mIterationNumber += 1
+        mine = [a for a in self.local_ids if a in active]
+        lib = self.agents[self.local_ids[0]].mProblem._lib
+        if not hasattr(self, "_io"):
+            self._io = {}
+        def arrays(ids, with_send):
+            key = (tuple(ids), with_send)
+            if key not in self._io:
+                hs = (C.c_void_p * len(ids))(*[self.agents[a].mProblem._h for a in ids])
+                hp = (C.c_void_p * len(ids))(*[C.c_void_p(self._hx_keep[a].data_ptr()) for a in ids])
+                sd = (C.c_void_p * len(ids))(*[C.c_void_p(self.send[a].data_ptr()) for a in ids]) if with_send else None
+                self._io[key] = (hs, hp, sd)
+            return self._io[key]
+        hs, hp, sd = arrays(self.local_ids, True)
+        capi.check(lib.dpgo_agents_host_io_async(hs, len(self.local_ids), hp, sd, 0, C.c_void_p(self._main_stream)))
+        if self.distributed:
+            self.dist.all_gather_into_tensor(self.gathered, self.send_all)
+        self._round(active, publish=False)               # the next host round re-publishes every agent's tiles
+        self._gathered_current = False
+        if mine:
+            hs, hp, _ = arrays(mine, False)
+            capi.check(lib.dpgo_agents_host_io_async(hs, len(mine), hp, None, 1, C.c_void_p(self._main_stream)))
+            self.agents[mine[0]].mProblem.sync()
+        for a in mine:
+            self.agents[a].X = hx[a]
+            self.agents[a].mIterationNumber += 1
         self.round += 1
 
     # -- the same round through the HOST-level interface (reference protocol: host matrices in and out) -------
@@ -974,6 +921,7 @@ class DistributedPGO:
                     poses[(b, int(q))] = hg[off:off + ts].reshape(self.r, dh, order="F")
                 ag.updateNeighborPoses(b, poses)
             ag.iterate(True)
+        self._gathered_current = False       # iterate() replaced the resident iterates behind the gathered tiles
         self.round += 1
 
     def host_bytes_per_step(self):
@@ -1010,14 +958,13 @@ class DistributedPGO:
 
     def _refresh_G(self) -> None:
         """Every local agent's G from the current public tiles: one exchange, or only the G rebuild when the gathered tiles
-        are current (concurrent rounds keep them so)."""
-        if self.concurrent and self._gathered_current:
+        are current (plain rounds keep them so)."""
+        if self._gathered_current:
             for a in self.local_ids:
                 self.agents[a].build_G(self.gathered.data_ptr(), self.k * self.plan.pmax)
         else:
             self.exchange()
-            if self.concurrent:
-                self._gathered_current = True
+            self._gathered_current = True
 
     def _status(self) -> TeamStatus:
         self._refresh_G()
@@ -1035,25 +982,10 @@ class DistributedPGO:
             self.dist.all_gather_into_tensor(self._status_all, self._status_local)
         return team_status(self._status_all.cpu().numpy().reshape(self.k, S))
 
-    def _solve_round(self, fresh: bool) -> None:
-        """One round without evaluation, as step(evaluate=False) issues it; fresh: every agent's G was built from the
-        current tiles by the status just taken, so the round does not repeat that exchange."""
-        active = self._active()
-        if self.concurrent:
-            if not self._gathered_current:
-                self.exchange(build=False)
-                self._gathered_current = True
-            self._round_concurrent(active)
-        else:
-            if not fresh:
-                self.exchange()
-            for a in self.local_ids:
-                if a in active:
-                    self.agents[a].opt.optimize_resident_async()
-        for a in self.local_ids:
-            if a in active:
-                self.agents[a].mIterationNumber += 1
-        self.round += 1
+    def _select(self, st: TeamStatus) -> None:
+        if self.schedule == "greedy":
+            cur = self.selected[0]
+            self.selected = [greedy_selection(cur, np.sqrt(st.records[:, 2]), bool(self.plan.tables[cur]["neighbors"]))]
 
     def solve(self, max_rounds: int = 500, gradnorm_tol: float = 0.1, rel_change_tol: float = 5e-3, check_every: int = 1,
               callback=None) -> SolveReport:
@@ -1067,20 +999,16 @@ class DistributedPGO:
 
     def _solve(self, max_rounds, gradnorm_tol, rel_change_tol, check_every, callback) -> SolveReport:
         calls_at_start = self.status().records[:, 4].copy()
-        rounds, fresh = 0, True
+        rounds = 0
         while True:
-            self._solve_round(fresh)
+            self.step(evaluate=False)
             rounds += 1
-            fresh = False
             if rounds % check_every != 0 and rounds < max_rounds:
                 continue
             st = self.status()
-            fresh = True
             if callback is not None:
                 callback(rounds, st.cost, st.gradnorm)
-            if self.schedule == "greedy":
-                cur = self.selected[0]
-                self.selected = [greedy_selection(cur, np.sqrt(st.records[:, 2]), bool(self.plan.tables[cur]["neighbors"]))]
+            self._select(st)
             reason = stop_reason(st.records, calls_at_start, rounds, max_rounds, gradnorm_tol, rel_change_tol)
             if reason is not None:
                 return SolveReport(rounds, reason, st.cost, st.gradnorm, st.records[:, 3].copy())

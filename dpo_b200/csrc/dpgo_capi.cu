@@ -56,7 +56,8 @@ struct dpgo_problem {
   cudaEvent_t ev_done = nullptr, ev_fork = nullptr;   // fork / join of dpgo_agents_round_async
   uint64_t generation = 0;       // bumped whenever device buffers a captured round refers to may have been replaced
   struct RoundGraph { std::vector<uint64_t> key; cudaGraphExec_t exec = nullptr; int uses = 0; bool failed = false; };
-  std::vector<RoundGraph> round_graphs;      // CUDA graphs of dpgo_agents_round_async, kept by the first agent of the round
+  std::vector<RoundGraph> round_graphs;      // CUDA graphs of the batched round / host I/O calls, kept by the call's first agent
+  template <class Job> struct JobTable { std::vector<uint64_t> key; Job *d_jobs = nullptr; int ctas = 0; };
   int launch_mode = -1;          // -1: by DPGO_CLUSTER_MAX_POSES (default off), 0: full cooperative grid, 1: one thread-block cluster
   // Q in block-CSR
   int64_t nb = 0;
@@ -92,8 +93,7 @@ struct dpgo_problem {
   unsigned *d_acc_ticket = nullptr;
   long long acc_rounds = 0;
   bool acc_restart_due = false;
-  struct AccelTable { std::vector<uint64_t> key; dpgo::AccelJob *d_jobs = nullptr; int ctas = 0; };
-  std::vector<AccelTable> accel_tables;    // job tables of dpgo_agents_accel_begin_async, kept by the call's first agent
+  std::vector<JobTable<dpgo::AccelJob>> accel_tables;    // job tables of dpgo_agents_accel_begin_async, kept by the call's first agent
   double *d_vec[dpgo::V_COUNT] = {};
   double *d_S[2] = {nullptr, nullptr};
   double *d_partials = nullptr;
@@ -126,8 +126,7 @@ struct dpgo_problem {
   // team status (dpgo_status.cu): last optimising call's relative change + count, per-CTA partials, ticket of the last CTA
   double *d_opt_record = nullptr, *d_status_part = nullptr;
   unsigned *d_status_ticket = nullptr;
-  struct StatusTable { std::vector<uint64_t> key; dpgo::StatusJob *d_jobs = nullptr; int ctas = 0; };
-  std::vector<StatusTable> status_tables;  // job tables of dpgo_agents_status_async, kept by the call's first agent
+  std::vector<JobTable<dpgo::StatusJob>> status_tables;  // job tables of dpgo_agents_status_async, kept by the call's first agent
   double *d_anchor = nullptr, *d_traj = nullptr;   // dpgo_agent_trajectory_global
 
   size_t vec_bytes() const { return sizeof(double) * (size_t)r * (size_t)N; }
@@ -1611,6 +1610,51 @@ template <class Issue> int replay_or_issue(dpgo_problem *lead, const std::vector
   return DPGO_OK;
 }
 
+// DPGO_ROUND_GRAPH=0 keeps the eager launches of every call that would otherwise replay a CUDA graph
+bool round_graphs_enabled() {
+  static const bool on = [] { const char *e = std::getenv("DPGO_ROUND_GRAPH"); return !e || std::atoi(e) != 0; }();
+  return on;
+}
+
+// What the round calls check and prepare alike: every handle on the first one's device, with valid parameters and a join
+// event; the first handle's fork event; the stream the round forks from and joins into (main_stream, NULL: the stream the
+// first handle is set to); whether the round may be replayed as a CUDA graph.
+int round_preamble(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params, void *main_stream,
+                   cudaStream_t &main, bool &graph) {
+  graph = round_graphs_enabled();
+  for (int i = 0; i < num_active; ++i) {
+    dpgo_problem *p = agents[i];
+    DPGO_CHECK_HANDLE(p);
+    DPGO_REQUIRE(p->device == agents[0]->device, DPGO_ERR_INVALID_ARG, "the agents of a round must live on one device");
+    DPGO_TRY(check_params(p, params));
+    if (!p->ev_done) DPGO_CUDA(cudaEventCreateWithFlags(&p->ev_done, cudaEventDisableTiming));
+    // a cooperative launch does not capture; a pending G clear or an unbuilt factorisation must run eagerly first
+    if (!p->cluster || p->G_dirty || p->d_phase_ns || ((p->precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)) && !p->nd_ready))
+      graph = false;
+  }
+  dpgo_problem *lead = agents[0];
+  main = main_stream ? (cudaStream_t)main_stream : lead->stream;
+  DPGO_CUDA(cudaSetDevice(lead->device));
+  if (!lead->ev_fork) DPGO_CUDA(cudaEventCreateWithFlags(&lead->ev_fork, cudaEventDisableTiming));
+  if (main == cudaStreamLegacy || main == nullptr) graph = false;   // the legacy default stream cannot be captured
+  return DPGO_OK;
+}
+
+// The start of a round graph's key: a tag that keeps the keys of different calls apart, the stream, the slot count, the
+// parameters, every agent's handle and generation.  The caller appends the buffers its launches capture.
+std::vector<uint64_t> round_key(uint64_t tag, dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
+                                cudaStream_t main, int64_t num_slots) {
+  uint64_t w[(sizeof(*params) + 7) / 8] = {};
+  std::memcpy(w, params, sizeof(*params));
+  std::vector<uint64_t> key{tag, (uint64_t)(uintptr_t)main, (uint64_t)num_slots};
+  key.insert(key.end(), w, w + sizeof(w) / 8);
+  for (int i = 0; i < num_active; ++i) {
+    key.push_back((uint64_t)(uintptr_t)agents[i]);
+    key.push_back(agents[i]->generation);
+  }
+  return key;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1624,7 +1668,7 @@ static int issue_round(dpgo_problem_t *const *agents, int num_active, const dpgo
     DPGO_CUDA(cudaEventRecord(lead->ev_fork, main));
     for (int i = 0; i < num_active; ++i) {
       dpgo_problem *p = agents[i];
-      StreamSwap swap(p, p->own_stream);      // the agent's kernels go to its own stream
+      StreamSwap swap(p, p->cluster ? p->own_stream : main);   // cluster steps side by side, full-grid steps in order
       if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork, 0));
       if (pass == 0) {
         DPGO_TRY(dpgo_agent_build_G(p, gathered_dev, num_slots));
@@ -1640,58 +1684,30 @@ static int issue_round(dpgo_problem_t *const *agents, int num_active, const dpgo
   return DPGO_OK;
 }
 
-// One RBCD round of the agents of one GPU, issued with one call.  Every active agent works on its OWN stream:
-//   main stream --fork--> [ G rebuild from the gathered tiles -> RTR step (persistent kernel) -> pack of its public tiles ] --join--> main
-// so agents launched as single thread-block clusters (dpgo_problem_set_launch_mode(p, 1)) share the GPU: up to 8 clusters
-// of 16 CTAs run side by side.  Agents of one colour class are never neighbours, so a pack into the (aliased) gathered
-// buffer cannot race with another active agent's G rebuild; with pack_after_join != 0 (every agent active on the previous
-// round's poses) the packs are issued in a second fork/join instead.
-// A round with the same agents, buffers and parameters as an earlier one is replayed as a CUDA graph (the cluster launches
-// are ordinary launches, so the fork/join captures): 1 driver call per round instead of ~7 per agent, which is what
-// bounds 8 agents x ~100 us of GPU work otherwise.  DPGO_ROUND_GRAPH=0 keeps the eager launches.
+// One RBCD round of the agents of one GPU, issued with one call.  Per active agent: G rebuild from the gathered tiles -> RTR
+// step -> pack of its public tiles.  Agents launched as single thread-block clusters (dpgo_problem_set_launch_mode(p, 1))
+// work on their own streams between a fork from and a join into main, so up to 8 clusters of 16 CTAs share the GPU;
+// full-grid agents run in order on main.  Agents of one colour class are never neighbours, so a pack into the (aliased)
+// gathered buffer cannot race with another active agent's G rebuild; with pack_after_join != 0 (every agent active on the
+// previous round's poses) the packs are issued in a second pass instead.
+// A cluster round with the same agents, buffers and parameters as an earlier one is replayed as a CUDA graph (the cluster
+// launches are ordinary launches, so the fork/join captures): 1 driver call per round instead of ~7 per agent, which is
+// what bounds 8 agents x ~100 us of GPU work otherwise.  A round with a full-grid agent stays eager.
 int dpgo_agents_round_async(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
                             const double *gathered_dev, int64_t num_slots, double *const *send_dev, void *main_stream,
                             int pack_after_join) {
   DPGO_REQUIRE(num_active >= 0 && (num_active == 0 || (agents && send_dev)) && params, DPGO_ERR_INVALID_ARG, "bad arguments");
   if (num_active == 0) return DPGO_OK;
-  bool graphable = true;
-  for (int i = 0; i < num_active; ++i) {
-    DPGO_CHECK_HANDLE(agents[i]);
-    DPGO_REQUIRE(agents[i]->device == agents[0]->device, DPGO_ERR_INVALID_ARG, "the agents of a round must live on one device");
-    DPGO_TRY(check_params(agents[i], params));
-    if (!agents[i]->ev_done) DPGO_CUDA(cudaEventCreateWithFlags(&agents[i]->ev_done, cudaEventDisableTiming));
-    // a cooperative launch does not capture; a pending G clear or an unbuilt factorisation must run eagerly first
-    if (!agents[i]->cluster || agents[i]->G_dirty || agents[i]->d_phase_ns ||
-        ((agents[i]->precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)) && !agents[i]->nd_ready))
-      graphable = false;
-  }
-  dpgo_problem *lead = agents[0];
-  cudaStream_t main = main_stream ? (cudaStream_t)main_stream : lead->stream;   // NULL: the stream the first handle is set to
-  DPGO_CUDA(cudaSetDevice(lead->device));
-  if (!lead->ev_fork) DPGO_CUDA(cudaEventCreateWithFlags(&lead->ev_fork, cudaEventDisableTiming));
-  static const bool use_graph = [] { const char *e = std::getenv("DPGO_ROUND_GRAPH"); return !e || std::atoi(e) != 0; }();
-  if (main == cudaStreamLegacy || main == nullptr) graphable = false;   // the legacy default stream cannot be captured
-  if (!use_graph || !graphable)
-    return issue_round(agents, num_active, params, gathered_dev, num_slots, send_dev, main, pack_after_join);
-
-  std::vector<uint64_t> key;
-  key.reserve(3 * (size_t)num_active + 8 + sizeof(*params) / 8 + 1);
-  for (int i = 0; i < num_active; ++i) {
-    key.push_back((uint64_t)(uintptr_t)agents[i]);
-    key.push_back(agents[i]->generation);
-    key.push_back((uint64_t)(uintptr_t)send_dev[i]);
-  }
-  key.push_back((uint64_t)(uintptr_t)gathered_dev);
-  key.push_back((uint64_t)num_slots);
-  key.push_back((uint64_t)(uintptr_t)main);
-  key.push_back((uint64_t)pack_after_join);
-  {
-    uint64_t w[(sizeof(*params) + 7) / 8] = {};
-    std::memcpy(w, params, sizeof(*params));
-    key.insert(key.end(), w, w + sizeof(w) / 8);
-  }
+  cudaStream_t main = nullptr;
+  bool graph = false;
+  DPGO_TRY(round_preamble(agents, num_active, params, main_stream, main, graph));
   auto issue = [&]() { return issue_round(agents, num_active, params, gathered_dev, num_slots, send_dev, main, pack_after_join); };
-  return replay_or_issue(lead, key, main, issue);
+  if (!graph) return issue();
+  std::vector<uint64_t> key = round_key(0x726e640000ull, agents, num_active, params, main, num_slots);   // "rnd"
+  for (int i = 0; i < num_active; ++i) key.push_back((uint64_t)(uintptr_t)send_dev[i]);
+  key.push_back((uint64_t)(uintptr_t)gathered_dev);
+  key.push_back((uint64_t)pack_after_join);
+  return replay_or_issue(agents[0], key, main, issue);
 }
 
 // The host boundary of a round with one call per direction (the end-to-end path of DistributedPGO.step_host):
@@ -1735,11 +1751,10 @@ int dpgo_agents_host_io_async(dpgo_problem_t *const *agents, int count, double *
     }
     return DPGO_OK;
   };
-  static const bool use_graph = [] { const char *e = std::getenv("DPGO_ROUND_GRAPH"); return !e || std::atoi(e) != 0; }();
-  if (!use_graph || main == cudaStreamLegacy || main == nullptr) return issue();
+  if (!round_graphs_enabled() || main == cudaStreamLegacy || main == nullptr) return issue();
   std::vector<uint64_t> key;
   key.reserve(3 * (size_t)count + 4);
-  key.push_back(0x696f0000ull + (uint64_t)direction);       // "io": never equal to a round key (those start with a pointer)
+  key.push_back(0x696f0000ull + (uint64_t)direction);       // "io": never equal to a round key (those start with another tag)
   for (int i = 0; i < count; ++i) {
     key.push_back((uint64_t)(uintptr_t)agents[i]);
     key.push_back(agents[i]->generation);
@@ -1965,6 +1980,29 @@ int require_device() {
   return DPGO_OK;
 }
 constexpr size_t STATUS_TABLES_MAX = 32;
+
+// The job table of an agent list is filled (fill(jobs) returns the CTA count) and uploaded once, stream-ordered, and kept in
+// `tables` under `key`; a repeated call finds it, so the call is one kernel launch and nothing else and can be captured into
+// a CUDA graph.  Past STATUS_TABLES_MAX tables the oldest is freed.
+template <class Job, class Fill>
+int job_table(std::vector<dpgo_problem::JobTable<Job>> &tables, std::vector<uint64_t> &key, int count, cudaStream_t st,
+              Fill fill, const dpgo_problem::JobTable<Job> *&tab) {
+  for (const auto &t : tables)
+    if (t.key == key) { tab = &t; return DPGO_OK; }
+  if (tables.size() >= STATUS_TABLES_MAX) {                // a table may still be read by a launch in flight
+    DPGO_CUDA(cudaDeviceSynchronize());
+    free_dev(tables.front().d_jobs);
+    tables.erase(tables.begin());
+  }
+  std::vector<Job> jobs((size_t)count);
+  const int ctas = fill(jobs);
+  Job *d_jobs = nullptr;
+  DPGO_CUDA(cudaMalloc(&d_jobs, sizeof(Job) * (size_t)count));
+  DPGO_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(Job) * (size_t)count, cudaMemcpyHostToDevice, st));
+  tables.push_back({std::move(key), d_jobs, ctas});
+  tab = &tables.back();
+  return DPGO_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -1993,18 +2031,8 @@ int dpgo_agents_status_async(dpgo_problem_t *const *agents, int count, const int
   key.push_back((uint64_t)(uintptr_t)status_dev);
   DPGO_CUDA(cudaSetDevice(lead->device));
   cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
-  // The job table of an agent list is uploaded once (stream-ordered) and kept; a repeated call is one kernel launch
-  // and nothing else, so it can be captured into a CUDA graph.
-  dpgo_problem::StatusTable *tab = nullptr;
-  for (auto &t : lead->status_tables)
-    if (t.key == key) { tab = &t; break; }
-  if (!tab) {
-    if (lead->status_tables.size() >= STATUS_TABLES_MAX) {     // a table may still be read by a launch in flight
-      DPGO_CUDA(cudaDeviceSynchronize());
-      free_dev(lead->status_tables.front().d_jobs);
-      lead->status_tables.erase(lead->status_tables.begin());
-    }
-    std::vector<dpgo::StatusJob> jobs((size_t)count);
+  const dpgo_problem::JobTable<dpgo::StatusJob> *tab = nullptr;
+  DPGO_TRY(job_table(lead->status_tables, key, count, st, [&](std::vector<dpgo::StatusJob> &jobs) {
     int ctas = 0;
     for (int i = 0; i < count; ++i) {
       const dpgo_problem *p = agents[i];
@@ -2019,15 +2047,8 @@ int dpgo_agents_status_async(dpgo_problem_t *const *agents, int count, const int
       J.out = status_dev + (size_t)slot[i] * DPGO_STATUS_DOUBLES;
       ctas += dpgo::status_ctas(p->n);
     }
-    dpgo::StatusJob *d_jobs = nullptr;
-    DPGO_CUDA(cudaMalloc(&d_jobs, sizeof(dpgo::StatusJob) * (size_t)count));
-    DPGO_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(dpgo::StatusJob) * (size_t)count, cudaMemcpyHostToDevice, st));
-    lead->status_tables.emplace_back();
-    tab = &lead->status_tables.back();
-    tab->key = key;
-    tab->d_jobs = d_jobs;
-    tab->ctas = ctas;
-  }
+    return ctas;
+  }, tab));
   DPGO_CUDA(dpgo::launch_agents_status(lead->r, lead->dh, count, tab->ctas, tab->d_jobs, st));
   return DPGO_OK;
 }
@@ -2095,17 +2116,8 @@ int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, cons
   }
   DPGO_CUDA(cudaSetDevice(lead->device));
   cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
-  // as in dpgo_agents_status_async: the job table of an agent list and active set is uploaded once and kept
-  dpgo_problem::AccelTable *tab = nullptr;
-  for (auto &t : lead->accel_tables)
-    if (t.key == key) { tab = &t; break; }
-  if (!tab) {
-    if (lead->accel_tables.size() >= STATUS_TABLES_MAX) {      // a table may still be read by a launch in flight
-      DPGO_CUDA(cudaDeviceSynchronize());
-      free_dev(lead->accel_tables.front().d_jobs);
-      lead->accel_tables.erase(lead->accel_tables.begin());
-    }
-    std::vector<dpgo::AccelJob> jobs((size_t)count);
+  const dpgo_problem::JobTable<dpgo::AccelJob> *tab = nullptr;
+  DPGO_TRY(job_table(lead->accel_tables, key, count, st, [&](std::vector<dpgo::AccelJob> &jobs) {
     int ctas = 0;
     for (int i = 0; i < count; ++i) {
       const dpgo_problem *p = agents[i];
@@ -2120,15 +2132,8 @@ int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, cons
       J.ticket = p->d_acc_ticket;
       ctas += dpgo::accel_ctas(p->n);
     }
-    dpgo::AccelJob *d_jobs = nullptr;
-    DPGO_CUDA(cudaMalloc(&d_jobs, sizeof(dpgo::AccelJob) * (size_t)count));
-    DPGO_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(dpgo::AccelJob) * (size_t)count, cudaMemcpyHostToDevice, st));
-    lead->accel_tables.emplace_back();
-    tab = &lead->accel_tables.back();
-    tab->key = key;
-    tab->d_jobs = d_jobs;
-    tab->ctas = ctas;
-  }
+    return ctas;
+  }, tab));
   DPGO_CUDA(dpgo::launch_accel_agents(lead->r, lead->dh, count, tab->ctas, tab->d_jobs, momentum_N, restart_interval, st));
   for (int i = 0; i < count; ++i) {
     dpgo_problem *p = agents[i];
@@ -2172,46 +2177,24 @@ int dpgo_agents_accel_round_async(dpgo_problem_t *const *agents, int num_active,
   DPGO_TRY(require_device());
   DPGO_REQUIRE(num_active >= 0 && (num_active == 0 || agents) && params, DPGO_ERR_INVALID_ARG, "bad arguments");
   if (num_active == 0) return DPGO_OK;
-  bool graphable = true;
   for (int i = 0; i < num_active; ++i) {
     DPGO_CHECK_HANDLE(agents[i]);
-    DPGO_REQUIRE(agents[i]->device == agents[0]->device, DPGO_ERR_INVALID_ARG, "the agents of a round must live on one device");
     DPGO_ACC_READY(agents[i]);
     DPGO_REQUIRE(agents[i]->d_acc_state && agents[i]->acc_rounds > 0, DPGO_ERR_STATE,
                  "dpgo_agents_accel_begin_async has not been called");
     DPGO_REQUIRE(gathered_aux_dev || agents[i]->num_edges == 0, DPGO_ERR_INVALID_ARG, "null gathered buffer");
-    DPGO_TRY(check_params(agents[i], params));
-    if (!agents[i]->ev_done) DPGO_CUDA(cudaEventCreateWithFlags(&agents[i]->ev_done, cudaEventDisableTiming));
-    if (!agents[i]->cluster || agents[i]->G_dirty || agents[i]->d_phase_ns ||
-        ((agents[i]->precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)) && !agents[i]->nd_ready))
-      graphable = false;
   }
-  dpgo_problem *lead = agents[0];
-  cudaStream_t main = main_stream ? (cudaStream_t)main_stream : lead->stream;
-  DPGO_CUDA(cudaSetDevice(lead->device));
-  if (!lead->ev_fork) DPGO_CUDA(cudaEventCreateWithFlags(&lead->ev_fork, cudaEventDisableTiming));
-  static const bool use_graph = [] { const char *e = std::getenv("DPGO_ROUND_GRAPH"); return !e || std::atoi(e) != 0; }();
-  if (main == cudaStreamLegacy || main == nullptr) graphable = false;
+  cudaStream_t main = nullptr;
+  bool graph = false;
+  DPGO_TRY(round_preamble(agents, num_active, params, main_stream, main, graph));
   auto issue = [&]() { return issue_accel_round(agents, num_active, params, gathered_dev, gathered_aux_dev, num_slots, main); };
-  if (!use_graph || !graphable) return issue();
-  std::vector<uint64_t> key;
-  key.reserve(3 * (size_t)num_active + 6 + sizeof(*params) / 8 + 1);
-  key.push_back(0x6163630000ull);                           // "acc": never equal to a plain round key (those start with a pointer)
-  for (int i = 0; i < num_active; ++i) {
-    key.push_back((uint64_t)(uintptr_t)agents[i]);
-    key.push_back(agents[i]->generation);
+  if (!graph) return issue();
+  std::vector<uint64_t> key = round_key(0x6163630000ull, agents, num_active, params, main, num_slots);   // "acc"
+  for (int i = 0; i < num_active; ++i)
     key.push_back((uint64_t)agents[i]->acc_restart_due);    // two variants per active set: plain and restart rounds
-  }
   key.push_back((uint64_t)(uintptr_t)gathered_dev);
   key.push_back((uint64_t)(uintptr_t)gathered_aux_dev);
-  key.push_back((uint64_t)num_slots);
-  key.push_back((uint64_t)(uintptr_t)main);
-  {
-    uint64_t w[(sizeof(*params) + 7) / 8] = {};
-    std::memcpy(w, params, sizeof(*params));
-    key.insert(key.end(), w, w + sizeof(w) / 8);
-  }
-  return replay_or_issue(lead, key, main, issue);
+  return replay_or_issue(agents[0], key, main, issue);
 }
 
 int dpgo_agent_accel_state(dpgo_problem_t *p, double *out3) {

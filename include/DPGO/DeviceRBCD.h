@@ -4,11 +4,12 @@
 // std::map "PoseDict"s (examples/MultiRobotExample.cpp:229-334, src/PGOAgent.cpp:95-105,434-458).  This runner keeps
 // the iterates in HBM and replaces that "network" by ONE ncclAllGather per round over NVLink:
 //
-//   per round, on every GPU's stream:   dpgo_agent_pack_public  (public tiles -> send buffer)
-//                                       ncclAllGather           (padded public-pose slots of all agents)
-//                                       dpgo_agent_build_G      (linear term from the gathered tiles, ref :783-859)
-//                                       dpgo_optimize_resident_async for the agents of the round
+//   per round, on every GPU's stream:   dpgo_agents_round_async  per active agent: dpgo_agent_build_G (linear term from
+//                                                                the gathered tiles, ref :783-859) -> RTR step ->
+//                                                                pack of its public tiles into the send buffer
+//                                       ncclAllGather            (padded public-pose slots of all agents)
 //
+// so the gathered tiles stay current from round to round; an evaluation (step(true), status()) only rebuilds G from them.
 // K agents are spread over N GPUs of one node (K % N == 0, contiguous blocks), one process, one stream and one NCCL
 // communicator per GPU (ncclCommInitAll).  Schedules: "greedy" (the reference's: one agent per round, argmax of the block
 // gradient norms -- reproduces the shipped traces), "coloured" (all agents of one colour class of the agent graph per
@@ -107,7 +108,7 @@ class DeviceRBCD {
   DeviceRBCD &operator=(const DeviceRBCD &) = delete;
 
   void exchange();                              // pack -> all-gather -> G rebuild, asynchronous on the GPU streams
-  DeviceRBCDStats step(bool evaluate = true);   // one round (+ central cost / gradient norm / greedy selection)
+  DeviceRBCDStats step(bool evaluate = true);   // one round (+ status(): central cost / gradient norm / greedy selection)
   void runRounds(unsigned rounds);              // rounds without evaluation (throughput), asynchronous; call sync()
   void sync();
   Matrix assemble();                            // r x (d+1)n iterate on the host
@@ -127,9 +128,8 @@ class DeviceRBCD {
 
  private:
   struct Impl;
-  void roundConcurrent(const std::vector<unsigned> &active);
+  std::vector<unsigned> issueRound();           // one round of the schedule's active agents; returns them
   void roundAccelerated(const std::vector<unsigned> &active);
-  void solveRound(bool fresh);
   void alignWaves();
   std::vector<DeviceRBCDInitRecord> mInitReport;
   std::unique_ptr<Impl> impl;

@@ -305,10 +305,12 @@ DPGO_API int dpgo_agent_pack_public_aux(dpgo_problem_t *p, double *send_dev);
 DPGO_API int dpgo_optimize_resident_from_aux_async(dpgo_problem_t *p, const dpgo_opt_params_t *params);
 /* One RBCD round of the active agents of one GPU with one call (ref: the body of the round loop,
  * examples/MultiRobotExample.cpp:229-334: updateNeighborPoses -> iterate() -> getSharedPoseDict per selected agent).
- * Every agent works on its own stream between a fork from and a join into main_stream: G rebuild from gathered_dev ->
- * RTR step -> pack of its public tiles into send_dev[i].  main_stream NULL = the stream the first handle is set to.
- * pack_after_join != 0 issues the packs in a second fork/join
- * (needed when neighbouring agents are active in the same round and send_dev aliases gathered_dev). */
+ * Per agent: G rebuild from gathered_dev -> RTR step -> pack of its public tiles into send_dev[i] (thread-block cluster
+ * agents on their own streams between a fork from and a join into main_stream, full-grid agents in order on main_stream).
+ * main_stream NULL = the stream the first handle is set to.  pack_after_join != 0 issues the packs in a second pass,
+ * after every agent's step (needed when neighbouring agents are active in the same round and send_dev aliases
+ * gathered_dev).  A repeated round of cluster agents is replayed as a CUDA graph; a round with a full-grid agent is issued
+ * eagerly (a cooperative launch does not capture).  DPGO_ROUND_GRAPH=0 keeps the eager launches. */
 DPGO_API int dpgo_agents_round_async(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
                             const double *gathered_dev, int64_t num_slots, double *const *send_dev, void *main_stream,
                             int pack_after_join);

@@ -11,11 +11,14 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--dataset", default="sphere2500")
 ap.add_argument("--agents", type=int, default=16)
 ap.add_argument("--rounds", type=int, default=100)
+ap.add_argument("--concurrent", choices=("auto", "0", "1"), default="auto",
+                help="launch mode: agents side by side (1), one after the other as full-grid kernels (0), or the runner's default")
 args = ap.parse_args()
 edges, n = pg.read_g2o_file(os.path.join(ROOT, "data", args.dataset + ".g2o"))
 side = torch.cuda.Stream()
 with torch.cuda.stream(side):
-    run = DistributedPGO(edges, n, args.agents, r=5, schedule="coloured")
+    run = DistributedPGO(edges, n, args.agents, r=5, schedule="coloured",
+                         concurrent=None if args.concurrent == "auto" else args.concurrent == "1")
     for _ in range(6):
         run.step_host()
     torch.cuda.synchronize()

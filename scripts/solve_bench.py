@@ -7,8 +7,8 @@ step() loop of scripts/bench_configs.py.  One GPU, one process; the variants alt
 Per workload (sphere2500 / 16 agents coloured side by side, torus3D / 8 agents coloured, sphere2500 / 5 agents greedy):
   eval_us      one evaluated round's check, host clock over --reps calls, each ending in a device synchronise:
                "batched" = DistributedPGO.status() (exchange + one dpgo_agents_status_async + copy + synchronise),
-               "per_agent" = the same exchange (or G rebuild, when the gathered tiles are current) + evaluate() (one OP_EVAL
-               launch and one synchronising fetch per agent)
+               "per_agent" = the same exchange (or G rebuild, when the gathered tiles are current) + every agent's
+               problem_stats() (one OP_EVAL launch and one synchronising fetch per agent)
   solve        rounds to |g| < 0.1 and wall time of solve(check_every = c) and of the step() loop evaluating every c-th round
 Prints ONE JSON line with the GPU's name, power limit and maximum SM clock, and the registers / spills ptxas reported for
 the status kernel's instantiations (dpo_b200/lib/obj/dpgo_status.cu.ptxas.log, written by the build).
@@ -82,7 +82,8 @@ def main():
                 run.step(evaluate=False)
             run.status()
             run._refresh_G()
-            run.evaluate()
+            for a in run.local_ids:
+                run.agents[a].opt.problem_stats()
             ev = {"batched": [], "per_agent": []}
             for _ in range(2):
                 for variant in ("batched", "per_agent"):
@@ -93,7 +94,8 @@ def main():
                             run.status()
                         else:                            # the same exchange work as status()
                             run._refresh_G()
-                            run.evaluate()
+                            for a in run.local_ids:
+                                run.agents[a].opt.problem_stats()
                     ev[variant].append(round((time.perf_counter() - t0) / args.reps * 1e6, 1))
             rec = {"dataset": ds, "agents": k, "schedule": schedule, "concurrent": run.concurrent, "eval_us": ev,
                    "solve": []}

@@ -104,18 +104,28 @@ def test_final_trajectory_parking_garage(data_dir, golden_dir):
     assert np.abs(T - ref).max() <= 5e-4
 
 
-@pytest.mark.parametrize("conc", [False, True])
-def test_host_level_round_equals_resident_round(conc, data_dir):
-    """DistributedPGO.step_host (X from / to pinned host memory every round) == the device-resident rounds, bit for bit;
-    step_host_dict (the reference's PoseDict protocol on the host) agrees to rounding."""
+@pytest.mark.parametrize("schedule,conc", [("coloured", False), ("coloured", True), ("greedy", False), ("parallel", False)])
+def test_host_level_round_equals_resident_round(schedule, conc, data_dir):
+    """DistributedPGO.step_host (X from / to pinned host memory every round) and the rounds bench.py issues by hand
+    (exchange, then every active agent's optimize_resident_async) == the device-resident rounds, bit for bit;
+    step_host_dict (the reference's PoseDict protocol on the host) agrees to rounding.  The parallel schedule is the one
+    whose round call packs after every agent's step."""
     from dpo_b200.agent import DistributedPGO
     edges, n = load("smallGrid3D", data_dir)
-    runs = [DistributedPGO(edges, n, 5, r=5, schedule="coloured", concurrent=conc) for _ in range(3)]
+    runs = [DistributedPGO(edges, n, 5, r=5, schedule=schedule, concurrent=conc) for _ in range(4)]
+    hand = runs[3]
     for _ in range(6):
         runs[0].step(evaluate=False)
         runs[1].step_host()
         runs[2].step_host_dict()
+        active = hand._active()
+        hand.exchange()
+        for a in hand.local_ids:
+            if a in active:
+                hand.agents[a].opt.optimize_resident_async()
+        hand.round += 1
     X0 = runs[0].assemble()
+    assert np.array_equal(hand.assemble(), X0)
     dh = edges.d + 1
     for q, tol in ((1, 0.0), (2, 1e-11)):
         Xh = np.zeros_like(X0)
