@@ -139,6 +139,10 @@ SIGNATURES = {
     "dpgo_host_alloc_pinned": (C.c_int, [C.c_size_t, C.POINTER(_vp)]),
     "dpgo_host_free_pinned": (C.c_int, [_vp]),
     "dpgo_copy_to_host_async": (C.c_int, [C.c_int, _vp, _vp, C.c_size_t, _vp]),
+    "dpgo_agents_set_agent_graph": (C.c_int, [_vp, C.c_int, _ip, _ip]),
+    "dpgo_agents_select_round_async": (C.c_int, [C.POINTER(_vp), C.c_int, _ip, C.POINTER(OptParams), _vp, _vp, C.c_int64,
+                                                 C.POINTER(_vp), _vp]),
+    "dpgo_agents_selection_log": (C.c_int, [_vp, C.c_int64, C.c_int64, C.POINTER(C.c_uint8), C.POINTER(C.c_int64)]),
 }
 
 _lib = None

@@ -505,6 +505,18 @@ def greedy_selection(selected: int, agent_gradnorms: np.ndarray, has_neighbours:
     return int(np.argmax(agent_gradnorms)) if has_neighbours else int(selected)
 
 
+def greedy_independent_set(gradnorm2: np.ndarray, neighbours: Sequence[Sequence[int]]) -> List[int]:
+    """The agents of one round of the greedy_set schedule, sorted: walk the agents in decreasing squared block gradient norm
+    (ties to the lower id, as std::max_element), taking an agent unless one of its neighbours is already taken.  The result
+    is a maximal independent set of the agent graph; on a complete agent graph it is {argmax}, the reference's greedy choice
+    (ref examples/MultiRobotExample.cpp:308-325).  A NaN norm ranks last.  k_select_independent computes the same set."""
+    g = np.nan_to_num(np.asarray(gradnorm2, dtype=np.float64), nan=-1.0)
+    taken = np.zeros(g.shape[0], dtype=bool)
+    for a in sorted(range(g.shape[0]), key=lambda a: (-g[a], a)):
+        taken[a] = not any(taken[b] for b in neighbours[a])
+    return [int(a) for a in np.flatnonzero(taken)]
+
+
 def check_solve_arguments(schedule: str, acceleration: bool, max_rounds: int, check_every: int) -> None:
     if acceleration:
         raise ValueError("solve() does not support acceleration=True: the accelerated iterate's relative change is "
@@ -523,13 +535,18 @@ def check_accel_arguments(schedule: str, momentum_blocks: str) -> None:
                          "schedule='coloured'")
 
 
-def auto_concurrent(colour: Sequence[int], k: int, world: int, schedule: str, acceleration: bool) -> bool:
+def auto_concurrent(colour: Sequence[int], k: int, world: int, schedule: str, acceleration: bool,
+                    neighbours: Optional[Sequence[Sequence[int]]] = None) -> bool:
     """Default launch mode of a k-agent run over `world` ranks (contiguous blocks of k/world agents per rank): the agents of
     a round step side by side (thread-block clusters, dpgo_agents_round_async) when some rank hosts >= 2 agents of one
-    colour class under the coloured schedule.  A pure function of the global plan, so every rank decides alike."""
+    colour class under the coloured schedule, or >= 2 agents that are not neighbours under the greedy_set schedule.  A pure
+    function of the global plan, so every rank decides alike."""
+    per_rank = k // max(world, 1)
+    if schedule == "greedy_set" and neighbours is not None:
+        return any(b not in neighbours[a] for q in range(max(world, 1))
+                   for a in range(q * per_rank, (q + 1) * per_rank) for b in range(a + 1, (q + 1) * per_rank))
     if schedule != "coloured" or acceleration:
         return False
-    per_rank = k // max(world, 1)
     ncol = max(colour) + 1
     most = max(sum(1 for a in range(q * per_rank, (q + 1) * per_rank) if colour[a] == c)
                for q in range(max(world, 1)) for c in range(ncol))
@@ -542,7 +559,10 @@ class DistributedPGO:
     schedule = "greedy"   : the reference's synchronous driver (one agent per round, argmax of the per-agent
                             gradient norm; examples/MultiRobotExample.cpp:229-334) -- parity mode;
              = "coloured" : all agents of one colour class per round (concurrent, same RBCD semantics);
-             = "parallel" : every agent every round on the neighbours' previous poses.
+             = "parallel" : every agent every round on the neighbours' previous poses;
+             = "greedy_set": the greedy rule applied to as many agents as RBCD allows: each round a maximal set of agents
+                            that share no edge, taken in decreasing block gradient norm (greedy_independent_set), chosen on
+                            the device from the team status taken before the round, so rounds need no host synchronisation.
     Per round: G rebuild from the gathered public poses -> local optimise -> pack -> ONE all-gather; with evaluation, the
     team status (one status launch per GPU, one all-gather of the records) gives the central cost / gradient norm /
     selection.
@@ -573,6 +593,11 @@ class DistributedPGO:
         one exact block update and the momentum follows the rounds (schedule="coloured" only)."""
         import torch
         check_accel_arguments(schedule, momentum_blocks)
+        if schedule not in ("greedy", "coloured", "parallel", "greedy_set"):
+            raise ValueError("schedule must be 'greedy', 'coloured', 'parallel' or 'greedy_set'")
+        if schedule == "greedy_set" and acceleration:
+            raise ValueError("acceleration=True is not supported with schedule='greedy_set': the Nesterov momentum assumes a "
+                             "fixed block set per round")
         self.momentum_blocks = momentum_blocks
         self.acceleration, self.restart_interval = bool(acceleration), int(restart_interval)
         self.torch = torch
@@ -600,7 +625,8 @@ class DistributedPGO:
         per_rank = k // self.world
         self.local_ids = list(range(rank * per_rank, (rank + 1) * per_rank)) if self.distributed else list(range(k))
         if concurrent is None:
-            concurrent = auto_concurrent(self.colour, k, self.world, schedule, self.acceleration and momentum_blocks == "agents")
+            concurrent = auto_concurrent(self.colour, k, self.world, schedule, self.acceleration and momentum_blocks == "agents",
+                                         [t["neighbors"] for t in self.plan.tables])
         if concurrent and schedule == "parallel":
             raise ValueError("concurrent rounds are implemented for the greedy and coloured schedules")
         self.concurrent = bool(concurrent)
@@ -692,6 +718,17 @@ class DistributedPGO:
         self.selected = [0]
         self.round = 0
         self._gathered_current = False       # `gathered` holds every agent's current public tiles
+        self._records_current = False        # the status buffers hold every agent's record of the current iterates
+        if schedule == "greedy_set":
+            nb = [self.plan.tables[a]["neighbors"] for a in range(k)]
+            ptr = np.concatenate([[0], np.cumsum([len(x) for x in nb])]).astype(np.int32)
+            adj = np.array([b for x in nb for b in x] or [0], dtype=np.int32)
+            lead = self.agents[self.local_ids[0]].mProblem
+            capi.check(lead._lib.dpgo_agents_set_agent_graph(lead._h, k, capi.iptr(ptr), capi.iptr(adj)))
+            ids = self.local_ids
+            self._sel_args = ((C.c_void_p * len(ids))(*[self.agents[a].mProblem._h for a in ids]),
+                              np.array(ids, dtype=np.int32),
+                              (C.c_void_p * len(ids))(*[C.c_void_p(self.send[a].data_ptr()) for a in ids]))
 
     # -- distributed initialisation: alignment waves (ref src/PGOAgent.cpp:369-440, examples/MultiRobotExample.cpp:245-256) --
     def _align_waves(self) -> List[Dict[str, int]]:
@@ -757,6 +794,7 @@ class DistributedPGO:
         """G rebuild -> RTR step -> pack for every active local agent with one C call (thread-block cluster agents side by
         side on their own streams, full-grid agents one after the other); then, with publish, the all-gather of the new
         public tiles.  The gathered tiles must be current.  Asynchronous (no host synchronisation)."""
+        self._records_current = False
         mine = [a for a in self.local_ids if a in active]
         lib = self.agents[self.local_ids[0]].mProblem._lib
         if mine:
@@ -770,7 +808,44 @@ class DistributedPGO:
 
     _round_concurrent = _round               # bench.py times its rounds through this name
 
+    def _select_round(self) -> None:
+        """One greedy_set round: the team status of the current iterates on the device (skipped when it is current; multi-rank:
+        one all-gather of the records), then one dpgo_agents_select_round_async call (selection, then the gated G rebuild ->
+        step -> pack of every local agent), then the all-gather of the new public tiles.  No host synchronisation."""
+        if not self._gathered_current:
+            self.exchange(build=False)
+            self._gathered_current = True
+        if not self._records_current:
+            self._status_device()
+        hs, idx, sd = self._sel_args
+        lib = self.agents[self.local_ids[0]].mProblem._lib
+        capi.check(lib.dpgo_agents_select_round_async(hs, len(self.local_ids), capi.iptr(idx),
+                                                      C.byref(self.agents[self.local_ids[0]].opt._p),
+                                                      C.c_void_p(self._status_all.data_ptr()),
+                                                      C.c_void_p(self.gathered.data_ptr()), self.k * self.plan.pmax, sd,
+                                                      C.c_void_p(self._main_stream)))
+        if self.distributed:
+            self.dist.all_gather_into_tensor(self.gathered, self.send_all)
+        self._records_current = False
+
+    def selection_log(self, first: int = 0, count: Optional[int] = None) -> List[List[int]]:
+        """The agents each greedy_set round selected (sorted), rounds first .. first + count - 1 (None: to the last round
+        issued).  Synchronises the device."""
+        if self.schedule != "greedy_set":
+            raise ValueError("selection_log() needs schedule='greedy_set'")
+        lead = self.agents[self.local_ids[0]].mProblem
+        total = C.c_int64(0)
+        capi.check(lead._lib.dpgo_agents_selection_log(lead._h, 0, 0, None, C.byref(total)))
+        count = max(0, total.value - first) if count is None else max(0, min(count, total.value - first))
+        buf = np.zeros(max(count, 1) * self.k, dtype=np.uint8)
+        if count:
+            capi.check(lead._lib.dpgo_agents_selection_log(lead._h, first, count,
+                                                           buf.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(total)))
+        return [[int(a) for a in np.flatnonzero(row)] for row in buf[:count * self.k].reshape(count, self.k)]
+
     def _active(self) -> List[int]:
+        if self.schedule == "greedy_set":
+            raise ValueError("the greedy_set schedule selects on the device: drive it with step() or solve()")
         if self.schedule == "greedy":
             return list(self.selected)
         if self.schedule == "coloured":
@@ -814,10 +889,20 @@ class DistributedPGO:
         for a in mine:
             self.agents[a].mIterationNumber += 1
         self._gathered_current = False       # the gathered X tiles predate the active agents' steps
+        self._records_current = False
         return active
 
     def step(self, evaluate: bool = True) -> Optional[RoundStats]:
-        """One round, then (optionally) the team status: central cost, gradient norm and the greedy selection."""
+        """One round, then (optionally) the team status: central cost, gradient norm and the greedy selection.  Under the
+        greedy_set schedule the round's agents are read from the selection log, and only when evaluate is True."""
+        if self.schedule == "greedy_set":
+            with self.torch.cuda.stream(self._runner_stream()):
+                self._select_round()
+            self.round += 1
+            if not evaluate:
+                return None
+            st = self.status()
+            return RoundStats(st.cost, st.gradnorm, self.selection_log(self.round - 1, 1)[0])
         if self.acceleration:
             active = self._step_accelerated()
         else:
@@ -854,6 +939,7 @@ class DistributedPGO:
         memory and packs its public tiles, the all-gather publishes them, one call steps the active agents, one call reads
         their iterates back, then one synchronisation (the calls are replayed as CUDA graphs when they can be).  ag.X (host)
         is the state between rounds."""
+        self._records_current = False
         hx = self._host_buffers()
         for a in self.local_ids:
             if hx[a] is not self.agents[a].X:
@@ -892,6 +978,7 @@ class DistributedPGO:
         getSharedPoseDict -> (all-gather of the host-packed public poses) -> updateNeighborPoses -> iterate(), i.e.
         per active agent H2D of X and G, one persistent kernel, D2H of X.  Used for the end-to-end number."""
         torch = self.torch
+        self._records_current = False
         dh, ts = self.d + 1, self.r * (self.d + 1)
         if not hasattr(self, "_host_send"):
             self._host_send = torch.zeros(len(self.local_ids) * self.slot_elems, dtype=torch.float64).pin_memory()
@@ -967,6 +1054,12 @@ class DistributedPGO:
             self._gathered_current = True
 
     def _status(self) -> TeamStatus:
+        self._status_device()
+        return team_status(self._status_all.cpu().numpy().reshape(self.k, capi.STATUS_DOUBLES))
+
+    def _status_device(self) -> None:
+        """Every agent's status record into _status_all on the device (multi-rank: one all-gather of the records), on the
+        runner's stream, without a host synchronisation."""
         self._refresh_G()
         torch, S = self.torch, capi.STATUS_DOUBLES
         if not hasattr(self, "_status_local"):
@@ -980,7 +1073,7 @@ class DistributedPGO:
                                                 C.c_void_p(self._status_local.data_ptr()), C.c_void_p(self._main_stream)))
         if self.distributed:
             self.dist.all_gather_into_tensor(self._status_all, self._status_local)
-        return team_status(self._status_all.cpu().numpy().reshape(self.k, S))
+        self._records_current = True
 
     def _select(self, st: TeamStatus) -> None:
         if self.schedule == "greedy":

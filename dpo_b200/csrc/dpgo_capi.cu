@@ -128,6 +128,16 @@ struct dpgo_problem {
   unsigned *d_status_ticket = nullptr;
   std::vector<JobTable<dpgo::StatusJob>> status_tables;  // job tables of dpgo_agents_status_async, kept by the call's first agent
   double *d_anchor = nullptr, *d_traj = nullptr;   // dpgo_agent_trajectory_global
+  // greedy independent-set rounds (dpgo_select.cu), kept by the first agent of a runner on a GPU: the agent graph in CSR
+  // form, the round's k-byte mask, and the selection log (sel_cap rounds of k bytes; sel_rounds issued, the device counts
+  // its own rows).  A grown log retires the old buffer until the next read of the log or the handle's destruction.
+  int sel_k = 0;
+  int *d_sel_ptr = nullptr, *d_sel_adj = nullptr;
+  unsigned char *d_sel_mask = nullptr, *d_sel_log = nullptr;
+  unsigned long long *d_sel_count = nullptr;
+  long long sel_rounds = 0, sel_cap = 0;
+  std::vector<unsigned char *> sel_retired;
+  const unsigned char *gate = nullptr;     // set for the duration of a gated round: this agent's byte of the mask
 
   size_t vec_bytes() const { return sizeof(double) * (size_t)r * (size_t)N; }
 };
@@ -170,6 +180,7 @@ void fill_kparams(const dpgo_problem *p, dpgo::KParams &kp, int op, const dpgo_o
   kp.smem_doubles = 0;
   kp.phase_ns = p->d_phase_ns;
   kp.opt_record = p->d_opt_record;
+  kp.gate = p->gate;
   kp.prm = prm;
   kp.result = p->d_result;
 }
@@ -734,6 +745,9 @@ int dpgo_problem_destroy(dpgo_problem_t *p) {
   if (p->h_result) cudaFreeHost(p->h_result);
   for (auto &g : p->round_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   p->round_graphs.clear();
+  free_dev(p->d_sel_ptr); free_dev(p->d_sel_adj); free_dev(p->d_sel_mask); free_dev(p->d_sel_log); free_dev(p->d_sel_count);
+  for (auto *b : p->sel_retired) cudaFree(b);
+  p->sel_retired.clear();
   if (p->ev_done) cudaEventDestroy(p->ev_done);
   if (p->ev_fork) cudaEventDestroy(p->ev_fork);
   if (p->ev_align) cudaEventDestroy(p->ev_align);
@@ -1424,7 +1438,7 @@ int dpgo_agent_set_public_poses(dpgo_problem_t *p, int num_public, const int32_t
 int dpgo_agent_pack_public(dpgo_problem_t *p, double *send_dev) {
   DPGO_CHECK_HANDLE(p);
   DPGO_REQUIRE(send_dev || p->num_public == 0, DPGO_ERR_INVALID_ARG, "null send buffer");
-  DPGO_CUDA(dpgo::launch_pack_tiles(p->ts, p->num_public, p->d_public, p->d_vec[dpgo::V_X0], send_dev, p->stream));
+  DPGO_CUDA(dpgo::launch_pack_tiles(p->ts, p->num_public, p->d_public, p->d_vec[dpgo::V_X0], send_dev, p->stream, p->gate));
   return DPGO_OK;
 }
 
@@ -1493,7 +1507,7 @@ int dpgo_agent_build_G(dpgo_problem_t *p, const double *gathered_dev, int64_t nu
   }
   if (p->num_edges)
     DPGO_CUDA(dpgo::launch_build_G(p->r, p->dh, p->num_shared_poses, p->d_pose_ids, p->d_pose_ptr, p->d_edge_slot,
-                                   p->d_edge_out, p->d_edge_T, p->d_edge_om, gathered_dev, p->d_G, p->stream));
+                                   p->d_edge_out, p->d_edge_T, p->d_edge_om, gathered_dev, p->d_G, p->stream, p->gate));
   return DPGO_OK;
 }
 
@@ -2195,6 +2209,121 @@ int dpgo_agents_accel_round_async(dpgo_problem_t *const *agents, int num_active,
   key.push_back((uint64_t)(uintptr_t)gathered_dev);
   key.push_back((uint64_t)(uintptr_t)gathered_aux_dev);
   return replay_or_issue(agents[0], key, main, issue);
+}
+
+// ---- greedy independent-set rounds (dpgo_select.cu) -----------------------------------------------------------------------
+int dpgo_agents_set_agent_graph(dpgo_problem_t *lead, int num_agents, const int32_t *adj_ptr, const int32_t *adj) {
+  DPGO_TRY(require_device());
+  DPGO_CHECK_HANDLE(lead);
+  DPGO_REQUIRE(num_agents >= 1 && num_agents <= dpgo::SELECT_MAX_AGENTS && adj_ptr, DPGO_ERR_INVALID_ARG,
+               "the agent graph needs 1 to 1024 agents and a row pointer");
+  DPGO_REQUIRE(adj_ptr[0] == 0 && (adj_ptr[num_agents] == 0 || adj), DPGO_ERR_INVALID_ARG, "bad agent graph arrays");
+  for (int a = 0; a < num_agents; ++a) {
+    DPGO_REQUIRE(adj_ptr[a + 1] >= adj_ptr[a], DPGO_ERR_INVALID_ARG, "the agent graph's row pointer must not decrease");
+    for (int e = adj_ptr[a]; e < adj_ptr[a + 1]; ++e)
+      DPGO_REQUIRE(adj[e] >= 0 && adj[e] < num_agents && adj[e] != a, DPGO_ERR_INVALID_ARG,
+                   "agent graph neighbour out of range or a self loop");
+  }
+  DPGO_CUDA(cudaSetDevice(lead->device));
+  DPGO_CUDA(cudaDeviceSynchronize());                       // the old buffers may still be read by a round in flight
+  free_dev(lead->d_sel_ptr); free_dev(lead->d_sel_adj); free_dev(lead->d_sel_mask); free_dev(lead->d_sel_log);
+  for (auto *b : lead->sel_retired) cudaFree(b);
+  lead->sel_retired.clear();
+  const int m = adj_ptr[num_agents];
+  DPGO_CUDA(cudaMalloc(&lead->d_sel_ptr, sizeof(int) * (size_t)(num_agents + 1)));
+  DPGO_CUDA(cudaMalloc(&lead->d_sel_adj, sizeof(int) * (size_t)std::max(m, 1)));
+  DPGO_CUDA(cudaMalloc(&lead->d_sel_mask, (size_t)num_agents));
+  if (!lead->d_sel_count) DPGO_CUDA(cudaMalloc(&lead->d_sel_count, sizeof(unsigned long long)));
+  DPGO_CUDA(cudaMemcpy(lead->d_sel_ptr, adj_ptr, sizeof(int) * (size_t)(num_agents + 1), cudaMemcpyHostToDevice));
+  if (m) DPGO_CUDA(cudaMemcpy(lead->d_sel_adj, adj, sizeof(int) * (size_t)m, cudaMemcpyHostToDevice));
+  DPGO_CUDA(cudaMemset(lead->d_sel_count, 0, sizeof(unsigned long long)));
+  lead->sel_k = num_agents;
+  lead->sel_rounds = lead->sel_cap = 0;
+  ++lead->generation;
+  return DPGO_OK;
+}
+
+namespace {
+struct GateSet {                           // every agent of a round reads its byte of the mask for the duration of a call
+  dpgo_problem_t *const *agents; int count;
+  GateSet(dpgo_problem_t *const *a, int n, const unsigned char *mask, const int32_t *index) : agents(a), count(n) {
+    for (int i = 0; i < n; ++i) a[i]->gate = mask + index[i];
+  }
+  ~GateSet() { for (int i = 0; i < count; ++i) agents[i]->gate = nullptr; }
+};
+}  // namespace
+
+// One greedy independent-set round of the agents of one GPU: the selection from the gathered status records, then every
+// listed agent's G rebuild -> step -> pack, each kernel gated by the agent's byte of the mask.  The selected agents share
+// no edge, so packs into an aliased gathered buffer cannot race with another selected agent's G rebuild.
+int dpgo_agents_select_round_async(dpgo_problem_t *const *agents, int count, const int32_t *agent_index,
+                                   const dpgo_opt_params_t *params, const double *records_dev, const double *gathered_dev,
+                                   int64_t num_slots, double *const *send_dev, void *stream) {
+  DPGO_TRY(require_device());
+  DPGO_REQUIRE(count > 0 && agents && agent_index && params && records_dev && send_dev, DPGO_ERR_INVALID_ARG, "bad arguments");
+  dpgo_problem *lead = agents[0];
+  DPGO_CHECK_HANDLE(lead);
+  DPGO_REQUIRE(lead->sel_k > 0, DPGO_ERR_STATE, "dpgo_agents_set_agent_graph has not been called for the first agent");
+  std::vector<char> seen((size_t)lead->sel_k, 0);
+  for (int i = 0; i < count; ++i) {
+    DPGO_REQUIRE(agent_index[i] >= 0 && agent_index[i] < lead->sel_k && !seen[(size_t)agent_index[i]], DPGO_ERR_INVALID_ARG,
+                 "agent indices must be distinct and below the agent graph's size");
+    seen[(size_t)agent_index[i]] = 1;
+  }
+  cudaStream_t main = nullptr;
+  bool graph = false;
+  DPGO_TRY(round_preamble(agents, count, params, stream, main, graph));
+  if (lead->sel_rounds == lead->sel_cap) {                  // the log doubles; the old buffer is freed after the next read
+    const long long cap = std::max(64LL, 2 * lead->sel_cap);
+    unsigned char *grown = nullptr;
+    DPGO_CUDA(cudaMalloc(&grown, (size_t)cap * lead->sel_k));
+    if (lead->d_sel_log) {
+      DPGO_CUDA(cudaMemcpyAsync(grown, lead->d_sel_log, (size_t)lead->sel_rounds * lead->sel_k, cudaMemcpyDeviceToDevice, main));
+      lead->sel_retired.push_back(lead->d_sel_log);
+    }
+    lead->d_sel_log = grown;
+    lead->sel_cap = cap;
+  }
+  auto issue = [&]() -> int {
+    DPGO_CUDA(dpgo::launch_select_independent(lead->sel_k, records_dev, lead->d_sel_ptr, lead->d_sel_adj, lead->d_sel_mask,
+                                              lead->d_sel_log, lead->d_sel_count, main));
+    GateSet gates(agents, count, lead->d_sel_mask, agent_index);
+    return issue_round(agents, count, params, gathered_dev, num_slots, send_dev, main, 0);
+  };
+  int rc = DPGO_OK;
+  if (!graph) {
+    rc = issue();
+  } else {
+    std::vector<uint64_t> key = round_key(0x73656c0000ull, agents, count, params, main, num_slots);   // "sel"
+    for (int i = 0; i < count; ++i) {
+      key.push_back((uint64_t)(uintptr_t)send_dev[i]);
+      key.push_back((uint64_t)agent_index[i]);
+    }
+    key.push_back((uint64_t)(uintptr_t)gathered_dev);
+    key.push_back((uint64_t)(uintptr_t)records_dev);
+    key.push_back((uint64_t)(uintptr_t)lead->d_sel_log);
+    rc = replay_or_issue(lead, key, main, issue);
+  }
+  if (rc == DPGO_OK) ++lead->sel_rounds;
+  return rc;
+}
+
+int dpgo_agents_selection_log(dpgo_problem_t *lead, int64_t first_round, int64_t max_rounds, uint8_t *out_host,
+                              int64_t *total_rounds) {
+  DPGO_TRY(require_device());
+  DPGO_CHECK_HANDLE(lead);
+  DPGO_REQUIRE(lead->sel_k > 0, DPGO_ERR_STATE, "dpgo_agents_set_agent_graph has not been called for this agent");
+  DPGO_REQUIRE(first_round >= 0 && max_rounds >= 0 && (max_rounds == 0 || out_host), DPGO_ERR_INVALID_ARG, "bad log range");
+  DPGO_CUDA(cudaSetDevice(lead->device));
+  DPGO_CUDA(cudaDeviceSynchronize());                       // the log is written on the streams of the round calls
+  for (auto *b : lead->sel_retired) cudaFree(b);
+  lead->sel_retired.clear();
+  if (total_rounds) *total_rounds = lead->sel_rounds;
+  const int64_t rows = std::max<int64_t>(0, std::min<int64_t>(max_rounds, lead->sel_rounds - first_round));
+  if (rows > 0)
+    DPGO_CUDA(cudaMemcpy(out_host, lead->d_sel_log + (size_t)first_round * lead->sel_k, (size_t)rows * lead->sel_k,
+                         cudaMemcpyDeviceToHost));
+  return DPGO_OK;
 }
 
 int dpgo_agent_accel_state(dpgo_problem_t *p, double *out3) {

@@ -1011,6 +1011,9 @@ __device__ __forceinline__ void zero(double (&acc)[NRED]) {
 // The persistent kernel
 // ---------------------------------------------------------------------------------------------
 template <int R, int DH> __global__ void __launch_bounds__(OPT_THREADS, 1) k_optimize(const KParams kp) {
+  // a gated-off agent (selection of dpgo_agents_select_round_async): every CTA reads the same flag before anything else,
+  // so the whole grid returns and no barrier, result or opt_record is touched
+  if (kp.gate != nullptr && __ldg(kp.gate) == 0) return;
   extern __shared__ double smem[];
   BlockCtx bc;
   bc.sm_warp = smem;
@@ -1373,9 +1376,9 @@ template <int R, int DH> __global__ void k_stiefel_project(int n, const double *
 // PGOAgent::constructGMatrix :783-859)
 // ---------------------------------------------------------------------------------------------
 __global__ void k_pack_tiles(int ts, int count, const int *__restrict__ pose, const double *__restrict__ X,
-                             double *__restrict__ out) {
+                             double *__restrict__ out, const unsigned char *__restrict__ gate) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= count * ts) return;
+  if (t >= count * ts || (gate != nullptr && *gate == 0)) return;
   const int s = t / ts, e = t - s * ts;
   out[t] = X[(size_t)pose[s] * ts + e];
 }
@@ -1386,10 +1389,11 @@ template <int R, int DH>
 __global__ void k_build_G(int nposes, const int *__restrict__ pose_ids, const int *__restrict__ pose_ptr,
                           const int *__restrict__ edge_slot, const int *__restrict__ edge_out,
                           const double *__restrict__ edge_T, const double *__restrict__ edge_om,
-                          const double *__restrict__ gathered, double *__restrict__ G) {
+                          const double *__restrict__ gathered, double *__restrict__ G,
+                          const unsigned char *__restrict__ gate) {
   constexpr int TS = R * DH;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= nposes * TS) return;
+  if (t >= nposes * TS || (gate != nullptr && *gate == 0)) return;
   const int pi = t / TS, e = t - pi * TS;
   const int c = e / R, a = e - c * R;          // element (a, c) of the tile
   double acc = 0.0;
@@ -1625,10 +1629,11 @@ cudaError_t launch_stiefel_project(int r, int dh, int n, const double *M, double
   return cudaGetLastError();
 }
 
-cudaError_t launch_pack_tiles(int ts, int count, const int *pose, const double *X, double *out, cudaStream_t stream) {
+cudaError_t launch_pack_tiles(int ts, int count, const int *pose, const double *X, double *out, cudaStream_t stream,
+                              const unsigned char *gate) {
   if (count <= 0) return cudaSuccess;
   const int total = count * ts;
-  k_pack_tiles<<<(total + 255) / 256, 256, 0, stream>>>(ts, count, pose, X, out);
+  k_pack_tiles<<<(total + 255) / 256, 256, 0, stream>>>(ts, count, pose, X, out, gate);
   return cudaGetLastError();
 }
 
@@ -1688,13 +1693,13 @@ cudaError_t launch_bsr_to_dense(int n, int dh, int64_t nb, const int *rowptr, co
 
 cudaError_t launch_build_G(int r, int dh, int nposes, const int *pose_ids, const int *pose_ptr, const int *edge_slot,
                            const int *edge_out, const double *edge_T, const double *edge_om, const double *gathered,
-                           double *G, cudaStream_t stream) {
+                           double *G, cudaStream_t stream, const unsigned char *gate) {
   if (nposes <= 0) return cudaSuccess;
   bool ok = false;
   DPGO_DISPATCH(r, dh, {
     const int total = nposes * R * DH;
     k_build_G<R, DH><<<(total + 127) / 128, 128, 0, stream>>>(nposes, pose_ids, pose_ptr, edge_slot, edge_out, edge_T,
-                                                              edge_om, gathered, G);
+                                                              edge_om, gathered, G, gate);
     ok = true;
   });
   if (!ok) return cudaErrorInvalidValue;

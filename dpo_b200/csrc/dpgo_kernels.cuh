@@ -93,6 +93,7 @@ struct KParams {
   int smem_doubles;      // dynamic shared memory of this launch, in doubles
   unsigned long long *phase_ns; // diagnostic (nullable): per phase kind, ns seen by CTA 0 (dpgo_debug_phase_times)
   double *opt_record;    // 2 doubles: relative change of the last optimising call, optimising calls so far (OP_OPTIMIZE only)
+  const unsigned char *gate;   // nullable: the agent's byte of a selection mask; 0 = the launch returns at entry
 };
 
 // Instantiations of the compiled (r, d+1) pairs (every pair dpgo_problem_create accepts); R and DH are constexpr in the body.
@@ -127,10 +128,12 @@ int optimize_max_grid(int r, int dh, int device);   // co-resident CTA count for
 int optimize_max_cluster(int r, int dh, int device); // largest single-cluster grid (16, 8 or 0) the kernel can be launched with
 cudaError_t launch_stiefel_project(int r, int dh, int n, const double *M, double *out, cudaStream_t stream, double c0 = 1.0,
                                    const double *B = nullptr, double c1 = 0.0, const double *C = nullptr, double c2 = 0.0);
-cudaError_t launch_pack_tiles(int ts, int count, const int *pose, const double *X, double *out, cudaStream_t stream);
+// gate (nullable): the agent's byte of a selection mask; the launch does nothing when it is 0
+cudaError_t launch_pack_tiles(int ts, int count, const int *pose, const double *X, double *out, cudaStream_t stream,
+                              const unsigned char *gate = nullptr);
 cudaError_t launch_build_G(int r, int dh, int nposes, const int *pose_ids, const int *pose_ptr, const int *edge_slot,
                            const int *edge_out, const double *edge_T, const double *edge_om, const double *gathered,
-                           double *G, cudaStream_t stream);
+                           double *G, cudaStream_t stream, const unsigned char *gate = nullptr);
 cudaError_t launch_assemble_Q(int64_t nb, const int *cptr, const int2 *contrib, const double *eT, const double *eom, const double *ew,
                               const double *sblk, double *bval, cudaStream_t stream);
 cudaError_t launch_edge_weights(int r, int dh, int64_t m, const int *p1, const int *p2, const double *eT, const double *eom,
@@ -187,6 +190,14 @@ __host__ __device__ inline int status_ctas(int n) { return (n + STATUS_ROWS - 1)
 cudaError_t launch_agents_status(int r, int dh, int njobs, int total_ctas, const StatusJob *jobs, cudaStream_t stream);
 // T = [proj_SO(d)(Ya^T X_i R-block), Ya^T X_i t - Ya^T pa] per pose (d x (d+1)n column-major); anchor = [Ya pa], r x (d+1)
 cudaError_t launch_trajectory_global(int r, int dh, int n, const double *anchor, const double *X, double *T, cudaStream_t stream);
+
+// ---- greedy independent-set selection (dpgo_select.cu) ----
+// One CTA: rank of every agent by records[a * DPGO_STATUS_DOUBLES + 2] (|rgrad|^2) decreasing, ties by lower id; then the
+// greedy walk in that order over the agent graph (CSR adj_ptr / adj): an agent is taken unless a neighbour already is.
+// mask[a] = 1 for a taken agent; the mask is also appended to log + (*log_count) * k, and *log_count is incremented.
+constexpr int SELECT_MAX_AGENTS = 1024;
+cudaError_t launch_select_independent(int k, const double *records, const int *adj_ptr, const int *adj, unsigned char *mask,
+                                      unsigned char *log, unsigned long long *log_count, cudaStream_t stream);
 
 // ---- accelerated rounds (dpgo_accel.cu) ----
 // Momentum record of an agent: {gamma, alpha, iterations, gamma of the last round}; the last slot is the gamma the round's

@@ -56,7 +56,9 @@ struct DeviceRBCD::Impl {
   bool concurrent = false;         // active agents of a GPU side by side (cluster launches, own streams)
   bool gatheredCurrent = false;    // the gathered buffers hold every agent's current public tiles
   std::vector<double *> statusDev; // per GPU: its agents' status records
+  std::vector<double *> statusAll; // per GPU: every agent's record (N == 1: statusDev), the greedy_set selection's input
   double *statusHost = nullptr;    // pinned, all agents' records in agent order
+  bool recordsCurrent = false;     // statusAll holds the records of the current iterates
 
   // one ncclAllGather group: every GPU's send buffer into every GPU's gathered buffer (one GPU packs straight into it)
   void allGather(const std::vector<double *> &sendBuf, const std::vector<double *> &gatheredBuf) {
@@ -65,6 +67,18 @@ struct DeviceRBCD::Impl {
     for (unsigned g = 0; g < N; ++g) {
       check(dpgo_device_set((int)g), "dpgo_device_set");
       checkNccl(ncclAllGather(sendBuf[g], gatheredBuf[g], (size_t)perGpu * pmax * ts, ncclDouble, comm[g], (cudaStream_t)stream[g]),
+                "ncclAllGather");
+    }
+    checkNccl(ncclGroupEnd(), "ncclGroupEnd");
+  }
+  // one ncclAllGather group of the status records: every GPU's agents' records into every GPU's copy of all of them
+  void allGatherRecords() {
+    if (N == 1) return;
+    checkNccl(ncclGroupStart(), "ncclGroupStart");
+    for (unsigned g = 0; g < N; ++g) {
+      check(dpgo_device_set((int)g), "dpgo_device_set");
+      checkNccl(ncclAllGather(statusDev[g], statusAll[g], (size_t)perGpu * DPGO_STATUS_DOUBLES, ncclDouble, comm[g],
+                              (cudaStream_t)stream[g]),
                 "ncclAllGather");
     }
     checkNccl(ncclGroupEnd(), "ncclGroupEnd");
@@ -84,8 +98,11 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
   I.N = std::max(1u, opt.gpus);
   I.n = n;
   I.schedule = opt.schedule;
-  if (I.schedule != "greedy" && I.schedule != "coloured" && I.schedule != "parallel")
-    throw std::runtime_error("DeviceRBCD: schedule must be greedy, coloured or parallel");
+  if (I.schedule != "greedy" && I.schedule != "coloured" && I.schedule != "parallel" && I.schedule != "greedy_set")
+    throw std::runtime_error("DeviceRBCD: schedule must be greedy, coloured, parallel or greedy_set");
+  if (I.schedule == "greedy_set" && opt.acceleration)
+    throw std::invalid_argument("DeviceRBCD: acceleration is not supported with the greedy_set schedule: the Nesterov momentum "
+                                "assumes a fixed block set per round");
   if (I.K == 0 || n / I.K == 0) throw std::runtime_error("DeviceRBCD: more agents than poses");
   const bool distributed = (opt.initialization == "distributed");
   if (!distributed && opt.initialization != "central")
@@ -161,6 +178,11 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
           for (unsigned a = g * I.perGpu; a < (g + 1) * I.perGpu; ++a) cnt += (mColour[a] == c);
           most = std::max(most, cnt);
         }
+    if (I.schedule == "greedy_set")                      // some GPU hosts two agents that are not neighbours
+      for (unsigned g = 0; g < I.N; ++g)
+        for (unsigned a = g * I.perGpu; a < (g + 1) * I.perGpu; ++a)
+          for (unsigned b = a + 1; b < (g + 1) * I.perGpu; ++b)
+            if (!std::binary_search(I.neighbors[a].begin(), I.neighbors[a].end(), b)) most = 2;
     const bool agentMomentum = opt.acceleration && opt.momentumBlocks == "agents";
     I.concurrent = opt.concurrent < 0 ? (most >= 2 && !agentMomentum) : (opt.concurrent != 0);
     if (I.concurrent && I.schedule == "parallel")
@@ -343,6 +365,16 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
       }
     }
   }
+  if (I.schedule == "greedy_set") {                     // the agent graph in CSR form, with each GPU's first agent
+    std::vector<int32_t> ptr{0}, adj;
+    for (unsigned a = 0; a < K; ++a) {
+      for (unsigned b : I.neighbors[a]) adj.push_back((int32_t)b);
+      ptr.push_back((int32_t)adj.size());
+    }
+    for (unsigned g = 0; g < I.N; ++g)
+      check(dpgo_agents_set_agent_graph(I.h[(size_t)g * I.perGpu], (int)K, ptr.data(), adj.data()),
+            "dpgo_agents_set_agent_graph");
+  }
   dpgo_opt_params_default(&I.prm);
   I.prm.algorithm = (opt.algorithm == ROPTALG::RTR) ? DPGO_ALG_RTR : DPGO_ALG_RGD;
   I.prm.precond = (int)opt.preconditioner;
@@ -367,6 +399,7 @@ DeviceRBCD::~DeviceRBCD() {
       if (I.gatheredAux[g]) dpgo_device_free((int)g, I.gatheredAux[g]);
     }
     if (g < I.statusDev.size() && I.statusDev[g]) dpgo_device_free((int)g, I.statusDev[g]);
+    if (I.N > 1 && g < I.statusAll.size() && I.statusAll[g]) dpgo_device_free((int)g, I.statusAll[g]);
     if (I.stream[g]) dpgo_stream_destroy((int)g, I.stream[g]);
   }
   dpgo_host_free_pinned(I.statusHost);
@@ -494,6 +527,11 @@ void DeviceRBCD::roundAccelerated(const std::vector<unsigned> &active) {
 // (G rebuild -> RTR step -> pack per active agent), then the all-gather that publishes the new public tiles.
 std::vector<unsigned> DeviceRBCD::issueRound() {
   Impl &I = *impl;
+  if (I.schedule == "greedy_set") {
+    selectRound();
+    return {};
+  }
+  I.recordsCurrent = false;
   const std::vector<unsigned> active = activeSet(I.schedule, I.K, I.selected, mRound, mColour, mNumColours);
   if (I.acceleration) {
     roundAccelerated(active);
@@ -519,6 +557,48 @@ std::vector<unsigned> DeviceRBCD::issueRound() {
   return active;
 }
 
+// one greedy_set round: the status records of the current iterates on every GPU (skipped when current; N > 1: one
+// all-gather group of the records), per GPU ONE dpgo_agents_select_round_async call (selection on the device, then the
+// gated G rebuild -> step -> pack of every agent of the GPU), then the all-gather of the new public tiles.  No host
+// synchronisation: the round's agents are in the selection log.
+void DeviceRBCD::selectRound() {
+  Impl &I = *impl;
+  if (!I.gatheredCurrent) { exchange(); I.gatheredCurrent = true; }
+  if (!I.recordsCurrent) statusDevice();
+  const size_t slotElems = (size_t)I.pmax * I.ts;
+  for (unsigned g = 0; g < I.N; ++g) {
+    std::vector<dpgo_problem *> hs;
+    std::vector<int32_t> idx;
+    std::vector<double *> dst;
+    for (unsigned a = g * I.perGpu; a < (g + 1) * I.perGpu; ++a) {
+      hs.push_back(I.h[a]);
+      idx.push_back((int32_t)a);
+      dst.push_back((I.N == 1) ? I.gathered[g] + a * slotElems : I.send[g] + (a % I.perGpu) * slotElems);
+    }
+    check(dpgo_agents_select_round_async(hs.data(), (int)hs.size(), idx.data(), &I.prm, I.statusAll[g], I.gathered[g],
+                                         (int64_t)I.K * I.pmax, dst.data(), I.stream[g]),
+          "dpgo_agents_select_round_async");
+  }
+  I.allGather(I.send, I.gathered);
+  I.recordsCurrent = false;
+  ++mRound;
+}
+
+std::vector<std::vector<unsigned>> DeviceRBCD::selectionLog(unsigned first, unsigned count) {
+  Impl &I = *impl;
+  if (I.schedule != "greedy_set") throw std::invalid_argument("DeviceRBCD::selectionLog: needs the greedy_set schedule");
+  int64_t total = 0;
+  check(dpgo_agents_selection_log(I.h[0], 0, 0, nullptr, &total), "dpgo_agents_selection_log");
+  const int64_t rows = std::max<int64_t>(0, std::min<int64_t>(count, total - (int64_t)first));
+  std::vector<uint8_t> buf((size_t)std::max<int64_t>(rows, 1) * I.K);
+  if (rows > 0) check(dpgo_agents_selection_log(I.h[0], first, rows, buf.data(), &total), "dpgo_agents_selection_log");
+  std::vector<std::vector<unsigned>> out((size_t)rows);
+  for (int64_t q = 0; q < rows; ++q)
+    for (unsigned a = 0; a < I.K; ++a)
+      if (buf[(size_t)q * I.K + a]) out[(size_t)q].push_back(a);
+  return out;
+}
+
 void DeviceRBCD::runRounds(unsigned rounds) {
   for (unsigned it = 0; it < rounds; ++it) issueRound();
 }
@@ -531,6 +611,7 @@ DeviceRBCDStats DeviceRBCD::step(bool evaluate) {
   const DeviceRBCDStatus s = status();
   st.cost = s.cost;
   st.gradnorm = s.gradnorm;
+  if (I.schedule == "greedy_set") st.active = selectionLog(mRound - 1, 1)[0];
   if (I.schedule == "greedy") I.selected = greedySelection(I.selected, s, I.K, !I.neighbors[I.selected].empty());
   return st;
 }
@@ -550,6 +631,27 @@ Matrix DeviceRBCD::assemble() {
 DeviceRBCDStatus DeviceRBCD::status() {
   Impl &I = *impl;
   constexpr unsigned S = DPGO_STATUS_DOUBLES;
+  statusDevice();
+  for (unsigned g = 0; g < I.N; ++g)
+    check(dpgo_copy_to_host_async((int)g, I.statusHost + (size_t)g * I.perGpu * S, I.statusDev[g], sizeof(double) * S * I.perGpu,
+                                  I.stream[g]),
+          "dpgo_copy_to_host_async");
+  sync();
+  DeviceRBCDStatus st;
+  st.records.assign(I.statusHost, I.statusHost + (size_t)S * I.K);
+  double gn2 = 0;
+  for (unsigned a = 0; a < I.K; ++a) {
+    st.cost += st.at(a, 0) + st.at(a, 1);
+    gn2 += st.at(a, 2);
+  }
+  st.gradnorm = std::sqrt(gn2);
+  return st;
+}
+
+// every agent's status record on the device (G first, from the current tiles), N > 1: all-gathered; no synchronisation
+void DeviceRBCD::statusDevice() {
+  Impl &I = *impl;
+  constexpr unsigned S = DPGO_STATUS_DOUBLES;
   if (I.gatheredCurrent) {
     for (unsigned a = 0; a < I.K; ++a)
       check(dpgo_agent_build_G(I.h[a], I.gathered[(size_t)I.gpuOf[a]], (int64_t)I.K * I.pmax), "dpgo_agent_build_G");
@@ -564,6 +666,13 @@ DeviceRBCDStatus DeviceRBCD::status() {
       check(dpgo_device_malloc((int)g, sizeof(double) * S * I.perGpu, &p), "dpgo_device_malloc");
       I.statusDev[g] = static_cast<double *>(p);
     }
+    I.statusAll = I.statusDev;
+    if (I.N > 1)
+      for (unsigned g = 0; g < I.N; ++g) {
+        void *p = nullptr;
+        check(dpgo_device_malloc((int)g, sizeof(double) * S * I.K, &p), "dpgo_device_malloc");
+        I.statusAll[g] = static_cast<double *>(p);
+      }
     void *hp = nullptr;
     check(dpgo_host_alloc_pinned(sizeof(double) * S * I.K, &hp), "dpgo_host_alloc_pinned");
     I.statusHost = static_cast<double *>(hp);
@@ -574,20 +683,9 @@ DeviceRBCDStatus DeviceRBCD::status() {
     std::vector<dpgo_problem *> hs(I.h.begin() + (size_t)g * I.perGpu, I.h.begin() + (size_t)(g + 1) * I.perGpu);
     check(dpgo_agents_status_async(hs.data(), (int)hs.size(), slots.data(), I.statusDev[g], I.stream[g]),
           "dpgo_agents_status_async");
-    check(dpgo_copy_to_host_async((int)g, I.statusHost + (size_t)g * I.perGpu * S, I.statusDev[g], sizeof(double) * S * I.perGpu,
-                                  I.stream[g]),
-          "dpgo_copy_to_host_async");
   }
-  sync();
-  DeviceRBCDStatus st;
-  st.records.assign(I.statusHost, I.statusHost + (size_t)S * I.K);
-  double gn2 = 0;
-  for (unsigned a = 0; a < I.K; ++a) {
-    st.cost += st.at(a, 0) + st.at(a, 1);
-    gn2 += st.at(a, 2);
-  }
-  st.gradnorm = std::sqrt(gn2);
-  return st;
+  I.allGatherRecords();
+  I.recordsCurrent = true;
 }
 
 DeviceRBCDSolveReport DeviceRBCD::solve(const DeviceRBCDSolveOptions &o) {

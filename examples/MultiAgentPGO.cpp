@@ -1,7 +1,7 @@
 // MultiAgentPGO -- command-line driver of the GPU distributed pose-graph optimiser (C++ host API).
 //
 //   MultiAgentPGO <file.g2o> [--robots K] [--iters N] [--stop GRADNORM] [--accel] [--rgd] [--jacobi]
-//                 [--rank R] [--trace out.csv] [--resident [--gpus N] [--schedule greedy|coloured|parallel] [--bench ROUNDS]
+//                 [--rank R] [--trace out.csv] [--resident [--gpus N] [--schedule greedy|coloured|parallel|greedy_set] [--bench ROUNDS]
 //                                                           [--partition FILE] [--init central|distributed]]
 //
 // --resident runs the device-resident multi-GPU runner (DPGO::DeviceRBCD): iterates stay in HBM, K agents over N GPUs
@@ -60,7 +60,7 @@ static Options parse(int argc, char **argv) {
   }
   if (o.file.empty()) {
     std::cerr << "usage: MultiAgentPGO <file.g2o> [--robots K] [--iters N] [--stop G] [--accel] [--rgd] [--jacobi] "
-                 "[--rank R] [--trace out.csv] [--resident [--gpus N] [--schedule greedy|coloured|parallel] [--momentum agents|colours]]"
+                 "[--rank R] [--trace out.csv] [--resident [--gpus N] [--schedule greedy|coloured|parallel|greedy_set] [--momentum agents|colours]]"
               << std::endl;
     std::exit(2);
   }

@@ -13,7 +13,9 @@
 // K agents are spread over N GPUs of one node (K % N == 0, contiguous blocks), one process, one stream and one NCCL
 // communicator per GPU (ncclCommInitAll).  Schedules: "greedy" (the reference's: one agent per round, argmax of the block
 // gradient norms -- reproduces the shipped traces), "coloured" (all agents of one colour class of the agent graph per
-// round: same RBCD semantics, concurrent), "parallel" (all agents on the previous round's poses).
+// round: same RBCD semantics, concurrent), "parallel" (all agents on the previous round's poses), "greedy_set" (the greedy
+// rule applied to as many agents as RBCD allows: each round a maximal set of agents that share no edge, taken in decreasing
+// block gradient norm, chosen on the GPU from the status taken before the round; no host synchronisation per round).
 // When a GPU hosts several agents of one colour class, their steps run side by side (one thread-block cluster and one
 // stream per agent, the whole round of a GPU replayed as a CUDA graph): DeviceRBCDOptions::concurrent.
 #ifndef DPGO_DEVICE_RBCD_H
@@ -40,7 +42,8 @@ struct DeviceRBCDOptions {
   // empty: contiguous ranges, the last agent takes the remainder (ref :95-109)
   std::vector<unsigned> owner;
   // the active agents of a round that share a GPU step side by side, each as one thread-block cluster on its own stream
-  // (dpgo_agents_round_async; greedy / coloured schedules): -1 = when some GPU hosts >= 2 agents of one colour class
+  // (dpgo_agents_round_async; greedy / coloured / greedy_set schedules): -1 = when some GPU hosts >= 2 agents of one
+  // colour class (coloured) or >= 2 agents that are not neighbours (greedy_set)
   int concurrent = -1;
   // "central": the caller's XInit (r x (d+1)n); "distributed": the reference's multi-robot initialisation
   // (PGOAgentParameters::multirobot_initialization, ref include/DPGO/PGOAgent.h:129) on the GPUs -- every agent's chordal
@@ -81,7 +84,8 @@ struct DeviceRBCDStatus {
 // Stop rules of DeviceRBCD::solve (a tolerance of 0 disables its rule): the central gradient norm below gradnormTol
 // (ref examples/MultiRobotExample.cpp:302-305); every agent optimised since the solve began with its last relative change
 // <= relChangeTol (ref PGOAgent::shouldTerminate, src/PGOAgent.cpp:703-716,1007-1031); maxRounds rounds.  The status is
-// taken after every checkEvery-th round and after the last; the greedy schedule needs checkEvery == 1.
+// taken after every checkEvery-th round and after the last; the greedy schedule needs checkEvery == 1 (greedy_set takes
+// any: it selects on the GPU).
 struct DeviceRBCDSolveOptions {
   unsigned maxRounds = 500;
   double gradnormTol = 0.1;
@@ -125,10 +129,14 @@ class DeviceRBCD {
   // d x (d+1)n trajectory in global pose order, rounded on the device against agent 0's pose 0
   // (ref getTrajectoryInGlobalFrame, src/PGOAgent.cpp:500-519)
   Matrix trajectory();
+  // greedy_set: the agents of rounds first .. first + count - 1 (those issued so far), each sorted; synchronises the GPUs
+  std::vector<std::vector<unsigned>> selectionLog(unsigned first = 0, unsigned count = ~0u);
 
  private:
   struct Impl;
-  std::vector<unsigned> issueRound();           // one round of the schedule's active agents; returns them
+  std::vector<unsigned> issueRound();           // one round of the schedule's active agents; returns them (greedy_set: none)
+  void selectRound();
+  void statusDevice();
   void roundAccelerated(const std::vector<unsigned> &active);
   void alignWaves();
   std::vector<DeviceRBCDInitRecord> mInitReport;

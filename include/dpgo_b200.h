@@ -403,6 +403,35 @@ DPGO_API int dpgo_host_alloc_pinned(size_t bytes, void **ptr);
 DPGO_API int dpgo_host_free_pinned(void *ptr);
 DPGO_API int dpgo_copy_to_host_async(int device, void *dst_host, const void *src_dev, size_t bytes, void *stream);
 
+/* ---- greedy independent-set rounds (schedule "greedy_set" of the device runners): every round steps a maximal set of
+ *      agents that share no edge, chosen on the device by block gradient norm (ref examples/MultiRobotExample.cpp:308-325
+ *      chooses the single largest) ---------------------------------------------------------------------------------- */
+/* The agent graph of a runner's num_agents agents (1..1024) in CSR form: the neighbours of agent a are
+ * adj[adj_ptr[a] .. adj_ptr[a+1]).  Kept by `lead`, the first agent of the runner's agents on its GPU; once per runner and
+ * GPU.  Empties lead's selection log.  Synchronises the device. */
+DPGO_API int dpgo_agents_set_agent_graph(dpgo_problem_t *lead, int num_agents, const int32_t *adj_ptr, const int32_t *adj);
+/* One greedy independent-set round of `count` agents of one device (agents[0] = the lead of dpgo_agents_set_agent_graph;
+ * agent_index[i] = agents[i]'s id in the agent graph).  One launch on `stream` (NULL: the lead's) selects from the status
+ * records of ALL num_agents agents in records_dev (device memory, agent-major, DPGO_STATUS_DOUBLES each, as
+ * dpgo_agents_status_async writes them): agents in decreasing |rgrad|^2 (field 2), ties to the lower id, each taken unless a
+ * neighbour already is.  The k-byte mask is appended to lead's selection log.  Then, as dpgo_agents_round_async with
+ * pack_after_join = 0, every listed agent's G rebuild -> step -> pack into send_dev[i]; the kernels of an agent left out
+ * return at entry and touch nothing (iterate, G, tiles, result record, status fields 3 and 4).
+ * Ordering: the records must be complete on `stream` before the call (e.g. the status launch, or the all-gather of the
+ * records, issued earlier on the same stream); the calls that share a lead must be ordered.  A repeated call of cluster
+ * agents with the same buffers is replayed as a CUDA graph (the selection is device data, so one graph serves every set;
+ * the log's doubling starts a new one); a call with a full-grid agent is issued eagerly, and a left-out full-grid agent
+ * still costs its launches.  This call is itself never captured by the caller's graph: the log can grow on the host. */
+DPGO_API int dpgo_agents_select_round_async(dpgo_problem_t *const *agents, int count, const int32_t *agent_index,
+                                            const dpgo_opt_params_t *params, const double *records_dev,
+                                            const double *gathered_dev, int64_t num_slots, double *const *send_dev,
+                                            void *stream);
+/* lead's selection log: *total_rounds = rounds issued since dpgo_agents_set_agent_graph; rounds [first_round,
+ * first_round + max_rounds) that exist are copied to out_host, num_agents bytes per round (1 = selected).  Synchronises the
+ * device. */
+DPGO_API int dpgo_agents_selection_log(dpgo_problem_t *lead, int64_t first_round, int64_t max_rounds, uint8_t *out_host,
+                                       int64_t *total_rounds);
+
 #ifdef __cplusplus
 }
 #endif
