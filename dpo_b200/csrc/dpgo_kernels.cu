@@ -185,7 +185,7 @@ __device__ void phase_eval(const KParams &kp, const CtaRows &cr, int cb, bool sa
 //   HD = P_X( delta_new Q - [delta_new_Y S]_pose ),   acc[0] = <delta_new, HD>
 // If onfly == false the operand is read as is from `zsrc` (single-operation entry point).
 // ---------------------------------------------------------------------------------------------
-template <int R, int DH>
+template <int R, int DH, bool CLOCK>
 __device__ void phase_hess(const KParams &kp, const CtaRows &cr, int cb, const double *zsrc, const double *dold, double *dnew,
                            double beta, bool onfly, double (&acc)[NRED]) {
   constexpr int TS = R * DH;
@@ -196,7 +196,7 @@ __device__ void phase_hess(const KParams &kp, const CtaRows &cr, int cb, const d
   RowIter<R> it(cr);
   const bool valid = (it.a < R) && (it.c < DH);
   const int e = it.c * R + it.a;
-  const bool ticking = (kp.phase_ns != nullptr) && blockIdx.x == 0 && threadIdx.x == 0;
+  const bool ticking = CLOCK && (kp.phase_ns != nullptr) && blockIdx.x == 0 && threadIdx.x == 0;
   unsigned long long th0 = 0, th1 = 0;
   if (ticking) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(th0));
   for (int jb = it.jb; jb < it.r1; jb += it.stride) {
@@ -744,7 +744,7 @@ __device__ void phase_pz(const KParams &kp, const CtaRows &cr, int cb, const dou
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ int4 ld_int4(const void *p) { return __ldg(reinterpret_cast<const int4 *>(p)); }
 
-template <int R, int DH>
+template <int R, int DH, bool CLOCK>
 __device__ void phase_nd(const KParams &kp, int ph, const double *V, int cb, double *Zout, double *ys, double *slots,
                          int4 *grec, double (&acc)[NRED]) {
   constexpr int TS = R * DH;
@@ -764,7 +764,7 @@ __device__ void phase_nd(const KParams &kp, int ph, const double *V, int cb, dou
   const int nsub = nwarps * SGW;
   const double *X = kp.v[V_X0 + cb];
   const double *src = (dir == 0) ? V : N.TX;
-  const bool ticking = (kp.phase_ns != nullptr) && blockIdx.x == 0 && threadIdx.x == 0;
+  const bool ticking = CLOCK && (kp.phase_ns != nullptr) && blockIdx.x == 0 && threadIdx.x == 0;
   for (int si = s0; si < s1; ++si) {
     int g0 = ca.z, g1 = ca.w, j0 = cbq.x, j1 = cbq.y, e0 = cbq.z, e1 = cbq.w;      // the first step sits in the CTA record
     if (si != s0) {
@@ -1008,9 +1008,12 @@ __device__ __forceinline__ void zero(double (&acc)[NRED]) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// The persistent kernel
+// The persistent kernel.  FULL = false is the variant every launch uses unless it asks for the dense preconditioner or
+// the phase clock (see launch_optimize_t): without the dense pipeline's ring state and the clock's timestamps, which are
+// otherwise live across the whole kernel, the register allocator has room at the 128-register cap of
+// launch_bounds(512, 1), and every phase spills less.  Both variants compute the same values in the same order.
 // ---------------------------------------------------------------------------------------------
-template <int R, int DH> __global__ void __launch_bounds__(OPT_THREADS, 1) k_optimize(const KParams kp) {
+template <int R, int DH, bool FULL> __global__ void __launch_bounds__(OPT_THREADS, 1) k_optimize(const KParams kp) {
   // a gated-off agent (selection of dpgo_agents_select_round_async): every CTA reads the same flag before anything else,
   // so the whole grid returns and no barrier, result or opt_record is touched
   if (kp.gate != nullptr && __ldg(kp.gate) == 0) return;
@@ -1046,7 +1049,8 @@ template <int R, int DH> __global__ void __launch_bounds__(OPT_THREADS, 1) k_opt
   ring.count = 0;
   int *sMeta = reinterpret_cast<int *>(ring.empty + DENSE_NST);         // symmetric variant: (segment, first row) per window slot
   // bulk-TMA streaming needs 16-byte aligned rows (N even) and only pays off for a real stream
-  const bool dense_tma = (kp.prm.precond == DPGO_PRECOND_DENSE_EXACT) && (kp.pinv != nullptr) && ((kp.N & 1) == 0) && (kp.N >= 2048);
+  const bool dense_tma = FULL && (kp.prm.precond == DPGO_PRECOND_DENSE_EXACT) && (kp.pinv != nullptr) && ((kp.N & 1) == 0) &&
+                         (kp.N >= 2048);
   const bool dense_sym = dense_tma && (kp.sym_ok != 0);
   if (dense_tma) {
     if (dense_sym) {       // stale shared memory must be finite: tiles past N are multiplied by zero operands
@@ -1066,7 +1070,7 @@ template <int R, int DH> __global__ void __launch_bounds__(OPT_THREADS, 1) k_opt
   // diagnostic phase clock: CTA 0 / thread 0 charges the time since the previous tick to a phase kind
   // (0 eval, 1 dense apply, 2 partial sums + projection, 3 Hessian product, 4 tCG update, 5 retraction, 6 final)
   unsigned long long tick_last = 0;
-  const bool ticking = (kp.phase_ns != nullptr) && blockIdx.x == 0 && threadIdx.x == 0;
+  const bool ticking = FULL && (kp.phase_ns != nullptr) && blockIdx.x == 0 && threadIdx.x == 0;
   auto tick = [&](int kind) {
     if (ticking) {
       unsigned long long t;
@@ -1086,10 +1090,10 @@ template <int R, int DH> __global__ void __launch_bounds__(OPT_THREADS, 1) k_opt
   int4 *nd_grec = reinterpret_cast<int4 *>((reinterpret_cast<uintptr_t>(nd_slots + (size_t)kp.nd.max_slots * nd::PANEL_ROWS * R) + 15) & ~(uintptr_t)15);
   // Z = P_X( (Q + 0.1 I)^-1 V ), returns <Z, V> in acc[0]; every phase ends with a grid barrier
   auto apply_exact = [&](const double *Vv, int cbx, double *Zout) {
-    if (precond == DPGO_PRECOND_SPARSE_EXACT) {
+    if (!FULL || precond == DPGO_PRECOND_SPARSE_EXACT) {     // the lean variant is never launched with the dense one
       zero(acc);
       for (int ph = 0; ph < kp.nd.nphases; ++ph) {
-        phase_nd<R, DH>(kp, ph, Vv, cbx, Zout, nd_ys, nd_slots, nd_grec, acc);
+        phase_nd<R, DH, FULL>(kp, ph, Vv, cbx, Zout, nd_ys, nd_slots, nd_grec, acc);
         if (ph + 1 < kp.nd.nphases) { phase_end<0>(kp, bc, acc); tick(8 + min(ph, 15)); }
       }
       phase_end<1>(kp, bc, acc);
@@ -1177,7 +1181,7 @@ template <int R, int DH> __global__ void __launch_bounds__(OPT_THREADS, 1) k_opt
   }
   if (kp.op == OP_RHESS) {
     zero(acc);
-    phase_hess<R, DH>(kp, cr, 0, kp.v[V_AUX], nullptr, nullptr, 0.0, false, acc);
+    phase_hess<R, DH, FULL>(kp, cr, 0, kp.v[V_AUX], nullptr, nullptr, 0.0, false, acc);
     phase_end(kp, bc, acc);
     if (blockIdx.x == 0 && threadIdx.x == 0) { *kp.result = res; *kp.bar_epoch = bc.epoch; }
     return;
@@ -1225,7 +1229,7 @@ template <int R, int DH> __global__ void __launch_bounds__(OPT_THREADS, 1) k_opt
       for (int j = 0; j < prm.tr_max_inner; ++j) {
         double *dnew = kp.v[V_D0 + (1 - pd)];
         zero(acc);
-        phase_hess<R, DH>(kp, cr, cb, zsrc, kp.v[V_D0 + pd], dnew, beta, true, acc);
+        phase_hess<R, DH, FULL>(kp, cr, cb, zsrc, kp.v[V_D0 + pd], dnew, beta, true, acc);
         phase_end<1>(kp, bc, acc);
         tick(3);
         res.spmv_passes++;
@@ -1502,40 +1506,48 @@ template <int R, int DH> static size_t optimize_smem_doubles(const KParams &kp, 
   return base + 8;
 }
 
+// The full kernel (dense preconditioner, phase clock) or the lean one (everything else).
+template <int R, int DH> static void *optimize_kernel(bool full) {
+  return full ? (void *)k_optimize<R, DH, true> : (void *)k_optimize<R, DH, false>;
+}
+
 template <int R, int DH> static cudaError_t launch_optimize_t(const KParams &kp_in, cudaStream_t stream) {
   KParams kp = kp_in;
+  const bool full = (kp.phase_ns != nullptr) || (kp.prm.precond == DPGO_PRECOND_DENSE_EXACT);
+  const void *kern = optimize_kernel<R, DH>(full);
   const size_t smem_max = optimize_smem_doubles<R, DH>(kp, true) * sizeof(double);
   static_assert((size_t)ND_YCAP_TILES * R * DH + (size_t)(ND_SLOT_CAP + 1) * nd::PANEL_ROWS * R + 4 * (size_t)ND_YCAP_TILES + 8 <=
                     (size_t)DENSE_PER_MAX * R + (size_t)DENSE_RING_DOUBLES + 2 * DENSE_NST + (size_t)SYM_META_DOUBLES,
                 "the sparse plan's capacities must fit the kernel's maximum shared memory");
   kp.smem_doubles = (int)optimize_smem_doubles<R, DH>(kp, false);
   const size_t smem = (size_t)kp.smem_doubles * sizeof(double);
-  static bool attr_set[64] = {};
+  // per device and kernel variant
+  static bool attr_set[2][64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(k_optimize<R, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+  if (dev < 0 || dev >= 64 || !attr_set[full][dev]) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
     if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) attr_set[dev] = true;
+    if (dev >= 0 && dev < 64) attr_set[full][dev] = true;
   }
   {
     // shared-memory carve-out hint: what this launch needs (+ the 1 KB the system reserves), so that L1 gets the rest
-    static int last_pct[64];
+    static int last_pct[2][64];
     static bool init = false;
-    if (!init) { for (int i = 0; i < 64; ++i) last_pct[i] = -1; init = true; }
+    if (!init) { for (int i = 0; i < 64; ++i) last_pct[0][i] = last_pct[1][i] = -1; init = true; }
     const int pct = std::min(100, (int)((smem + 2048) * 100 / (228 * 1024)) + 1);
-    if (dev >= 0 && dev < 64 && last_pct[dev] != pct) {
-      cudaFuncSetAttribute(k_optimize<R, DH>, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-      last_pct[dev] = pct;
+    if (dev >= 0 && dev < 64 && last_pct[full][dev] != pct) {
+      cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
+      last_pct[full][dev] = pct;
     }
   }
   if (kp.cluster) {
     // one cluster = the whole grid: an ordinary (non-cooperative) launch, co-scheduling is guaranteed by the cluster
-    static bool np_set[64] = {};
-    if (kp.grid > 8 && (dev < 0 || dev >= 64 || !np_set[dev])) {
-      cudaError_t e = cudaFuncSetAttribute(k_optimize<R, DH>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    static bool np_set[2][64] = {};
+    if (kp.grid > 8 && (dev < 0 || dev >= 64 || !np_set[full][dev])) {
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
       if (e != cudaSuccess) return e;
-      if (dev >= 0 && dev < 64) np_set[dev] = true;
+      if (dev >= 0 && dev < 64) np_set[full][dev] = true;
     }
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(kp.grid);
@@ -1549,15 +1561,16 @@ template <int R, int DH> static cudaError_t launch_optimize_t(const KParams &kp_
     at[0].val.clusterDim.z = 1;
     cfg.attrs = at;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, k_optimize<R, DH>, kp);
+    void *args[] = {(void *)&kp};
+    return cudaLaunchKernelExC(&cfg, kern, args);
   }
   void *args[] = {(void *)&kp};
-  return cudaLaunchCooperativeKernel((void *)k_optimize<R, DH>, dim3(kp.grid), dim3(OPT_THREADS), args, smem, stream);
+  return cudaLaunchCooperativeKernel(kern, dim3(kp.grid), dim3(OPT_THREADS), args, smem, stream);
 }
 
 template <int R, int DH> static int max_cluster_t(int device) {
   const size_t smem = ((OPT_THREADS / 32) * NRED + 2 * NRED + SP_CACHE_INTS / 2 + (size_t)ND_SMEM_NEED_SMALL) * sizeof(double);
-  cudaFuncSetAttribute(k_optimize<R, DH>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+  for (int f = 0; f < 2; ++f) cudaFuncSetAttribute(optimize_kernel<R, DH>(f != 0), cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
   for (int cs : {16, 8}) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(cs);
@@ -1570,8 +1583,10 @@ template <int R, int DH> static int max_cluster_t(int device) {
     at[0].val.clusterDim.z = 1;
     cfg.attrs = at;
     cfg.numAttrs = 1;
-    int nclusters = 0;
-    if (cudaOccupancyMaxActiveClusters(&nclusters, k_optimize<R, DH>, &cfg) == cudaSuccess && nclusters >= 1) return cs;
+    int n0 = 0, n1 = 0;
+    if (cudaOccupancyMaxActiveClusters(&n0, optimize_kernel<R, DH>(false), &cfg) == cudaSuccess && n0 >= 1 &&
+        cudaOccupancyMaxActiveClusters(&n1, optimize_kernel<R, DH>(true), &cfg) == cudaSuccess && n1 >= 1)
+      return cs;
   }
   cudaGetLastError();
   return 0;
@@ -1579,9 +1594,14 @@ template <int R, int DH> static int max_cluster_t(int device) {
 
 template <int R, int DH> static int max_grid_t(int device) {
   const size_t smem = ((OPT_THREADS / 32) * NRED + 2 * NRED + SP_CACHE_INTS / 2 + (size_t)DENSE_PER_MAX * R + (size_t)DENSE_RING_DOUBLES + 2 * DENSE_NST + (size_t)SYM_META_DOUBLES) * sizeof(double);
-  cudaFuncSetAttribute(k_optimize<R, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  int per_sm = 0, sms = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_optimize<R, DH>, OPT_THREADS, smem) != cudaSuccess) return 0;
+  int per_sm = 1, sms = 0;
+  for (int f = 0; f < 2; ++f) {
+    const void *kern = optimize_kernel<R, DH>(f != 0);
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    int ps = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ps, kern, OPT_THREADS, smem) != cudaSuccess) return 0;
+    per_sm = std::min(per_sm, ps);
+  }
   if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
   return per_sm > 0 ? sms : 0;      // one CTA per SM
 }
