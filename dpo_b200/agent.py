@@ -517,10 +517,14 @@ def greedy_independent_set(gradnorm2: np.ndarray, neighbours: Sequence[Sequence[
     return [int(a) for a in np.flatnonzero(taken)]
 
 
-def check_solve_arguments(schedule: str, acceleration: bool, max_rounds: int, check_every: int) -> None:
-    if acceleration:
-        raise ValueError("solve() does not support acceleration=True: the accelerated iterate's relative change is "
-                         "measured against the Nesterov step's XPrev; drive it with step()")
+def check_solve_arguments(schedule: str, acceleration: bool, max_rounds: int, check_every: int,
+                          momentum_blocks: str = "agents") -> None:
+    """solve() runs accelerated rounds only with the momentum over colour classes: there an accelerated round ends with
+    every active agent's status record as the reference's iterate() leaves it (relative change against XPrev, one
+    optimising call per round)."""
+    if acceleration and (schedule != "coloured" or momentum_blocks != "colours"):
+        raise ValueError("solve() supports acceleration=True only with schedule='coloured' and momentum_blocks='colours'; "
+                         "drive other accelerated runs with step()")
     if max_rounds < 1 or check_every < 1:
         raise ValueError("max_rounds and check_every must be >= 1")
     if schedule == "greedy" and check_every != 1:
@@ -1085,8 +1089,8 @@ class DistributedPGO:
         """Run rounds until the stop rule holds (see stop_reason): the status is taken after every check_every-th round
         and after the last one; the rounds in between are issued without a host synchronisation.  callback(round, cost,
         gradnorm) sees every check.  The greedy schedule selects the next agent from each round's status, as step() does,
-        so it needs check_every = 1."""
-        check_solve_arguments(self.schedule, self.acceleration, max_rounds, check_every)
+        so it needs check_every = 1.  Accelerated runs need schedule="coloured" with momentum_blocks="colours"."""
+        check_solve_arguments(self.schedule, self.acceleration, max_rounds, check_every, self.momentum_blocks)
         with self.torch.cuda.stream(self._runner_stream()):
             return self._solve(max_rounds, gradnorm_tol, rel_change_tol, check_every, callback)
 

@@ -9,11 +9,17 @@
 //                        of the agent and written by its last one (ticket counter), so a replayed round takes no
 //                        per-round kernel arguments.
 //  k_accel_finish<R,DH>  an active agent after its step: V = proj(V + gamma (X - Y)); on a restart round X = XPrev before
-//                        the plain step and V = Y = X after it.
+//                        the plain step and V = Y = X after it.  The launch that ends the round (ACCEL_FINISH_V on a
+//                        plain round, ACCEL_FINISH_RESTART_END on a restart round) also writes the agent's status record
+//                        as the reference's iterate() does (src/PGOAgent.cpp:673,703-716): relative change
+//                        sqrt(|X - XPrev|^2 / n) of the whole accelerated iteration, and one optimising call more than at
+//                        the round's begin (k_accel_agents snapshots the count), however many steps the round took.
+//                        Per-CTA partials, summed in CTA order by the agent's last CTA (ticket counter), as k_agents_status.
 // Both reuse stiefel_project_tile with the operand order of k_stiefel_project, so the iterates are bitwise those of the
 // per-agent dpgo_agent_accel_* calls.
 #include <cuda_runtime.h>
 
+#include "dpgo_device.cuh"
 #include "dpgo_kernels.cuh"
 #include "dpgo_rotation.cuh"
 
@@ -97,24 +103,64 @@ __global__ void __launch_bounds__(ACCEL_THREADS) k_accel_agents(int njobs, const
       J.state[1] = restart ? 0.0 : alpha;
       J.state[2] = (double)it;
       J.state[3] = gamma;
+      J.state[4] = __ldcg(J.opt_record + 1);              // optimising calls at the round's begin
       *J.ticket = 0u;                                       // ready for the next launch on the stream
     }
   }
 }
 
+constexpr int ACCEL_WARPS = ACCEL_THREADS / 32;
+
 template <int R, int DH>
-__global__ void k_accel_finish(int n, double *X, double *Y, double *V, const double *XP, const double *state, int mode) {
+__global__ void k_accel_finish(int n, double *X, double *Y, double *V, const double *XP, const double *state, int mode,
+                               double *partials, unsigned *ticket, double *opt_record) {
   constexpr int TS = R * DH;
+  __shared__ double sm_warp[ACCEL_WARPS];
+  __shared__ bool last;
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n) return;
-  double *Xj = X + (size_t)j * TS, *Yj = Y + (size_t)j * TS, *Vj = V + (size_t)j * TS;
-  if (mode == ACCEL_FINISH_RESTART_END) {
-    copy_tile<TS>(Xj, Vj);
-    copy_tile<TS>(Xj, Yj);
-    return;
+  double d2 = 0.0;
+  if (j < n) {
+    double *Xj = X + (size_t)j * TS, *Yj = Y + (size_t)j * TS, *Vj = V + (size_t)j * TS;
+    const double *XPj = XP + (size_t)j * TS;
+    if (mode == ACCEL_FINISH_RESTART_END) {
+      copy_tile<TS>(Xj, Vj);
+      copy_tile<TS>(Xj, Yj);
+    } else {
+      update_V<R, DH>(Xj, Yj, Vj, __ldg(state + 3));
+      if (mode == ACCEL_FINISH_V_RESTART) copy_tile<TS>(XPj, Xj);
+    }
+    if (mode != ACCEL_FINISH_V_RESTART) {
+#pragma unroll
+      for (int e = 0; e < TS; ++e) {
+        const double t = Xj[e] - XPj[e];
+        d2 = fma(t, t, d2);
+      }
+    }
   }
-  update_V<R, DH>(Xj, Yj, Vj, __ldg(state + 3));
-  if (mode == ACCEL_FINISH_V_RESTART) copy_tile<TS>(XP + (size_t)j * TS, Xj);
+  if (mode == ACCEL_FINISH_V_RESTART) return;              // the restart's step follows: the round is not over
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  d2 = warp_sum(d2);
+  if (lane == 0) sm_warp[warp] = d2;
+  __syncthreads();
+  const int ncta = accel_ctas(n);
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int w = 0; w < ACCEL_WARPS; ++w) s += sm_warp[w];
+    partials[blockIdx.x] = s;
+    __threadfence();                                        // partial visible before the ticket
+    last = atomicAdd(ticket, 1u) == (unsigned)(ncta - 1);
+  }
+  __syncthreads();
+  if (!last || warp != 0) return;
+  __threadfence();
+  double t = 0.0;
+  for (int b = lane; b < ncta; b += 32) t += __ldcg(partials + b);   // fixed order: lane-strided, then a fixed shuffle tree
+  t = warp_sum(t);
+  if (lane == 0) {
+    opt_record[0] = sqrt(t / (double)n);
+    opt_record[1] = __ldcg(state + 4) + 1.0;
+    *ticket = 0u;                                           // ready for the next launch on the stream
+  }
 }
 
 }  // namespace
@@ -132,10 +178,12 @@ cudaError_t launch_accel_agents(int r, int dh, int njobs, int total_ctas, const 
 }
 
 cudaError_t launch_accel_finish(int r, int dh, int n, double *X, double *Y, double *V, const double *XP, const double *state,
-                                int mode, cudaStream_t stream) {
+                                int mode, double *partials, unsigned *ticket, double *opt_record, cudaStream_t stream) {
+  if (n <= 0) return cudaErrorInvalidValue;
   bool ok = false;
   DPGO_DISPATCH(r, dh, {
-    k_accel_finish<R, DH><<<(n + 127) / 128, 128, 0, stream>>>(n, X, Y, V, XP, state, mode);
+    k_accel_finish<R, DH><<<accel_ctas(n), ACCEL_THREADS, 0, stream>>>(n, X, Y, V, XP, state, mode, partials, ticket,
+                                                                      opt_record);
     ok = true;
   });
   if (!ok) return cudaErrorInvalidValue;

@@ -90,7 +90,8 @@ struct dpgo_problem {
   // accelerated rounds (dpgo_accel.cu): momentum record + ticket on the device; the host's count of begun rounds and the
   // restart rule of the last begin, which decide whether the agent's next dpgo_agents_accel_round_async restarts
   double *d_acc_state = nullptr;
-  unsigned *d_acc_ticket = nullptr;
+  double *d_acc_part = nullptr;  // accel_ctas(n) per-CTA partials of the finish launch's |X - XPrev|^2
+  unsigned *d_acc_ticket = nullptr;   // [0] begin launch, [1] finish launch (the finish runs on the agent's own stream)
   long long acc_rounds = 0;
   bool acc_restart_due = false;
   std::vector<JobTable<dpgo::AccelJob>> accel_tables;    // job tables of dpgo_agents_accel_begin_async, kept by the call's first agent
@@ -739,7 +740,7 @@ int dpgo_problem_destroy(dpgo_problem_t *p) {
   free_dev(p->d_cand_w); free_dev(p->d_T_align); free_dev(p->d_align_info); free_dev(p->d_jobs); free_dev(p->d_ready);
   free_dev(p->d_opt_record); free_dev(p->d_status_part); free_dev(p->d_status_ticket); free_dev(p->d_anchor); free_dev(p->d_traj);
   for (auto &t : p->status_tables) free_dev(t.d_jobs);
-  free_dev(p->d_acc_state); free_dev(p->d_acc_ticket); free_dev(p->d_pub_slot);
+  free_dev(p->d_acc_state); free_dev(p->d_acc_part); free_dev(p->d_acc_ticket); free_dev(p->d_pub_slot);
   for (auto &t : p->accel_tables) free_dev(t.d_jobs);
   free_nd(p);
   if (p->h_result) cudaFreeHost(p->h_result);
@@ -1520,9 +1521,10 @@ int dpgo_agent_accel_init(dpgo_problem_t *p) {
     DPGO_CUDA(cudaMemcpyAsync(p->d_acc[i], p->d_vec[dpgo::V_X0], p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
   }
   if (!p->d_acc_state) DPGO_CUDA(cudaMalloc(&p->d_acc_state, sizeof(double) * dpgo::ACCEL_STATE_DOUBLES));
-  if (!p->d_acc_ticket) DPGO_CUDA(cudaMalloc(&p->d_acc_ticket, sizeof(unsigned)));
+  if (!p->d_acc_part) DPGO_CUDA(cudaMalloc(&p->d_acc_part, sizeof(double) * (size_t)dpgo::accel_ctas(p->n)));
+  if (!p->d_acc_ticket) DPGO_CUDA(cudaMalloc(&p->d_acc_ticket, 2 * sizeof(unsigned)));
   DPGO_CUDA(cudaMemsetAsync(p->d_acc_state, 0, sizeof(double) * dpgo::ACCEL_STATE_DOUBLES, p->stream));
-  DPGO_CUDA(cudaMemsetAsync(p->d_acc_ticket, 0, sizeof(unsigned), p->stream));
+  DPGO_CUDA(cudaMemsetAsync(p->d_acc_ticket, 0, 2 * sizeof(unsigned), p->stream));
   p->acc_rounds = 0;
   p->acc_restart_due = false;
   return DPGO_OK;
@@ -2141,6 +2143,7 @@ int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, cons
       J.active = active_flags[i] != 0;
       J.X = p->d_vec[dpgo::V_X0]; J.Y = p->d_acc[0]; J.V = p->d_acc[1]; J.XP = p->d_acc[2];
       J.state = p->d_acc_state;
+      J.opt_record = p->d_opt_record;
       J.pub_slot = p->d_pub_slot;
       J.send_x = send_dev[i]; J.send_y = send_aux_dev[i];
       J.ticket = p->d_acc_ticket;
@@ -2170,12 +2173,13 @@ static int issue_accel_round(dpgo_problem_t *const *agents, int num_active, cons
     DPGO_CUDA(cudaMemcpyAsync(X, Y, p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
     DPGO_TRY(dpgo_optimize_resident_async(p, params));
     DPGO_CUDA(dpgo::launch_accel_finish(p->r, p->dh, p->n, X, Y, V, XP, p->d_acc_state,
-                                        p->acc_restart_due ? dpgo::ACCEL_FINISH_V_RESTART : dpgo::ACCEL_FINISH_V, p->stream));
+                                        p->acc_restart_due ? dpgo::ACCEL_FINISH_V_RESTART : dpgo::ACCEL_FINISH_V, p->d_acc_part,
+                                        p->d_acc_ticket + 1, p->d_opt_record, p->stream));
     if (p->acc_restart_due) {
       DPGO_TRY(dpgo_agent_build_G(p, gathered_dev, num_slots));
       DPGO_TRY(dpgo_optimize_resident_async(p, params));
       DPGO_CUDA(dpgo::launch_accel_finish(p->r, p->dh, p->n, X, Y, V, XP, p->d_acc_state, dpgo::ACCEL_FINISH_RESTART_END,
-                                          p->stream));
+                                          p->d_acc_part, p->d_acc_ticket + 1, p->d_opt_record, p->stream));
     }
     if (p->stream != main) {
       DPGO_CUDA(cudaEventRecord(p->ev_done, p->stream));

@@ -200,14 +200,16 @@ cudaError_t launch_select_independent(int k, const double *records, const int *a
                                       unsigned char *log, unsigned long long *log_count, cudaStream_t stream);
 
 // ---- accelerated rounds (dpgo_accel.cu) ----
-// Momentum record of an agent: {gamma, alpha, iterations, gamma of the last round}; the last slot is the gamma the round's
-// V update uses, which a restart has already cleared from slot 0.
-constexpr int ACCEL_STATE_DOUBLES = 4;
+// Momentum record of an agent: {gamma, alpha, iterations, gamma of the last round, optimising calls at the last begin}; slot
+// 3 is the gamma the round's V update uses, which a restart has already cleared from slot 0; slot 4 is KParams::opt_record[1]
+// as the round began, from which the finish launch counts the round as one optimising call.
+constexpr int ACCEL_STATE_DOUBLES = 5;
 // One agent of an accelerated begin launch: CTAs [cta0, cta0 + accel_ctas(n)) own ACCEL_THREADS consecutive poses each.
 struct AccelJob {
   int n, cta0, active;
   double *X, *Y, *V, *XP;
   double *state;                           // ACCEL_STATE_DOUBLES
+  const double *opt_record;                // KParams::opt_record of the agent (its count is snapshot into state[4])
   const int *pub_slot;                     // n: public slot of the pose, -1 when it is not public
   double *send_x, *send_y;                 // the agent's public tiles of X and of Y
   unsigned *ticket;                        // CTAs of the agent done in this launch (the last one resets it to 0)
@@ -216,8 +218,10 @@ constexpr int ACCEL_THREADS = 128;
 __host__ __device__ inline int accel_ctas(int n) { return (n + ACCEL_THREADS - 1) / ACCEL_THREADS; }
 cudaError_t launch_accel_agents(int r, int dh, int njobs, int total_ctas, const AccelJob *jobs, double momentum_n,
                                 int restart_interval, cudaStream_t stream);
+// ACCEL_FINISH_V and ACCEL_FINISH_RESTART_END end a round: they also write opt_record = {sqrt(|X - XP|^2 / n), state[4] + 1},
+// reducing through partials (accel_ctas(n) doubles) and ticket (the last CTA resets it to 0).
 enum AccelFinish { ACCEL_FINISH_V = 0, ACCEL_FINISH_V_RESTART = 1, ACCEL_FINISH_RESTART_END = 2 };
 cudaError_t launch_accel_finish(int r, int dh, int n, double *X, double *Y, double *V, const double *XP, const double *state,
-                                int mode, cudaStream_t stream);
+                                int mode, double *partials, unsigned *ticket, double *opt_record, cudaStream_t stream);
 
 }  // namespace dpgo

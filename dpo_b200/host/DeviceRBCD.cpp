@@ -49,6 +49,7 @@ struct DeviceRBCD::Impl {
   bool acceleration = false;
   unsigned restartInterval = 30;
   double momentumN = 1;
+  bool colourMomentum = false;     // momentumBlocks == "colours"
   std::vector<ncclComm_t> comm;
   std::vector<std::vector<unsigned>> neighbors;
   dpgo_opt_params_t prm;
@@ -118,6 +119,7 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
     throw std::invalid_argument("DeviceRBCD: momentumBlocks = colours counts the colour classes of the coloured schedule");
   if (opt.acceleration && opt.restartInterval < 1) throw std::invalid_argument("DeviceRBCD: restartInterval must be >= 1");
   I.acceleration = opt.acceleration;
+  I.colourMomentum = opt.momentumBlocks == "colours";
   I.restartInterval = opt.restartInterval;
   int ndev = 0;
   check(dpgo_device_count(&ndev), "dpgo_device_count");
@@ -690,9 +692,9 @@ void DeviceRBCD::statusDevice() {
 
 DeviceRBCDSolveReport DeviceRBCD::solve(const DeviceRBCDSolveOptions &o) {
   Impl &I = *impl;
-  if (I.acceleration)
-    throw std::invalid_argument("DeviceRBCD::solve: acceleration is not supported: the accelerated iterate's relative change "
-                                "is measured against the Nesterov step's XPrev; drive it with step()");
+  if (I.acceleration && !I.colourMomentum)
+    throw std::invalid_argument("DeviceRBCD::solve: acceleration is supported only with the coloured schedule and "
+                                "momentumBlocks = colours; drive other accelerated runs with step()");
   if (o.maxRounds < 1 || o.checkEvery < 1) throw std::invalid_argument("DeviceRBCD::solve: maxRounds and checkEvery must be >= 1");
   if (I.schedule == "greedy" && o.checkEvery != 1)
     throw std::invalid_argument("DeviceRBCD::solve: the greedy schedule selects the next agent from every round's status: "

@@ -54,7 +54,9 @@ struct DeviceRBCDOptions {
   // finish iterate(false), the X and Y tiles are exchanged (one ncclAllGather group per buffer), the active agents step
   // from Y.  momentumBlocks is the N of the recurrence: "agents" = the number of agents (the reference's), "colours" = the
   // number of colour classes (schedule "coloured" only: a coloured round is one exact block update).  With "agents" the
-  // automatic launch mode is one agent at a time.  solve() rejects acceleration.
+  // automatic launch mode is one agent at a time.  solve() takes acceleration with "colours" only: there each accelerated
+  // round leaves every active agent's status record as the reference's iterate() does (relative change against XPrev,
+  // one optimising call per round, restart or not).
   bool acceleration = false;
   unsigned restartInterval = 30;
   std::string momentumBlocks = "agents";

@@ -337,7 +337,10 @@ DPGO_API int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int co
  * the Y tiles in gathered_aux_dev.  Per agent: G from the Y tiles -> X = Y -> one step (thread-block cluster agents on
  * their own streams between a fork from and a join into main_stream, full-grid agents in order on main_stream) ->
  * V = proj(V + gamma (X - Y)); on a restart round then X = XPrev -> G from the X tiles -> one plain step -> V = Y = X.
- * Nothing is packed.  A repeated round is replayed as a CUDA graph (two variants per active set: plain and restart);
+ * The round then counts as ONE optimising call of the agent, as the reference's iterate() (src/PGOAgent.cpp:673,703-716):
+ * its status record (dpgo_agents_status_async) gets [3] = sqrt(|X - XPrev|^2 / n), X the iterate after the V update and
+ * any restart, XPrev the iterate at the round's begin, and [4] = the count at the begin + 1, on plain and restart rounds
+ * alike.  Agents idle in the round keep their fields [3] and [4].  Nothing is packed.  A repeated round is replayed as a CUDA graph (two variants per active set: plain and restart);
  * DPGO_ROUND_GRAPH=0 keeps the eager launches. */
 DPGO_API int dpgo_agents_accel_round_async(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
                                            const double *gathered_dev, const double *gathered_aux_dev, int64_t num_slots,
@@ -382,7 +385,8 @@ DPGO_API int dpgo_robust_single_rotation_averaging(int device, int d, int m, con
 /* doubles per agent record of dpgo_agents_status_async:
  *   [0] <XQ, X>   [1] <X, G>   [2] |P_X(XQ + G)|^2 (the same quantities as quad_init, lin_init, gradnorm_init^2 of an
  *   evaluation)   [3] relative change sqrt(|X - XPrev|^2 / n) of the agent's most recent optimising call (RTR or RGD;
- *   evaluations leave it alone)   [4] optimising calls since the handle was created */
+ *   evaluations leave it alone)   [4] optimising calls since the handle was created.  An accelerated round of
+ *   dpgo_agents_accel_round_async is one optimising call measured from the round's XPrev (see there). */
 #define DPGO_STATUS_DOUBLES 5
 /* One launch for every listed agent (all on one device, one d and r): agent i's record goes to
  * status_dev + slot[i] * DPGO_STATUS_DOUBLES (device memory; slots distinct).  An agent's record depends only on that

@@ -7,9 +7,11 @@ One GPU, one process; the variants alternate and each is run twice.
 Per workload (sphere2500 / 16 agents, torus3D / 8 agents, coloured schedule, r = 5, exact preconditioner):
   rounds_per_s   step(evaluate=False) rounds per second, host clock over --rounds rounds ending in a device synchronise:
                  "plain_concurrent" (no acceleration, agents side by side), "accel_sequential" (momentum over agents,
-                 full-grid steps one after the other), "accel_concurrent" (momentum over agents, side by side)
-  to_tol         rounds and wall time to |g| < 0.1 for plain coloured rounds and for momentum_blocks="colours" (both side
-                 by side), status() after every 5th round
+                 full-grid steps one after the other), "accel_concurrent" (momentum over agents, side by side),
+                 "accel_colours" (momentum over colour classes, side by side)
+  to_tol         rounds and wall time to |g| < 0.1 (all side by side, a check after every 5th round): the step() loop with
+                 status() for plain coloured rounds ("plain") and for momentum_blocks="colours" ("colours"), and
+                 solve(check_every=5, rel_change_tol=0) for momentum_blocks="colours" ("colours_solve")
 Prints ONE JSON line with the GPU's name, power limit and maximum SM clock, read in the same run.
 """
 from __future__ import annotations
@@ -27,8 +29,10 @@ sys.path.insert(0, ROOT)
 WORKLOADS = [("sphere2500", 16), ("torus3D", 8)]
 RATE_VARIANTS = {"plain_concurrent": dict(acceleration=False, concurrent=True),
                  "accel_sequential": dict(acceleration=True, concurrent=False),
-                 "accel_concurrent": dict(acceleration=True, concurrent=True)}
-TOL_VARIANTS = {"plain": dict(acceleration=False), "colours": dict(acceleration=True, momentum_blocks="colours")}
+                 "accel_concurrent": dict(acceleration=True, concurrent=True),
+                 "accel_colours": dict(acceleration=True, momentum_blocks="colours", concurrent=True)}
+COLOURS = dict(acceleration=True, momentum_blocks="colours")
+TOL_VARIANTS = {"plain": (dict(acceleration=False), False), "colours": (COLOURS, False), "colours_solve": (COLOURS, True)}
 
 
 def device_info():
@@ -58,20 +62,25 @@ def rate(torch, edges, n, k, rounds, kw):
     return rounds / (time.perf_counter() - t0)
 
 
-def to_tol(torch, edges, n, k, kw, check_every=5, cap=1000):
+def to_tol(torch, edges, n, k, kw, use_solve, check_every=5, cap=1000):
     run = make(edges, n, k, **kw)
     run.status()
     torch.cuda.synchronize()
     t0 = time.perf_counter()
-    st = None
-    for i in range(1, cap + 1):
-        run.step(evaluate=False)
-        if i % check_every == 0:
-            st = run.status()
-            if st.gradnorm < 0.1:
-                break
+    if use_solve:
+        rep = run.solve(max_rounds=cap, gradnorm_tol=0.1, rel_change_tol=0, check_every=check_every)
+        i, cost, gradnorm = rep.rounds, rep.cost, rep.gradnorm
+    else:
+        st = None
+        for i in range(1, cap + 1):
+            run.step(evaluate=False)
+            if i % check_every == 0:
+                st = run.status()
+                if st.gradnorm < 0.1:
+                    break
+        cost, gradnorm = st.cost, st.gradnorm
     torch.cuda.synchronize()
-    return {"rounds": i, "wall_s": time.perf_counter() - t0, "cost": st.cost, "gradnorm": st.gradnorm}
+    return {"rounds": i, "wall_s": time.perf_counter() - t0, "cost": cost, "gradnorm": gradnorm}
 
 
 def main():
@@ -92,8 +101,8 @@ def main():
                 for v, kw in RATE_VARIANTS.items():
                     w["rounds_per_s"][v].append(round(rate(torch, edges, n, k, args.rounds, kw), 1))
             for _ in range(2):
-                for v, kw in TOL_VARIANTS.items():
-                    r = to_tol(torch, edges, n, k, kw)
+                for v, (kw, use_solve) in TOL_VARIANTS.items():
+                    r = to_tol(torch, edges, n, k, kw, use_solve)
                     w["to_tol"][v].append({"rounds": r["rounds"], "wall_s": round(r["wall_s"], 4),
                                            "cost": round(r["cost"], 4), "gradnorm": round(r["gradnorm"], 5)})
             res["workloads"][f"{ds}x{k}"] = w
