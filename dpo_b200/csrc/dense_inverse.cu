@@ -7,6 +7,7 @@
 //   A_ij -= C_i Rw_j (i,j != k);  A_ik = -C_i Pinv;  A_kj = Rw_j;  A_kk = Pinv
 // 2 N^3 flops in N/B rank-B updates; each update streams A once (N^2 * 16 B of traffic).
 #include <cuda_runtime.h>
+#include "dpgo_devbuf.cuh"
 #include "dpgo_kernels.cuh"
 
 namespace dpgo {
@@ -124,20 +125,19 @@ __global__ void __launch_bounds__(256) k_gj_update(double *__restrict__ A, int N
 }
 
 cudaError_t dense_spd_inverse(double *A, int N, cudaStream_t stream) {
-  double *piv = nullptr, *Rw = nullptr, *C = nullptr;
+  DevBuf<double> piv, Rw, C;
   cudaError_t e;
-  if ((e = cudaMalloc(&piv, sizeof(double) * GJB * GJB)) != cudaSuccess) return e;
-  if ((e = cudaMalloc(&Rw, sizeof(double) * GJB * (size_t)N)) != cudaSuccess) { cudaFree(piv); return e; }
-  if ((e = cudaMalloc(&C, sizeof(double) * GJB * (size_t)N)) != cudaSuccess) { cudaFree(piv); cudaFree(Rw); return e; }
+  if ((e = piv.alloc((size_t)GJB * GJB)) != cudaSuccess) return e;
+  if ((e = Rw.alloc((size_t)GJB * N)) != cudaSuccess) return e;
+  if ((e = C.alloc((size_t)GJB * N)) != cudaSuccess) return e;
   const int tiles = (N + GJT - 1) / GJT;
   for (int k0 = 0; k0 < N; k0 += GJB) {
     const int bs = (N - k0 < GJB) ? (N - k0) : GJB;
-    k_gj_pivot<<<1, dim3(GJB, GJB), 0, stream>>>(A, N, k0, bs, piv);
-    k_gj_panels<<<(N + 255) / 256, 256, 0, stream>>>(A, N, k0, bs, piv, Rw, C);
-    k_gj_update<<<dim3(tiles, tiles), 256, 0, stream>>>(A, N, k0, bs, piv, Rw, C);
+    k_gj_pivot<<<1, dim3(GJB, GJB), 0, stream>>>(A, N, k0, bs, piv.get());
+    k_gj_panels<<<(N + 255) / 256, 256, 0, stream>>>(A, N, k0, bs, piv.get(), Rw.get(), C.get());
+    k_gj_update<<<dim3(tiles, tiles), 256, 0, stream>>>(A, N, k0, bs, piv.get(), Rw.get(), C.get());
   }
   e = cudaStreamSynchronize(stream);
-  cudaFree(piv); cudaFree(Rw); cudaFree(C);
   if (e != cudaSuccess) return e;
   return cudaGetLastError();
 }

@@ -8,11 +8,15 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <numeric>
 #include <string>
 #include <vector>
 
+#include "dpgo_devbuf.cuh"
 #include "dpgo_kernels.cuh"
+
+using dpgo::DevBuf;
 
 namespace {
 
@@ -41,103 +45,123 @@ int fail(int code, const std::string &msg) {
     if (_s != DPGO_OK) return _s; \
   } while (0)
 
-template <class T> void free_dev(T *&p) {
-  if (p) cudaFree(p);
-  p = nullptr;
-}
-
 }  // namespace
 
 struct dpgo_problem {
+  dpgo::Stream own_stream;       // declared first: destroyed after every buffer, event and graph below
   int n = 0, d = 0, r = 0, dh = 0, N = 0, ts = 0;
   int device = 0, sms = 0, grid = 0, max_grid = 0, max_cluster = 0;
   bool cluster = false;          // the persistent kernel runs as ONE thread-block cluster (small agents)
-  cudaStream_t own_stream = nullptr, stream = nullptr;
-  cudaEvent_t ev_done = nullptr, ev_fork = nullptr;   // fork / join of dpgo_agents_round_async
+  cudaStream_t stream = nullptr;
+  dpgo::Event ev_done, ev_fork;  // fork / join of dpgo_agents_round_async
   uint64_t generation = 0;       // bumped whenever device buffers a captured round refers to may have been replaced
-  struct RoundGraph { std::vector<uint64_t> key; cudaGraphExec_t exec = nullptr; int uses = 0; bool failed = false; };
+  struct RoundGraph { std::vector<uint64_t> key; dpgo::GraphExec exec; int uses = 0; bool failed = false; };
   std::vector<RoundGraph> round_graphs;      // CUDA graphs of the batched round / host I/O calls, kept by the call's first agent
-  template <class Job> struct JobTable { std::vector<uint64_t> key; Job *d_jobs = nullptr; int ctas = 0; };
+  template <class Job> struct JobTable { std::vector<uint64_t> key; DevBuf<Job> jobs; int ctas = 0; };
   int launch_mode = -1;          // -1: by DPGO_CLUSTER_MAX_POSES (default off), 0: full cooperative grid, 1: one thread-block cluster
-  // Q in block-CSR
-  int64_t nb = 0;
-  bool have_Q = false;
-  unsigned precond_mask = 0;
-  int *d_rowptr = nullptr, *d_bcol = nullptr, *d_cta_rows = nullptr;
-  int2 *d_groups = nullptr;      // row groups of the TMA-fed SpMV
-  int ngroups = 0;
-  double *d_bval = nullptr, *d_dinv = nullptr, *d_pinv = nullptr, *d_dense_part = nullptr, *d_dense_t2 = nullptr;
-  int dense_per = 1;
-  int sym_ok = 0;                // symmetric (upper-triangle) dense preconditioner planned
-  double *d_ppack = nullptr;
-  long long *d_sym_off = nullptr;
-  int *d_sym_cut = nullptr, *d_sym_segptr = nullptr, *d_sym_cfirst = nullptr, *d_sym_ccount = nullptr;
-  // host copy of the block-CSR (lazy preconditioner setup) and the sparse exact preconditioner
-  std::vector<int> h_rowptr, h_bcol;
-  std::vector<double> h_bval;
-  bool nd_ready = false;
-  dpgo::KNd nd = {};
-  dpgo::nd::Hierarchy *nd_H = nullptr;
-  int64_t nd_info[16] = {};
+  // Q in block-CSR, its launch tables and its host copy (lazy preconditioner setup): build_from_triplets
+  struct BlockQ {
+    int64_t nb = 0;
+    bool have = false;
+    unsigned precond_mask = 0;
+    DevBuf<int> rowptr, bcol, cta_rows;
+    DevBuf<int2> groups;         // row groups of the TMA-fed SpMV
+    int ngroups = 0;
+    DevBuf<double> bval, dinv, partials;
+    std::vector<int> h_rowptr, h_bcol;
+    std::vector<double> h_bval;
+  } bsr;
+  // the dense exact preconditioner (ensure_dense); dropped whenever Q changes
+  struct Dense {
+    DevBuf<double> pinv, part, t2, ppack;
+    int per = 1;
+    int sym_ok = 0;              // symmetric (upper-triangle) dense preconditioner planned
+    DevBuf<long long> sym_off;
+    DevBuf<int> sym_cut, sym_segptr, sym_cfirst, sym_ccount;
+  } dense;
+  // the sparse exact preconditioner: the nested-dissection factorisation (ensure_nd); dropped whenever Q changes
+  struct Nd {
+    bool ready = false;
+    dpgo::KNd k = {};            // kernel view of the buffers below
+    DevBuf<dpgo::nd::CtaPhase> cta_phase;
+    DevBuf<dpgo::nd::Step> steps;
+    DevBuf<dpgo::nd::Gather> gathers;
+    DevBuf<dpgo::nd::Job> jobs;
+    DevBuf<dpgo::nd::Epi> epis;
+    DevBuf<int> csrc;
+    DevBuf<double> blob, TX, C;
+    std::unique_ptr<dpgo::nd::Hierarchy> H;
+    int64_t info[16] = {};
+  } nd;
   // edge records for the device-side Q assembly / robust re-weighting (dpgo_problem_set_edges)
-  int64_t ne = 0;
-  int *d_e_p1 = nullptr, *d_e_p2 = nullptr, *d_e_fixed = nullptr, *d_cptr = nullptr;
-  int2 *d_contrib = nullptr;
-  double *d_eT = nullptr, *d_eom = nullptr, *d_ew = nullptr, *d_sblk = nullptr, *d_eres = nullptr;
+  struct Edges {
+    int64_t ne = 0;
+    DevBuf<int> p1, p2, fixed, cptr;
+    DevBuf<int2> contrib;
+    DevBuf<double> T, om, w, sblk, res;
+  } edges;
   // vectors
-  double *d_G = nullptr;
-  double *d_acc[3] = {nullptr, nullptr, nullptr};   // Nesterov acceleration: Y, V, XPrev (allocated by accel_init)
-  // accelerated rounds (dpgo_accel.cu): momentum record + ticket on the device; the host's count of begun rounds and the
-  // restart rule of the last begin, which decide whether the agent's next dpgo_agents_accel_round_async restarts
-  double *d_acc_state = nullptr;
-  double *d_acc_part = nullptr;  // accel_ctas(n) per-CTA partials of the finish launch's |X - XPrev|^2
-  unsigned *d_acc_ticket = nullptr;   // [0] begin launch, [1] finish launch (the finish runs on the agent's own stream)
-  long long acc_rounds = 0;
-  bool acc_restart_due = false;
-  std::vector<JobTable<dpgo::AccelJob>> accel_tables;    // job tables of dpgo_agents_accel_begin_async, kept by the call's first agent
-  double *d_vec[dpgo::V_COUNT] = {};
-  double *d_S[2] = {nullptr, nullptr};
-  double *d_partials = nullptr;
-  unsigned *d_bar = nullptr;     // [0] arrival counter, [1] epoch
-  unsigned long long *d_phase_ns = nullptr;   // diagnostic phase clock (8 slots), allocated on request
-  dpgo_opt_result_t *d_result = nullptr;
-  dpgo_opt_result_t *h_result = nullptr;   // pinned
+  DevBuf<double> G, vec[dpgo::V_COUNT], S[2];
+  DevBuf<unsigned> bar;          // [0] arrival counter, [1] epoch
+  DevBuf<unsigned long long> phase_ns;       // diagnostic phase clock (8 slots), allocated on request
+  DevBuf<dpgo_opt_result_t> result;
+  std::unique_ptr<dpgo_opt_result_t, dpgo::CudaFreeHost> h_result;   // pinned
   bool async_pending = false;
   std::chrono::high_resolution_clock::time_point async_t0;
-  // exchange
-  int num_public = 0;
-  int *d_public = nullptr;
-  int *d_pub_slot = nullptr;     // n: public slot of each pose, -1 when the pose is not public
-  bool pub_slot_unique = true;   // no pose is listed twice (the accelerated rounds pack through d_pub_slot)
-  int num_edges = 0, num_shared_poses = 0, max_slot = -1;
+  // exchange: the public poses (dpgo_agent_set_public_poses) and the shared edges (dpgo_agent_set_shared_edges)
+  struct Public {
+    int num = 0;
+    DevBuf<int> pose, slot;      // slot: n, the public slot of each pose, -1 when the pose is not public
+    bool slot_unique = true;     // no pose is listed twice (the accelerated rounds pack through slot)
+  } pub;
+  struct Shared {
+    int num_edges = 0, num_poses = 0, max_slot = -1;
+    DevBuf<int> pose_ids, pose_ptr, slot, out;
+    DevBuf<double> T, om;
+  } shared;
   bool G_dirty = true;           // G may hold values that dpgo_agent_build_G does not overwrite
-  int *d_pose_ids = nullptr, *d_pose_ptr = nullptr, *d_edge_slot = nullptr, *d_edge_out = nullptr;
-  double *d_edge_T = nullptr, *d_edge_om = nullptr;
   // distributed initialisation (dpgo_align.cu): local-frame trajectory, lift, alignment candidates, result
-  double *d_Tloc = nullptr, *d_ylift = nullptr;
-  int align_groups = 0, align_cands = 0, align_max_slot = -1, align_max_nbr = -1;
-  int *d_grp_nbr = nullptr, *d_grp_ptr = nullptr, *d_cand_local = nullptr, *d_cand_slot = nullptr, *d_cand_out = nullptr;
-  double *d_cand_T = nullptr, *d_cand_R = nullptr, *d_cand_t = nullptr, *d_cand_w = nullptr;
-  double *d_T_align = nullptr;
-  int *d_align_info = nullptr;
-  dpgo::AlignJob *d_jobs = nullptr;        // per-call tables of dpgo_agents_align_async (kept by the call's first agent)
-  int *d_ready = nullptr;
+  DevBuf<double> Tloc, ylift;
+  struct Align {
+    int groups = 0, cands = 0, max_slot = -1, max_nbr = -1;
+    DevBuf<int> grp_nbr, grp_ptr, cand_local, cand_slot, cand_out;
+    DevBuf<double> cand_T, cand_R, cand_t, cand_w;
+  } align;
+  DevBuf<double> T_align;
+  DevBuf<int> align_info;
+  DevBuf<dpgo::AlignJob> align_jobs;       // per-call tables of dpgo_agents_align_async (kept by the call's first agent)
+  DevBuf<int> ready;
   int jobs_cap = 0, ready_cap = 0;
-  cudaEvent_t ev_align = nullptr;          // recorded on the stream of the last dpgo_agents_align_async that aligned this agent
+  dpgo::Event ev_align;                    // recorded on the stream of the last dpgo_agents_align_async that aligned this agent
   // team status (dpgo_status.cu): last optimising call's relative change + count, per-CTA partials, ticket of the last CTA
-  double *d_opt_record = nullptr, *d_status_part = nullptr;
-  unsigned *d_status_ticket = nullptr;
-  std::vector<JobTable<dpgo::StatusJob>> status_tables;  // job tables of dpgo_agents_status_async, kept by the call's first agent
-  double *d_anchor = nullptr, *d_traj = nullptr;   // dpgo_agent_trajectory_global
+  struct Status {
+    DevBuf<double> opt_record, part;
+    DevBuf<unsigned> ticket;
+    std::vector<JobTable<dpgo::StatusJob>> tables;   // job tables of dpgo_agents_status_async, kept by the call's first agent
+  } status;
+  DevBuf<double> anchor, traj;   // dpgo_agent_trajectory_global
+  // accelerated rounds: Y, V, XPrev (allocated by accel_init); (dpgo_accel.cu) momentum record + ticket on the device; the
+  // host's count of begun rounds and the restart rule of the last begin, which decide whether the agent's next
+  // dpgo_agents_accel_round_async restarts
+  struct Accel {
+    DevBuf<double> vec[3], state;
+    DevBuf<double> part;         // accel_ctas(n) per-CTA partials of the finish launch's |X - XPrev|^2
+    DevBuf<unsigned> ticket;     // [0] begin launch, [1] finish launch (the finish runs on the agent's own stream)
+    long long rounds = 0;
+    bool restart_due = false;
+    std::vector<JobTable<dpgo::AccelJob>> tables;    // job tables of dpgo_agents_accel_begin_async, kept by the call's first agent
+  } acc;
   // greedy independent-set rounds (dpgo_select.cu), kept by the first agent of a runner on a GPU: the agent graph in CSR
-  // form, the round's k-byte mask, and the selection log (sel_cap rounds of k bytes; sel_rounds issued, the device counts
+  // form, the round's k-byte mask, and the selection log (cap rounds of k bytes; rounds issued, the device counts
   // its own rows).  A grown log retires the old buffer until the next read of the log or the handle's destruction.
-  int sel_k = 0;
-  int *d_sel_ptr = nullptr, *d_sel_adj = nullptr;
-  unsigned char *d_sel_mask = nullptr, *d_sel_log = nullptr;
-  unsigned long long *d_sel_count = nullptr;
-  long long sel_rounds = 0, sel_cap = 0;
-  std::vector<unsigned char *> sel_retired;
+  struct Select {
+    int k = 0;
+    DevBuf<int> ptr, adj;
+    DevBuf<unsigned char> mask, log;
+    DevBuf<unsigned long long> count;
+    long long rounds = 0, cap = 0;
+    std::vector<DevBuf<unsigned char>> retired;
+  } sel;
   const unsigned char *gate = nullptr;     // set for the duration of a gated round: this agent's byte of the mask
 
   size_t vec_bytes() const { return sizeof(double) * (size_t)r * (size_t)N; }
@@ -150,48 +174,47 @@ void fill_kparams(const dpgo_problem *p, dpgo::KParams &kp, int op, const dpgo_o
   kp.N = p->N;
   kp.grid = p->grid;
   kp.op = op;
-  kp.rowptr = p->d_rowptr;
-  kp.bcol = p->d_bcol;
-  kp.bval = p->d_bval;
-  kp.dinv = p->d_dinv;
-  kp.pinv = p->d_pinv;
-  kp.dense_part = p->d_dense_part;
-  kp.dense_per = p->dense_per;
-  kp.sym_ok = p->sym_ok;
-  kp.ppack = p->d_ppack;
-  kp.sym_off = p->d_sym_off;
-  kp.sym_cut = p->d_sym_cut;
-  kp.sym_segptr = p->d_sym_segptr;
-  kp.sym_cfirst = p->d_sym_cfirst;
-  kp.sym_ccount = p->d_sym_ccount;
-  kp.dense_t2 = p->d_dense_t2;
-  kp.cta_rows = p->d_cta_rows;
-  kp.G = p->d_G;
-  for (int i = 0; i < dpgo::V_COUNT; ++i) kp.v[i] = p->d_vec[i];
-  kp.S[0] = p->d_S[0];
-  kp.S[1] = p->d_S[1];
-  kp.partials = p->d_partials;
-  kp.bar_counter = p->d_bar;
-  kp.bar_epoch = p->d_bar + 1;
-  kp.nd = p->nd;
-  if (!p->nd_ready) kp.nd.nphases = 0;
+  kp.rowptr = p->bsr.rowptr.get();
+  kp.bcol = p->bsr.bcol.get();
+  kp.bval = p->bsr.bval.get();
+  kp.dinv = p->bsr.dinv.get();
+  kp.pinv = p->dense.pinv.get();
+  kp.dense_part = p->dense.part.get();
+  kp.dense_per = p->dense.per;
+  kp.sym_ok = p->dense.sym_ok;
+  kp.ppack = p->dense.ppack.get();
+  kp.sym_off = p->dense.sym_off.get();
+  kp.sym_cut = p->dense.sym_cut.get();
+  kp.sym_segptr = p->dense.sym_segptr.get();
+  kp.sym_cfirst = p->dense.sym_cfirst.get();
+  kp.sym_ccount = p->dense.sym_ccount.get();
+  kp.dense_t2 = p->dense.t2.get();
+  kp.cta_rows = p->bsr.cta_rows.get();
+  kp.G = p->G.get();
+  for (int i = 0; i < dpgo::V_COUNT; ++i) kp.v[i] = p->vec[i].get();
+  for (int i = 0; i < 2; ++i) kp.S[i] = p->S[i].get();
+  kp.partials = p->bsr.partials.get();
+  kp.bar_counter = p->bar.get();
+  kp.bar_epoch = p->bar.get() + 1;
+  kp.nd = p->nd.k;
+  if (!p->nd.ready) kp.nd.nphases = 0;
   static const int strict = [] { const char *e = std::getenv("DPGO_STRICT_ACQUIRE"); return (e && e[0] == '1') ? 1 : 0; }();
   kp.strict_acquire = strict;
   kp.cluster = p->cluster ? 1 : 0;
   kp.smem_doubles = 0;
-  kp.phase_ns = p->d_phase_ns;
-  kp.opt_record = p->d_opt_record;
+  kp.phase_ns = p->phase_ns.get();
+  kp.opt_record = p->status.opt_record.get();
   kp.gate = p->gate;
   kp.prm = prm;
-  kp.result = p->d_result;
+  kp.result = p->result.get();
 }
 
 cudaError_t run_spmv(const dpgo_problem *p, const double *X, const double *G, double *out) {
   static const bool force_gather = [] { const char *e = std::getenv("DPGO_SPMV_KERNEL"); return e && std::string(e) == "gather"; }();
-  if (p->ngroups > 0 && !force_gather)
-    return dpgo::launch_spmv_tma(p->r, p->dh, p->ngroups, p->d_groups, p->d_rowptr, p->d_bcol, p->d_bval, X, G, out, p->sms,
-                                 p->stream);
-  return dpgo::launch_spmv(p->r, p->dh, p->n, p->d_rowptr, p->d_bcol, p->d_bval, X, G, out, p->stream);
+  if (p->bsr.ngroups > 0 && !force_gather)
+    return dpgo::launch_spmv_tma(p->r, p->dh, p->bsr.ngroups, p->bsr.groups.get(), p->bsr.rowptr.get(), p->bsr.bcol.get(),
+                                 p->bsr.bval.get(), X, G, out, p->sms, p->stream);
+  return dpgo::launch_spmv(p->r, p->dh, p->n, p->bsr.rowptr.get(), p->bsr.bcol.get(), p->bsr.bval.get(), X, G, out, p->stream);
 }
 
 // Work decomposition of the symmetric (upper-triangle) dense apply (phase_dense_sym) -- host only, also exported as
@@ -266,50 +289,46 @@ bool make_sym_plan(int64_t N, int G, double chunk_cost, SymPlan &pl) {
 // The dense inverse (Q + 0.1 I)^-1 is built on first use (one-shot: scatter block-CSR into N x N in HBM, blocked
 // Gauss-Jordan in place) -- problems that are only evaluated (e.g. the drivers' centralised problem) never pay for it.
 int ensure_dense(dpgo_problem *p) {
-  if (p->d_pinv) return DPGO_OK;
-  if (!(p->precond_mask & (1u << DPGO_PRECOND_DENSE_EXACT)))
+  if (p->dense.pinv) return DPGO_OK;
+  if (!(p->bsr.precond_mask & (1u << DPGO_PRECOND_DENSE_EXACT)))
     return fail(DPGO_ERR_STATE, "dense exact preconditioner was not requested in set_Q (precond_mask)");
   const size_t N = (size_t)p->N;
   if (N * N * sizeof(double) > (size_t)48 << 30)
     return fail(DPGO_ERR_UNSUPPORTED, "dense exact preconditioner limited to N^2*8 <= 48 GiB; use block-Jacobi");
-  p->dense_per = (int)((N + p->grid - 1) / p->grid);
-  if (p->dense_per > dpgo::DENSE_PER_MAX)
+  dpgo_problem::Dense &D = p->dense;
+  D.per = (int)((N + p->grid - 1) / p->grid);
+  if (D.per > dpgo::DENSE_PER_MAX)
     return fail(DPGO_ERR_UNSUPPORTED, "dense exact preconditioner: N too large for the per-CTA slab; use block-Jacobi");
-  DPGO_CUDA(cudaMalloc(&p->d_dense_part, sizeof(double) * (size_t)p->grid * p->r * N));
-  DPGO_CUDA(cudaMemsetAsync(p->d_dense_part, 0, sizeof(double) * (size_t)p->grid * p->r * N, p->stream));
-  DPGO_CUDA(cudaMalloc(&p->d_pinv, N * N * sizeof(double)));
-  DPGO_CUDA(cudaMemsetAsync(p->d_pinv, 0, N * N * sizeof(double), p->stream));
-  cudaError_t e = dpgo::launch_bsr_to_dense(p->n, p->dh, p->nb, p->d_rowptr, p->d_bcol, p->d_bval, 0.1, p->d_pinv, p->N,
-                                            p->stream);
-  if (e == cudaSuccess) e = dpgo::dense_spd_inverse(p->d_pinv, p->N, p->stream);
+  DPGO_CUDA(D.part.alloc((size_t)p->grid * p->r * N));
+  DPGO_CUDA(cudaMemsetAsync(D.part.get(), 0, sizeof(double) * (size_t)p->grid * p->r * N, p->stream));
+  DPGO_CUDA(D.pinv.alloc(N * N));
+  DPGO_CUDA(cudaMemsetAsync(D.pinv.get(), 0, N * N * sizeof(double), p->stream));
+  cudaError_t e = dpgo::launch_bsr_to_dense(p->n, p->dh, p->bsr.nb, p->bsr.rowptr.get(), p->bsr.bcol.get(), p->bsr.bval.get(),
+                                            0.1, D.pinv.get(), p->N, p->stream);
+  if (e == cudaSuccess) e = dpgo::dense_spd_inverse(D.pinv.get(), p->N, p->stream);
   if (e != cudaSuccess) {
-    free_dev(p->d_pinv);
-    free_dev(p->d_dense_part);
+    D = {};
     return fail(DPGO_ERR_CUDA, std::string("dense preconditioner setup: ") + cudaGetErrorString(e));
   }
   // symmetric (upper-triangle) variant: plan, packed copy, partial buffers (falls back to the full matrix otherwise)
   static const bool no_sym = [] { const char *e2 = std::getenv("DPGO_DENSE_FULL"); return e2 && e2[0] == '1'; }();
   static const double chunk_cost = [] { const char *e4 = std::getenv("DPGO_SYM_CHUNK_COST"); return e4 ? std::atof(e4) : SYM_CHUNK_COST; }();
-  p->sym_ok = 0;
+  D.sym_ok = 0;
   SymPlan plan;
   if (!no_sym && make_sym_plan((int64_t)N, p->grid, chunk_cost, plan)) {
     const int nseg = plan.nseg, nchunks = plan.nchunks;
-    DPGO_CUDA(cudaMalloc(&p->d_sym_cut, sizeof(int) * plan.cut.size()));
-    DPGO_CUDA(cudaMalloc(&p->d_sym_segptr, sizeof(int) * plan.segptr.size()));
-    DPGO_CUDA(cudaMalloc(&p->d_sym_cfirst, sizeof(int) * plan.cfirst.size()));
-    DPGO_CUDA(cudaMalloc(&p->d_sym_ccount, sizeof(int) * plan.ccount.size()));
-    DPGO_CUDA(cudaMalloc(&p->d_dense_t2, sizeof(double) * (size_t)nseg * p->r * N));
-    DPGO_CUDA(cudaMemsetAsync(p->d_dense_t2, 0, sizeof(double) * (size_t)nseg * p->r * N, p->stream));
-    DPGO_CUDA(cudaMalloc(&p->d_sym_off, sizeof(long long) * plan.off.size()));
-    DPGO_CUDA(cudaMalloc(&p->d_ppack, sizeof(double) * (size_t)plan.off[(size_t)nchunks]));
-    DPGO_CUDA(cudaMemcpy(p->d_sym_off, plan.off.data(), sizeof(long long) * plan.off.size(), cudaMemcpyHostToDevice));
-    DPGO_CUDA(cudaMemcpy(p->d_sym_cut, plan.cut.data(), sizeof(int) * plan.cut.size(), cudaMemcpyHostToDevice));
-    DPGO_CUDA(cudaMemcpy(p->d_sym_segptr, plan.segptr.data(), sizeof(int) * plan.segptr.size(), cudaMemcpyHostToDevice));
-    DPGO_CUDA(cudaMemcpy(p->d_sym_cfirst, plan.cfirst.data(), sizeof(int) * plan.cfirst.size(), cudaMemcpyHostToDevice));
-    DPGO_CUDA(cudaMemcpy(p->d_sym_ccount, plan.ccount.data(), sizeof(int) * plan.ccount.size(), cudaMemcpyHostToDevice));
-    DPGO_CUDA(dpgo::launch_pack_sym(p->d_pinv, (int)N, nchunks, p->d_sym_segptr, nseg, p->d_sym_off, p->d_ppack, p->stream));
+    DPGO_CUDA(D.t2.alloc((size_t)nseg * p->r * N));
+    DPGO_CUDA(cudaMemsetAsync(D.t2.get(), 0, sizeof(double) * (size_t)nseg * p->r * N, p->stream));
+    DPGO_CUDA(D.ppack.alloc((size_t)plan.off[(size_t)nchunks]));
+    DPGO_CUDA(D.sym_off.assign(plan.off.data(), plan.off.size(), p->stream));
+    DPGO_CUDA(D.sym_cut.assign(plan.cut.data(), plan.cut.size(), p->stream));
+    DPGO_CUDA(D.sym_segptr.assign(plan.segptr.data(), plan.segptr.size(), p->stream));
+    DPGO_CUDA(D.sym_cfirst.assign(plan.cfirst.data(), plan.cfirst.size(), p->stream));
+    DPGO_CUDA(D.sym_ccount.assign(plan.ccount.data(), plan.ccount.size(), p->stream));
+    DPGO_CUDA(dpgo::launch_pack_sym(D.pinv.get(), (int)N, nchunks, D.sym_segptr.get(), nseg, D.sym_off.get(), D.ppack.get(),
+                                    p->stream));
     DPGO_CUDA(cudaStreamSynchronize(p->stream));
-    p->sym_ok = 1;
+    D.sym_ok = 1;
   }
   return DPGO_OK;
 }
@@ -342,77 +361,62 @@ dpgo::nd::Options nd_options(int grid, int r, bool cluster = false) {
   return opt;
 }
 
-template <class T> int upload_array(const std::vector<T> &h, const T *&d, cudaStream_t stream) {
-  T *ptr = nullptr;
-  const size_t bytes = sizeof(T) * std::max<size_t>(h.size(), 1);
-  DPGO_CUDA(cudaMalloc(&ptr, bytes));
-  if (!h.empty()) DPGO_CUDA(cudaMemcpyAsync(ptr, h.data(), sizeof(T) * h.size(), cudaMemcpyHostToDevice, stream));
-  d = ptr;
-  return DPGO_OK;
-}
-
 void free_nd(dpgo_problem *p) {
   ++p->generation;
-  auto fr = [](const void *q) { if (q) cudaFree(const_cast<void *>(q)); };
-  fr(p->nd.cta_phase); fr(p->nd.steps); fr(p->nd.gathers); fr(p->nd.jobs); fr(p->nd.epis); fr(p->nd.csrc);
-  fr(p->nd.blob); fr(p->nd.TX); fr(p->nd.C);
-  p->nd = dpgo::KNd();
-  delete p->nd_H;
-  p->nd_H = nullptr;
-  p->nd_ready = false;
+  p->nd = {};
 }
 
 // The nested-dissection block factorisation of Q + 0.1 I is built on first use (host: ordering, symbolic, plan; the
 // dense algebra of large blocks on the device), like the dense inverse.
 int ensure_nd(dpgo_problem *p) {
-  if (p->nd_ready) return DPGO_OK;
-  if (!(p->precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)))
+  if (p->nd.ready) return DPGO_OK;
+  if (!(p->bsr.precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)))
     return fail(DPGO_ERR_STATE, "sparse exact preconditioner was not requested in set_Q (precond_mask)");
   namespace nd = dpgo::nd;
   free_nd(p);
   nd::Plan plan;
   std::vector<double> blob;
-  nd::Hierarchy *H = new nd::Hierarchy();
+  auto H = std::make_unique<nd::Hierarchy>();
   try {
     const nd::Options opt = nd_options(p->grid, p->r, p->cluster);
-    nd::BsrView Q{p->n, p->dh, p->h_rowptr.data(), p->h_bcol.data(), p->h_bval.data()};
+    nd::BsrView Q{p->n, p->dh, p->bsr.h_rowptr.data(), p->bsr.h_bcol.data(), p->bsr.h_bval.data()};
     nd::build_hierarchy(Q, opt, *H);
     nd::build_numeric(Q, opt, *H, blob);
     nd::build_plan(*H, opt, plan);
   } catch (const std::exception &e) {
-    delete H;
     return fail(DPGO_ERR_UNSUPPORTED, std::string("sparse exact preconditioner setup: ") + e.what());
   }
-  if (plan.max_ytiles > dpgo::ND_YCAP_TILES || plan.max_slots > dpgo::ND_SLOT_CAP) {
-    delete H;
+  if (plan.max_ytiles > dpgo::ND_YCAP_TILES || plan.max_slots > dpgo::ND_SLOT_CAP)
     return fail(DPGO_ERR_UNSUPPORTED, "sparse exact preconditioner: plan exceeds the shared-memory capacities");
-  }
-  p->nd_H = H;
-  nd_fill_info(*H, plan, p->nd_info);
-  if ((int)plan.phases.size() > dpgo::nd::MAX_PHASES) {
-    delete H;
-    p->nd_H = nullptr;
+  dpgo_problem::Nd &F = p->nd;
+  nd_fill_info(*H, plan, F.info);
+  if ((int)plan.phases.size() > dpgo::nd::MAX_PHASES)
     return fail(DPGO_ERR_UNSUPPORTED, "sparse exact preconditioner: too many phases");
-  }
-  for (size_t k = 0; k < plan.phases.size(); ++k) { p->nd.dir[k] = plan.phases[k].dir; p->nd.cta0[k] = plan.phases[k].cta0; }
-  p->nd.max_ytiles = std::max(plan.max_ytiles, 1);
-  p->nd.max_slots = std::max(plan.max_slots, 1);
-  p->nd.max_gathers = p->nd.max_ytiles;          // a step gathers at most what its shared-memory tiles hold
-  DPGO_TRY(upload_array(plan.cta_phase, p->nd.cta_phase, p->stream));
-  DPGO_TRY(upload_array(plan.steps, p->nd.steps, p->stream));
-  DPGO_TRY(upload_array(plan.gathers, p->nd.gathers, p->stream));
-  DPGO_TRY(upload_array(plan.jobs, p->nd.jobs, p->stream));
-  DPGO_TRY(upload_array(plan.epis, p->nd.epis, p->stream));
-  DPGO_TRY(upload_array(plan.csrc, p->nd.csrc, p->stream));
-  DPGO_TRY(upload_array(blob, p->nd.blob, p->stream));
-  const size_t tile = sizeof(double) * (size_t)p->ts;
-  DPGO_CUDA(cudaMalloc(&p->nd.TX, tile * (size_t)p->n));
-  DPGO_CUDA(cudaMalloc(&p->nd.C, tile * (size_t)H->cbuf_tiles));
-  DPGO_CUDA(cudaMemsetAsync(p->nd.TX, 0, tile * (size_t)p->n, p->stream));
-  DPGO_CUDA(cudaMemsetAsync(p->nd.C, 0, tile * (size_t)H->cbuf_tiles, p->stream));
+  F.H = std::move(H);
+  dpgo::KNd &K = F.k;
+  for (size_t k = 0; k < plan.phases.size(); ++k) { K.dir[k] = plan.phases[k].dir; K.cta0[k] = plan.phases[k].cta0; }
+  K.max_ytiles = std::max(plan.max_ytiles, 1);
+  K.max_slots = std::max(plan.max_slots, 1);
+  K.max_gathers = K.max_ytiles;          // a step gathers at most what its shared-memory tiles hold
+  DPGO_CUDA(F.cta_phase.assign(plan.cta_phase.data(), plan.cta_phase.size(), p->stream));
+  DPGO_CUDA(F.steps.assign(plan.steps.data(), plan.steps.size(), p->stream));
+  DPGO_CUDA(F.gathers.assign(plan.gathers.data(), plan.gathers.size(), p->stream));
+  DPGO_CUDA(F.jobs.assign(plan.jobs.data(), plan.jobs.size(), p->stream));
+  DPGO_CUDA(F.epis.assign(plan.epis.data(), plan.epis.size(), p->stream));
+  DPGO_CUDA(F.csrc.assign(plan.csrc.data(), plan.csrc.size(), p->stream));
+  DPGO_CUDA(F.blob.assign(blob.data(), blob.size(), p->stream));
+  K.cta_phase = F.cta_phase.get(); K.steps = F.steps.get(); K.gathers = F.gathers.get(); K.jobs = F.jobs.get();
+  K.epis = F.epis.get(); K.csrc = F.csrc.get(); K.blob = F.blob.get();
+  const size_t tile = (size_t)p->ts;
+  DPGO_CUDA(F.TX.alloc(tile * (size_t)p->n));
+  DPGO_CUDA(F.C.alloc(tile * (size_t)F.H->cbuf_tiles));
+  K.TX = F.TX.get();
+  K.C = F.C.get();
+  DPGO_CUDA(cudaMemsetAsync(K.TX, 0, sizeof(double) * tile * (size_t)p->n, p->stream));
+  DPGO_CUDA(cudaMemsetAsync(K.C, 0, sizeof(double) * tile * (size_t)F.H->cbuf_tiles, p->stream));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
-  p->nd.nphases = (int)plan.phases.size();
-  p->nd_ready = true;
+  K.nphases = (int)plan.phases.size();
+  F.ready = true;
   ++p->generation;
   return DPGO_OK;
 }
@@ -420,14 +424,14 @@ int ensure_nd(dpgo_problem *p) {
 int check_precond(dpgo_problem *p, int precond) {
   if (precond < 0 || precond > 3) return fail(DPGO_ERR_INVALID_ARG, "unknown preconditioner id");
   if (precond == DPGO_PRECOND_SPARSE_EXACT) return ensure_nd(p);
-  if (precond == DPGO_PRECOND_BLOCK_JACOBI && !p->d_dinv)
+  if (precond == DPGO_PRECOND_BLOCK_JACOBI && !p->bsr.dinv)
     return fail(DPGO_ERR_STATE, "block-Jacobi preconditioner was not prepared by set_Q (precond_mask)");
   if (precond == DPGO_PRECOND_DENSE_EXACT) return ensure_dense(p);
   return DPGO_OK;
 }
 
 int run_op(dpgo_problem *p, int op, const dpgo_opt_params_t &prm) {
-  DPGO_REQUIRE(p->have_Q, DPGO_ERR_STATE, "set_Q has not been called");
+  DPGO_REQUIRE(p->bsr.have, DPGO_ERR_STATE, "set_Q has not been called");
   dpgo::KParams kp;
   fill_kparams(p, kp, op, prm);
   DPGO_CUDA(dpgo::launch_optimize(p->r, p->dh, kp, p->stream));
@@ -547,35 +551,26 @@ int build_from_triplets(dpgo_problem *p, std::vector<BlockTriplet> &trip, unsign
 
   // upload
   cudaSetDevice(p->device);
-  free_dev(p->d_rowptr); free_dev(p->d_bcol); free_dev(p->d_bval); free_dev(p->d_dinv); free_dev(p->d_pinv);
-  free_dev(p->d_cta_rows); free_dev(p->d_partials); free_dev(p->d_dense_part); free_dev(p->d_groups);
-  free_dev(p->d_dense_t2); free_dev(p->d_ppack); free_dev(p->d_sym_off); free_dev(p->d_sym_cut); free_dev(p->d_sym_segptr); free_dev(p->d_sym_cfirst); free_dev(p->d_sym_ccount);
-  p->sym_ok = 0;
-  p->have_Q = false;
-  p->ngroups = 0;
+  p->bsr = {};
+  p->dense = {};
   free_nd(p);
-  p->h_rowptr = rowptr;
-  p->h_bcol = bcol;
-  p->h_bval = bval;
+  dpgo_problem::BlockQ &B = p->bsr;
+  B.h_rowptr = rowptr;
+  B.h_bcol = bcol;
+  B.h_bval = bval;
   // +8 ints of slack: the bulk-TMA windows are rounded out to 16 bytes
-  DPGO_CUDA(cudaMalloc(&p->d_rowptr, sizeof(int) * (n + 1 + 8)));
-  DPGO_CUDA(cudaMalloc(&p->d_bcol, sizeof(int) * (std::max<int64_t>(nb, 1) + 8)));
-  DPGO_CUDA(cudaMemsetAsync(p->d_rowptr, 0, sizeof(int) * (n + 1 + 8), p->stream));
-  DPGO_CUDA(cudaMemsetAsync(p->d_bcol, 0, sizeof(int) * (std::max<int64_t>(nb, 1) + 8), p->stream));
-  DPGO_CUDA(cudaMalloc(&p->d_bval, sizeof(double) * 16 * std::max<int64_t>(nb, 1)));
-  DPGO_CUDA(cudaMalloc(&p->d_cta_rows, sizeof(int) * (grid + 1)));
-  DPGO_CUDA(cudaMalloc(&p->d_partials, sizeof(double) * 2 * grid * dpgo::NRED));
-  DPGO_CUDA(cudaMemcpyAsync(p->d_rowptr, rowptr.data(), sizeof(int) * (n + 1), cudaMemcpyHostToDevice, p->stream));
-  if (nb) {
-    DPGO_CUDA(cudaMemcpyAsync(p->d_bcol, bcol.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, p->stream));
-    DPGO_CUDA(cudaMemcpyAsync(p->d_bval, bval.data(), sizeof(double) * 16 * nb, cudaMemcpyHostToDevice, p->stream));
-  }
-  DPGO_CUDA(cudaMemcpyAsync(p->d_cta_rows, cta_rows.data(), sizeof(int) * (grid + 1), cudaMemcpyHostToDevice, p->stream));
-  DPGO_CUDA(cudaMemsetAsync(p->d_partials, 0, sizeof(double) * 2 * grid * dpgo::NRED, p->stream));
-  if (!dinv.empty()) {
-    DPGO_CUDA(cudaMalloc(&p->d_dinv, sizeof(double) * dinv.size()));
-    DPGO_CUDA(cudaMemcpyAsync(p->d_dinv, dinv.data(), sizeof(double) * dinv.size(), cudaMemcpyHostToDevice, p->stream));
-  }
+  DPGO_CUDA(B.rowptr.alloc((size_t)n + 1 + 8));
+  DPGO_CUDA(B.bcol.alloc((size_t)std::max<int64_t>(nb, 1) + 8));
+  DPGO_CUDA(cudaMemsetAsync(B.rowptr.get(), 0, sizeof(int) * (n + 1 + 8), p->stream));
+  DPGO_CUDA(cudaMemsetAsync(B.bcol.get(), 0, sizeof(int) * (std::max<int64_t>(nb, 1) + 8), p->stream));
+  DPGO_CUDA(B.bval.alloc(16 * (size_t)std::max<int64_t>(nb, 1)));
+  DPGO_CUDA(B.cta_rows.assign(cta_rows.data(), cta_rows.size(), p->stream));
+  DPGO_CUDA(B.partials.alloc((size_t)2 * grid * dpgo::NRED));
+  DPGO_CUDA(B.rowptr.upload(rowptr.data(), (size_t)n + 1, p->stream));
+  DPGO_CUDA(B.bcol.upload(bcol.data(), (size_t)nb, p->stream));
+  DPGO_CUDA(B.bval.upload(bval.data(), 16 * (size_t)nb, p->stream));
+  DPGO_CUDA(cudaMemsetAsync(B.partials.get(), 0, sizeof(double) * 2 * grid * dpgo::NRED, p->stream));
+  if (!dinv.empty()) DPGO_CUDA(B.dinv.assign(dinv.data(), dinv.size(), p->stream));
   // row groups for the TMA-fed SpMV: consecutive rows, <= SPMV_GROUP_BLOCKS blocks and rows each
   {
     const int BT = dpgo::spmv_group_blocks();
@@ -594,30 +589,29 @@ int build_from_triplets(dpgo_problem *p, std::vector<BlockTriplet> &trip, unsign
     }
     if (ok && nb > 0) {
       groups.push_back(make_int2(n, (int)nb));
-      DPGO_CUDA(cudaMalloc(&p->d_groups, sizeof(int2) * groups.size()));
-      DPGO_CUDA(cudaMemcpyAsync(p->d_groups, groups.data(), sizeof(int2) * groups.size(), cudaMemcpyHostToDevice, p->stream));
-      p->ngroups = (int)groups.size() - 1;
+      DPGO_CUDA(B.groups.assign(groups.data(), groups.size(), p->stream));
+      B.ngroups = (int)groups.size() - 1;
     }
   }
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
-  p->nb = nb;
+  B.nb = nb;
   p->grid = grid;
-  p->precond_mask = precond_mask;
+  B.precond_mask = precond_mask;
 
-  p->have_Q = true;
+  B.have = true;
   return DPGO_OK;
 }
 
 int upload_vec(dpgo_problem *p, int id, const double *host) {
-  DPGO_CUDA(cudaMemcpyAsync(p->d_vec[id], host, p->vec_bytes(), cudaMemcpyHostToDevice, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(p->vec[id].get(), host, p->vec_bytes(), cudaMemcpyHostToDevice, p->stream));
   return DPGO_OK;
 }
 int download_vec(dpgo_problem *p, int id, double *host) {
-  DPGO_CUDA(cudaMemcpyAsync(host, p->d_vec[id], p->vec_bytes(), cudaMemcpyDeviceToHost, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(host, p->vec[id].get(), p->vec_bytes(), cudaMemcpyDeviceToHost, p->stream));
   return DPGO_OK;
 }
 int fetch_result(dpgo_problem *p) {
-  DPGO_CUDA(cudaMemcpyAsync(p->h_result, p->d_result, sizeof(dpgo_opt_result_t), cudaMemcpyDeviceToHost, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(p->h_result.get(), p->result.get(), sizeof(dpgo_opt_result_t), cudaMemcpyDeviceToHost, p->stream));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
 }
@@ -685,33 +679,37 @@ int dpgo_problem_create(int n, int d, int r, int device, dpgo_problem_t **out) {
   auto bail = [&](int code, const std::string &m) { dpgo_problem_destroy(p); return fail(code, m); };
   if (cudaDeviceGetAttribute(&p->sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess)
     return bail(DPGO_ERR_CUDA, "cudaDeviceGetAttribute failed");
-  if (cudaStreamCreateWithFlags(&p->own_stream, cudaStreamNonBlocking) != cudaSuccess)
-    return bail(DPGO_ERR_CUDA, "cudaStreamCreate failed");
-  p->stream = p->own_stream;
+  cudaStream_t own = nullptr;
+  const cudaError_t se = cudaStreamCreateWithFlags(&own, cudaStreamNonBlocking);
+  p->own_stream.reset(own);
+  if (se != cudaSuccess) return bail(DPGO_ERR_CUDA, "cudaStreamCreate failed");
+  p->stream = own;
   p->max_grid = dpgo::optimize_max_grid(r, d + 1, device);
   p->max_cluster = dpgo::optimize_max_cluster(r, d + 1, device);
   if (p->max_grid <= 0) return bail(DPGO_ERR_CUDA, "persistent kernel cannot be made resident on this device");
   const size_t vb = p->vec_bytes();
   for (int i = 0; i < dpgo::V_COUNT; ++i) {
-    if (cudaMalloc(&p->d_vec[i], vb) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed (vectors)");
-    cudaMemsetAsync(p->d_vec[i], 0, vb, p->stream);
+    if (p->vec[i].alloc((size_t)r * p->N) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed (vectors)");
+    cudaMemsetAsync(p->vec[i].get(), 0, vb, p->stream);
   }
-  if (cudaMalloc(&p->d_G, vb) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed (G)");
-  cudaMemsetAsync(p->d_G, 0, vb, p->stream);
+  if (p->G.alloc((size_t)r * p->N) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed (G)");
+  cudaMemsetAsync(p->G.get(), 0, vb, p->stream);
   for (int i = 0; i < 2; ++i) {
-    if (cudaMalloc(&p->d_S[i], sizeof(double) * 9 * (size_t)n) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed (S)");
-    cudaMemsetAsync(p->d_S[i], 0, sizeof(double) * 9 * (size_t)n, p->stream);
+    if (p->S[i].alloc(9 * (size_t)n) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed (S)");
+    cudaMemsetAsync(p->S[i].get(), 0, sizeof(double) * 9 * (size_t)n, p->stream);
   }
-  if (cudaMalloc(&p->d_bar, 2 * sizeof(unsigned)) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed");
-  cudaMemsetAsync(p->d_bar, 0, 2 * sizeof(unsigned), p->stream);
-  if (cudaMalloc(&p->d_result, sizeof(dpgo_opt_result_t)) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed");
-  if (cudaMalloc(&p->d_opt_record, 2 * sizeof(double)) != cudaSuccess ||
-      cudaMalloc(&p->d_status_part, sizeof(double) * 3 * (size_t)dpgo::status_ctas(n)) != cudaSuccess ||
-      cudaMalloc(&p->d_status_ticket, sizeof(unsigned)) != cudaSuccess)
+  if (p->bar.alloc(2) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed");
+  cudaMemsetAsync(p->bar.get(), 0, 2 * sizeof(unsigned), p->stream);
+  if (p->result.alloc(1) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "device allocation failed");
+  if (p->status.opt_record.alloc(2) != cudaSuccess || p->status.part.alloc(3 * (size_t)dpgo::status_ctas(n)) != cudaSuccess ||
+      p->status.ticket.alloc(1) != cudaSuccess)
     return bail(DPGO_ERR_ALLOC, "device allocation failed (status)");
-  cudaMemsetAsync(p->d_opt_record, 0, 2 * sizeof(double), p->stream);
-  cudaMemsetAsync(p->d_status_ticket, 0, sizeof(unsigned), p->stream);
-  if (cudaMallocHost(&p->h_result, sizeof(dpgo_opt_result_t)) != cudaSuccess) return bail(DPGO_ERR_ALLOC, "pinned allocation failed");
+  cudaMemsetAsync(p->status.opt_record.get(), 0, 2 * sizeof(double), p->stream);
+  cudaMemsetAsync(p->status.ticket.get(), 0, sizeof(unsigned), p->stream);
+  dpgo_opt_result_t *pinned = nullptr;
+  const cudaError_t he = cudaMallocHost(&pinned, sizeof(dpgo_opt_result_t));
+  p->h_result.reset(pinned);
+  if (he != cudaSuccess) return bail(DPGO_ERR_ALLOC, "pinned allocation failed");
   if (cudaStreamSynchronize(p->stream) != cudaSuccess) return bail(DPGO_ERR_CUDA, "device initialisation failed");
   // empty Q (ref: ctor calls setQ(SparseMatrix(N,N)), src/QuadraticProblem.cpp:23)
   std::vector<BlockTriplet> none;
@@ -725,34 +723,6 @@ int dpgo_problem_destroy(dpgo_problem_t *p) {
   if (!p) return DPGO_OK;
   cudaSetDevice(p->device);
   if (p->stream) cudaStreamSynchronize(p->stream);
-  free_dev(p->d_rowptr); free_dev(p->d_bcol); free_dev(p->d_cta_rows); free_dev(p->d_bval); free_dev(p->d_groups);
-  free_dev(p->d_dinv); free_dev(p->d_pinv); free_dev(p->d_dense_part); free_dev(p->d_G);
-  free_dev(p->d_dense_t2); free_dev(p->d_ppack); free_dev(p->d_sym_off); free_dev(p->d_sym_cut); free_dev(p->d_sym_segptr); free_dev(p->d_sym_cfirst); free_dev(p->d_sym_ccount);
-  for (int i = 0; i < dpgo::V_COUNT; ++i) free_dev(p->d_vec[i]);
-  free_dev(p->d_S[0]); free_dev(p->d_S[1]); free_dev(p->d_partials); free_dev(p->d_bar); free_dev(p->d_phase_ns); free_dev(p->d_result);
-  free_dev(p->d_acc[0]); free_dev(p->d_acc[1]); free_dev(p->d_acc[2]);
-  free_dev(p->d_e_p1); free_dev(p->d_e_p2); free_dev(p->d_e_fixed); free_dev(p->d_cptr); free_dev(p->d_contrib);
-  free_dev(p->d_eT); free_dev(p->d_eom); free_dev(p->d_ew); free_dev(p->d_sblk); free_dev(p->d_eres);
-  free_dev(p->d_public); free_dev(p->d_pose_ids); free_dev(p->d_pose_ptr); free_dev(p->d_edge_slot);
-  free_dev(p->d_edge_out); free_dev(p->d_edge_T); free_dev(p->d_edge_om);
-  free_dev(p->d_Tloc); free_dev(p->d_ylift); free_dev(p->d_grp_nbr); free_dev(p->d_grp_ptr); free_dev(p->d_cand_local);
-  free_dev(p->d_cand_slot); free_dev(p->d_cand_out); free_dev(p->d_cand_T); free_dev(p->d_cand_R); free_dev(p->d_cand_t);
-  free_dev(p->d_cand_w); free_dev(p->d_T_align); free_dev(p->d_align_info); free_dev(p->d_jobs); free_dev(p->d_ready);
-  free_dev(p->d_opt_record); free_dev(p->d_status_part); free_dev(p->d_status_ticket); free_dev(p->d_anchor); free_dev(p->d_traj);
-  for (auto &t : p->status_tables) free_dev(t.d_jobs);
-  free_dev(p->d_acc_state); free_dev(p->d_acc_part); free_dev(p->d_acc_ticket); free_dev(p->d_pub_slot);
-  for (auto &t : p->accel_tables) free_dev(t.d_jobs);
-  free_nd(p);
-  if (p->h_result) cudaFreeHost(p->h_result);
-  for (auto &g : p->round_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-  p->round_graphs.clear();
-  free_dev(p->d_sel_ptr); free_dev(p->d_sel_adj); free_dev(p->d_sel_mask); free_dev(p->d_sel_log); free_dev(p->d_sel_count);
-  for (auto *b : p->sel_retired) cudaFree(b);
-  p->sel_retired.clear();
-  if (p->ev_done) cudaEventDestroy(p->ev_done);
-  if (p->ev_fork) cudaEventDestroy(p->ev_fork);
-  if (p->ev_align) cudaEventDestroy(p->ev_align);
-  if (p->own_stream) cudaStreamDestroy(p->own_stream);
   delete p;
   return DPGO_OK;
 }
@@ -760,7 +730,7 @@ int dpgo_problem_destroy(dpgo_problem_t *p) {
 int dpgo_problem_set_stream(dpgo_problem_t *p, void *cuda_stream) {
   DPGO_CHECK_HANDLE(p);
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
-  p->stream = cuda_stream ? (cudaStream_t)cuda_stream : p->own_stream;
+  p->stream = cuda_stream ? (cudaStream_t)cuda_stream : p->own_stream.get();
   return DPGO_OK;
 }
 
@@ -790,7 +760,7 @@ int dpgo_problem_dims(const dpgo_problem_t *p, int *n, int *d, int *r, int64_t *
   if (n) *n = p->n;
   if (d) *d = p->d;
   if (r) *r = p->r;
-  if (num_blocks) *num_blocks = p->nb;
+  if (num_blocks) *num_blocks = p->bsr.nb;
   return DPGO_OK;
 }
 
@@ -853,9 +823,9 @@ int dpgo_problem_set_G_dense(dpgo_problem_t *p, const double *G_host) {
   DPGO_CHECK_HANDLE(p);
   p->G_dirty = true;
   if (!G_host) {
-    DPGO_CUDA(cudaMemsetAsync(p->d_G, 0, p->vec_bytes(), p->stream));
+    DPGO_CUDA(cudaMemsetAsync(p->G.get(), 0, p->vec_bytes(), p->stream));
   } else {
-    DPGO_CUDA(cudaMemcpyAsync(p->d_G, G_host, p->vec_bytes(), cudaMemcpyHostToDevice, p->stream));
+    DPGO_CUDA(cudaMemcpyAsync(p->G.get(), G_host, p->vec_bytes(), cudaMemcpyHostToDevice, p->stream));
   }
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
@@ -905,9 +875,9 @@ int dpgo_problem_egrad(dpgo_problem_t *p, const double *X_host, double *out_host
 int dpgo_problem_ehess(dpgo_problem_t *p, const double *V_host, double *out_host) {
   DPGO_CHECK_HANDLE(p);
   DPGO_REQUIRE(V_host && out_host, DPGO_ERR_INVALID_ARG, "null argument");
-  DPGO_REQUIRE(p->have_Q, DPGO_ERR_STATE, "set_Q has not been called");
+  DPGO_REQUIRE(p->bsr.have, DPGO_ERR_STATE, "set_Q has not been called");
   DPGO_TRY(upload_vec(p, dpgo::V_AUX, V_host));
-  DPGO_CUDA(run_spmv(p, p->d_vec[dpgo::V_AUX], nullptr, p->d_vec[dpgo::V_HD]));
+  DPGO_CUDA(run_spmv(p, p->vec[dpgo::V_AUX].get(), nullptr, p->vec[dpgo::V_HD].get()));
   DPGO_TRY(download_vec(p, dpgo::V_HD, out_host));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
@@ -982,7 +952,7 @@ int dpgo_manifold_project(dpgo_problem_t *p, const double *M_host, double *out_h
   DPGO_CHECK_HANDLE(p);
   DPGO_REQUIRE(M_host && out_host, DPGO_ERR_INVALID_ARG, "null argument");
   DPGO_TRY(upload_vec(p, dpgo::V_AUX, M_host));
-  DPGO_CUDA(dpgo::launch_stiefel_project(p->r, p->dh, p->n, p->d_vec[dpgo::V_AUX], p->d_vec[dpgo::V_T], p->stream));
+  DPGO_CUDA(dpgo::launch_stiefel_project(p->r, p->dh, p->n, p->vec[dpgo::V_AUX].get(), p->vec[dpgo::V_T].get(), p->stream));
   DPGO_TRY(download_vec(p, dpgo::V_T, out_host));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
@@ -1045,19 +1015,19 @@ int dpgo_problem_download_X_async(dpgo_problem_t *p, double *X_host) {
 int dpgo_problem_copy_X_from_device(dpgo_problem_t *p, const double *X_dev) {
   DPGO_CHECK_HANDLE(p);
   DPGO_REQUIRE(X_dev, DPGO_ERR_INVALID_ARG, "null X");
-  DPGO_CUDA(cudaMemcpyAsync(p->d_vec[dpgo::V_X0], X_dev, p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(p->vec[dpgo::V_X0].get(), X_dev, p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
   return DPGO_OK;
 }
 
 int dpgo_problem_device_X(dpgo_problem_t *p, double **X_dev) {
   DPGO_REQUIRE(p && X_dev, DPGO_ERR_INVALID_ARG, "null argument");
-  *X_dev = p->d_vec[dpgo::V_X0];
+  *X_dev = p->vec[dpgo::V_X0].get();
   return DPGO_OK;
 }
 
 int dpgo_problem_device_G(dpgo_problem_t *p, double **G_dev) {
   DPGO_REQUIRE(p && G_dev, DPGO_ERR_INVALID_ARG, "null argument");
-  *G_dev = p->d_G;
+  *G_dev = p->G.get();
   p->G_dirty = true;             // the caller may write G directly
   return DPGO_OK;
 }
@@ -1089,22 +1059,20 @@ int dpgo_debug_phase_latency(dpgo_problem_t *p, int phases, double *us_per_phase
   dpgo_opt_params_t prm;
   dpgo_opt_params_default(&prm);
   prm.precond = DPGO_PRECOND_NONE;
-  cudaEvent_t e0, e1;
-  DPGO_CUDA(cudaEventCreate(&e0));
-  DPGO_CUDA(cudaEventCreate(&e1));
+  dpgo::Event e0, e1;
+  DPGO_CUDA(dpgo::create_event(e0, cudaEventDefault));
+  DPGO_CUDA(dpgo::create_event(e1, cudaEventDefault));
   float ms[2] = {0, 0};
   const int counts[2] = {1, phases + 1};
   for (int rep = 0; rep < 2; ++rep) {
     prm.tr_max_inner = counts[rep];
     for (int w = 0; w < 3; ++w) DPGO_TRY(run_op(p, dpgo::OP_PHASE_BENCH, prm));
-    DPGO_CUDA(cudaEventRecord(e0, p->stream));
+    DPGO_CUDA(cudaEventRecord(e0.get(), p->stream));
     for (int w = 0; w < 10; ++w) DPGO_TRY(run_op(p, dpgo::OP_PHASE_BENCH, prm));
-    DPGO_CUDA(cudaEventRecord(e1, p->stream));
-    DPGO_CUDA(cudaEventSynchronize(e1));
-    DPGO_CUDA(cudaEventElapsedTime(&ms[rep], e0, e1));
+    DPGO_CUDA(cudaEventRecord(e1.get(), p->stream));
+    DPGO_CUDA(cudaEventSynchronize(e1.get()));
+    DPGO_CUDA(cudaEventElapsedTime(&ms[rep], e0.get(), e1.get()));
   }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
   *us_per_phase = 1e3 * (ms[1] - ms[0]) / 10.0 / phases;
   if (us_launch) *us_launch = 1e3 * ms[0] / 10.0 - *us_per_phase;
   return DPGO_OK;
@@ -1112,18 +1080,18 @@ int dpgo_debug_phase_latency(dpgo_problem_t *p, int phases, double *us_per_phase
 
 static int phase_times_impl(dpgo_problem_t *p, int enable, double *ms_by_kind, int nout) {
   DPGO_CHECK_HANDLE(p);
-  if (enable && !p->d_phase_ns) {
-    DPGO_CUDA(cudaMalloc(&p->d_phase_ns, 64 * sizeof(unsigned long long)));
-    DPGO_CUDA(cudaMemsetAsync(p->d_phase_ns, 0, 64 * sizeof(unsigned long long), p->stream));
+  if (enable && !p->phase_ns) {
+    DPGO_CUDA(p->phase_ns.alloc(64));
+    DPGO_CUDA(cudaMemsetAsync(p->phase_ns.get(), 0, 64 * sizeof(unsigned long long), p->stream));
   }
-  if (p->d_phase_ns) {
+  if (p->phase_ns) {
     unsigned long long ns[64];
     DPGO_CUDA(cudaStreamSynchronize(p->stream));
-    DPGO_CUDA(cudaMemcpy(ns, p->d_phase_ns, sizeof(ns), cudaMemcpyDeviceToHost));
+    DPGO_CUDA(cudaMemcpy(ns, p->phase_ns.get(), sizeof(ns), cudaMemcpyDeviceToHost));
     if (ms_by_kind)
       for (int i = 0; i < nout; ++i) ms_by_kind[i] = 1e-6 * (double)ns[i];
-    DPGO_CUDA(cudaMemset(p->d_phase_ns, 0, sizeof(ns)));
-    if (!enable) { cudaFree(p->d_phase_ns); p->d_phase_ns = nullptr; }
+    DPGO_CUDA(cudaMemset(p->phase_ns.get(), 0, sizeof(ns)));
+    if (!enable) p->phase_ns = {};
   } else if (ms_by_kind) {
     for (int i = 0; i < nout; ++i) ms_by_kind[i] = 0.0;
   }
@@ -1137,8 +1105,8 @@ int dpgo_debug_phase_times64(dpgo_problem_t *p, int enable, double *ms_by_kind) 
 int dpgo_spmv_device(dpgo_problem_t *p, const double *X_dev, double *out_dev, int add_G) {
   DPGO_CHECK_HANDLE(p);
   DPGO_REQUIRE(X_dev && out_dev, DPGO_ERR_INVALID_ARG, "null argument");
-  DPGO_REQUIRE(p->have_Q, DPGO_ERR_STATE, "set_Q has not been called");
-  DPGO_CUDA(run_spmv(p, X_dev, add_G ? p->d_G : nullptr, out_dev));
+  DPGO_REQUIRE(p->bsr.have, DPGO_ERR_STATE, "set_Q has not been called");
+  DPGO_CUDA(run_spmv(p, X_dev, add_G ? p->G.get() : nullptr, out_dev));
   return DPGO_OK;
 }
 
@@ -1146,7 +1114,7 @@ int64_t dpgo_spmv_algorithmic_bytes(const dpgo_problem_t *p, int add_G) {
   if (!p) return 0;
   // SURVEY 8(d): nb*((d+1)^2*8 + 4) + (n+1)*4 + 2*r*(d+1)*n*8 (+ r*(d+1)*n*8 if G is read)
   const int64_t dh = p->dh;
-  int64_t b = p->nb * (dh * dh * 8 + 4) + ((int64_t)p->n + 1) * 4 + 2 * (int64_t)p->r * dh * p->n * 8;
+  int64_t b = p->bsr.nb * (dh * dh * 8 + 4) + ((int64_t)p->n + 1) * 4 + 2 * (int64_t)p->r * dh * p->n * 8;
   if (add_G) b += (int64_t)p->r * dh * p->n * 8;
   return b;
 }
@@ -1180,20 +1148,20 @@ int64_t dpgo_precond_algorithmic_bytes(const dpgo_problem_t *p, int precondition
   if (!p) return 0;
   const int64_t N = (int64_t)p->dh * p->n, vec = (int64_t)p->r * N * 8;
   if (preconditioner == DPGO_PRECOND_BLOCK_JACOBI) return (int64_t)p->n * 16 * 8 + 2 * vec;
-  if (preconditioner == DPGO_PRECOND_SPARSE_EXACT) return p->nd_ready ? p->nd_info[4] + 2 * vec : 0;
+  if (preconditioner == DPGO_PRECOND_SPARSE_EXACT) return p->nd.ready ? p->nd.info[4] + 2 * vec : 0;
   if (preconditioner != DPGO_PRECOND_DENSE_EXACT) return 0;
   // the inverse is symmetric: the unique data is its upper triangle in 8-row groups (what phase_dense_sym reads);
   // the full-matrix variants read all of it
-  const int64_t mat = p->sym_ok ? (N * N + 8 * N) / 2 * 8 : N * N * 8;
+  const int64_t mat = p->dense.sym_ok ? (N * N + 8 * N) / 2 * 8 : N * N * 8;
   return mat + 2 * vec;
 }
 
 int dpgo_nd_info(dpgo_problem_t *p, int64_t *info16) {
   DPGO_CHECK_HANDLE(p);
   DPGO_REQUIRE(info16, DPGO_ERR_INVALID_ARG, "null argument");
-  DPGO_REQUIRE(p->have_Q, DPGO_ERR_STATE, "set_Q has not been called");
+  DPGO_REQUIRE(p->bsr.have, DPGO_ERR_STATE, "set_Q has not been called");
   DPGO_TRY(ensure_nd(p));
-  std::copy(p->nd_info, p->nd_info + 16, info16);
+  std::copy(p->nd.info, p->nd.info + 16, info16);
   return DPGO_OK;
 }
 
@@ -1259,20 +1227,21 @@ int dpgo_nd_debug_emulate(int n, int d, int r, int64_t nb, const int32_t *brow, 
 
 // ---- Q from edge records on the device, robust re-weighting -----------------------------------------------------
 static int reassemble_Q(dpgo_problem *p) {
-  DPGO_CUDA(dpgo::launch_assemble_Q(p->nb, p->d_cptr, p->d_contrib, p->d_eT, p->d_eom, p->d_ew, p->d_sblk, p->d_bval, p->stream));
+  const dpgo_problem::Edges &E = p->edges;
+  DPGO_CUDA(dpgo::launch_assemble_Q(p->bsr.nb, E.cptr.get(), E.contrib.get(), E.T.get(), E.om.get(), E.w.get(), E.sblk.get(),
+                                    p->bsr.bval.get(), p->stream));
   // the host copy feeds the lazily built exact preconditioners; block-Jacobi blocks are refreshed right away
-  DPGO_CUDA(cudaMemcpyAsync(p->h_bval.data(), p->d_bval, sizeof(double) * 16 * (size_t)p->nb, cudaMemcpyDeviceToHost, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(p->bsr.h_bval.data(), p->bsr.bval.get(), sizeof(double) * 16 * (size_t)p->bsr.nb,
+                            cudaMemcpyDeviceToHost, p->stream));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
-  if (p->d_dinv) {
+  if (p->bsr.dinv) {
     std::vector<double> dinv;
-    jacobi_blocks(p->n, p->dh, p->h_rowptr, p->h_bcol, p->h_bval, dinv);
-    DPGO_CUDA(cudaMemcpyAsync(p->d_dinv, dinv.data(), sizeof(double) * dinv.size(), cudaMemcpyHostToDevice, p->stream));
+    jacobi_blocks(p->n, p->dh, p->bsr.h_rowptr, p->bsr.h_bcol, p->bsr.h_bval, dinv);
+    DPGO_CUDA(p->bsr.dinv.upload(dinv.data(), dinv.size(), p->stream));
     DPGO_CUDA(cudaStreamSynchronize(p->stream));
   }
   free_nd(p);                                            // (Q + 0.1 I)^-1 changed: rebuilt on next use
-  free_dev(p->d_pinv); free_dev(p->d_dense_part); free_dev(p->d_dense_t2); free_dev(p->d_ppack); free_dev(p->d_sym_off);
-  free_dev(p->d_sym_cut); free_dev(p->d_sym_segptr); free_dev(p->d_sym_cfirst); free_dev(p->d_sym_ccount);
-  p->sym_ok = 0;
+  p->dense = {};
   return DPGO_OK;
 }
 
@@ -1295,12 +1264,12 @@ int dpgo_problem_set_edges(dpgo_problem_t *p, int64_t m, const int32_t *p1, cons
   for (int64_t q = 0; q < num_static; ++q) add(static_pose[q], static_pose[q]);
   DPGO_TRY(build_from_triplets(p, trip, precond_mask));
   // ... and every block's contribution list in input order: block (bi, bj) = entry with bcol == bi in row bj
-  const std::vector<int> &rowptr = p->h_rowptr, &bcol = p->h_bcol;
+  const std::vector<int> &rowptr = p->bsr.h_rowptr, &bcol = p->bsr.h_bcol;
   auto find_block = [&](int bi, int bj) {
     const int *lo = bcol.data() + rowptr[(size_t)bj], *hi = bcol.data() + rowptr[(size_t)bj + 1];
     return (int)(std::lower_bound(lo, hi, bi) - bcol.data());
   };
-  const int64_t nb = p->nb;
+  const int64_t nb = p->bsr.nb;
   std::vector<int> cnt((size_t)nb + 1, 0);
   std::vector<std::pair<int, int2>> items;             // (block, (index, kind))
   items.reserve((size_t)(4 * m + num_static));
@@ -1337,41 +1306,42 @@ int dpgo_problem_set_edges(dpgo_problem_t *p, int64_t m, const int32_t *p1, cons
   for (int64_t q = 0; q < num_static; ++q)
     for (int a = 0; a < dh; ++a)
       for (int b = 0; b < dh; ++b) sb[(size_t)q * 16 + a * 4 + b] = static_blocks[(size_t)q * dh * dh + a * dh + b];
-  free_dev(p->d_e_p1); free_dev(p->d_e_p2); free_dev(p->d_e_fixed); free_dev(p->d_cptr); free_dev(p->d_contrib);
-  free_dev(p->d_eT); free_dev(p->d_eom); free_dev(p->d_ew); free_dev(p->d_sblk); free_dev(p->d_eres);
-  p->ne = m;
-  auto up = [&](auto *&dst, const auto &src) -> cudaError_t {
-    using T = typename std::remove_reference<decltype(src[0])>::type;
-    cudaError_t e = cudaMalloc(&dst, sizeof(T) * std::max<size_t>(src.size(), 1));
-    if (e == cudaSuccess && !src.empty()) e = cudaMemcpy(dst, src.data(), sizeof(T) * src.size(), cudaMemcpyHostToDevice);
-    return e;
-  };
-  DPGO_CUDA(up(p->d_e_p1, q1)); DPGO_CUDA(up(p->d_e_p2, q2)); DPGO_CUDA(up(p->d_e_fixed, fx)); DPGO_CUDA(up(p->d_cptr, cnt));
-  DPGO_CUDA(up(p->d_contrib, contrib)); DPGO_CUDA(up(p->d_eT, eT)); DPGO_CUDA(up(p->d_eom, eom)); DPGO_CUDA(up(p->d_ew, ew));
-  DPGO_CUDA(up(p->d_sblk, sb));
-  DPGO_CUDA(cudaMalloc(&p->d_eres, sizeof(double) * std::max<int64_t>(m, 1)));
+  p->edges = {};
+  dpgo_problem::Edges &E = p->edges;
+  E.ne = m;
+  DPGO_CUDA(E.p1.assign(q1.data(), q1.size(), p->stream));
+  DPGO_CUDA(E.p2.assign(q2.data(), q2.size(), p->stream));
+  DPGO_CUDA(E.fixed.assign(fx.data(), fx.size(), p->stream));
+  DPGO_CUDA(E.cptr.assign(cnt.data(), cnt.size(), p->stream));
+  DPGO_CUDA(E.contrib.assign(contrib.data(), contrib.size(), p->stream));
+  DPGO_CUDA(E.T.assign(eT.data(), eT.size(), p->stream));
+  DPGO_CUDA(E.om.assign(eom.data(), eom.size(), p->stream));
+  DPGO_CUDA(E.w.assign(ew.data(), ew.size(), p->stream));
+  DPGO_CUDA(E.sblk.assign(sb.data(), sb.size(), p->stream));
+  DPGO_CUDA(E.res.alloc((size_t)m));
   return reassemble_Q(p);
 }
 
 int dpgo_problem_set_edge_weights(dpgo_problem_t *p, const double *weights_host) {
   DPGO_CHECK_HANDLE(p);
-  DPGO_REQUIRE(p->d_cptr, DPGO_ERR_STATE, "dpgo_problem_set_edges has not been called");
-  DPGO_REQUIRE(weights_host || p->ne == 0, DPGO_ERR_INVALID_ARG, "null weights");
-  if (p->ne) DPGO_CUDA(cudaMemcpyAsync(p->d_ew, weights_host, sizeof(double) * (size_t)p->ne, cudaMemcpyHostToDevice, p->stream));
+  DPGO_REQUIRE(p->edges.cptr, DPGO_ERR_STATE, "dpgo_problem_set_edges has not been called");
+  DPGO_REQUIRE(weights_host || p->edges.ne == 0, DPGO_ERR_INVALID_ARG, "null weights");
+  DPGO_CUDA(p->edges.w.upload(weights_host, (size_t)p->edges.ne, p->stream));
   return reassemble_Q(p);
 }
 
 int dpgo_problem_robust_reweight(dpgo_problem_t *p, int cost, double mu, double param, double *weights_host, double *residuals2_host) {
   DPGO_CHECK_HANDLE(p);
-  DPGO_REQUIRE(p->d_cptr, DPGO_ERR_STATE, "dpgo_problem_set_edges has not been called");
+  DPGO_REQUIRE(p->edges.cptr, DPGO_ERR_STATE, "dpgo_problem_set_edges has not been called");
   DPGO_REQUIRE(cost >= 0 && cost <= 5, DPGO_ERR_INVALID_ARG, "unknown robust cost");
   DPGO_REQUIRE(cost != 5 || mu > 0, DPGO_ERR_INVALID_ARG, "GNC needs mu > 0");
-  DPGO_CUDA(dpgo::launch_edge_weights(p->r, p->dh, p->ne, p->d_e_p1, p->d_e_p2, p->d_eT, p->d_eom, p->d_e_fixed, p->d_vec[dpgo::V_X0], cost,
-                                      mu, param, p->d_ew, p->d_eres, p->stream));
-  if (weights_host && p->ne)
-    DPGO_CUDA(cudaMemcpyAsync(weights_host, p->d_ew, sizeof(double) * (size_t)p->ne, cudaMemcpyDeviceToHost, p->stream));
-  if (residuals2_host && p->ne)
-    DPGO_CUDA(cudaMemcpyAsync(residuals2_host, p->d_eres, sizeof(double) * (size_t)p->ne, cudaMemcpyDeviceToHost, p->stream));
+  const dpgo_problem::Edges &E = p->edges;
+  DPGO_CUDA(dpgo::launch_edge_weights(p->r, p->dh, E.ne, E.p1.get(), E.p2.get(), E.T.get(), E.om.get(), E.fixed.get(),
+                                      p->vec[dpgo::V_X0].get(), cost, mu, param, E.w.get(), E.res.get(), p->stream));
+  if (weights_host && E.ne)
+    DPGO_CUDA(cudaMemcpyAsync(weights_host, E.w.get(), sizeof(double) * (size_t)E.ne, cudaMemcpyDeviceToHost, p->stream));
+  if (residuals2_host && E.ne)
+    DPGO_CUDA(cudaMemcpyAsync(residuals2_host, E.res.get(), sizeof(double) * (size_t)E.ne, cudaMemcpyDeviceToHost, p->stream));
   return reassemble_Q(p);
 }
 
@@ -1419,27 +1389,23 @@ int dpgo_agent_set_public_poses(dpgo_problem_t *p, int num_public, const int32_t
   DPGO_REQUIRE(num_public >= 0 && (num_public == 0 || public_pose), DPGO_ERR_INVALID_ARG, "bad public pose list");
   for (int s = 0; s < num_public; ++s)
     if (public_pose[s] < 0 || public_pose[s] >= p->n) return fail(DPGO_ERR_INVALID_ARG, "public pose index out of range");
+  p->pub = {};
   std::vector<int> pub_slot((size_t)p->n, -1);
-  p->pub_slot_unique = true;
   for (int s = 0; s < num_public; ++s) {
-    if (pub_slot[(size_t)public_pose[s]] >= 0) p->pub_slot_unique = false;
+    if (pub_slot[(size_t)public_pose[s]] >= 0) p->pub.slot_unique = false;
     else pub_slot[(size_t)public_pose[s]] = s;
   }
-  free_dev(p->d_public);
-  p->num_public = num_public;
-  if (num_public) {
-    DPGO_CUDA(cudaMalloc(&p->d_public, sizeof(int) * num_public));
-    DPGO_CUDA(cudaMemcpy(p->d_public, public_pose, sizeof(int) * num_public, cudaMemcpyHostToDevice));
-  }
-  if (!p->d_pub_slot) DPGO_CUDA(cudaMalloc(&p->d_pub_slot, sizeof(int) * (size_t)p->n));
-  DPGO_CUDA(cudaMemcpy(p->d_pub_slot, pub_slot.data(), sizeof(int) * (size_t)p->n, cudaMemcpyHostToDevice));
+  p->pub.num = num_public;
+  if (num_public) DPGO_CUDA(p->pub.pose.assign(public_pose, (size_t)num_public, p->stream));
+  DPGO_CUDA(p->pub.slot.assign(pub_slot.data(), pub_slot.size(), p->stream));
+  DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
 }
 
 int dpgo_agent_pack_public(dpgo_problem_t *p, double *send_dev) {
   DPGO_CHECK_HANDLE(p);
-  DPGO_REQUIRE(send_dev || p->num_public == 0, DPGO_ERR_INVALID_ARG, "null send buffer");
-  DPGO_CUDA(dpgo::launch_pack_tiles(p->ts, p->num_public, p->d_public, p->d_vec[dpgo::V_X0], send_dev, p->stream, p->gate));
+  DPGO_REQUIRE(send_dev || p->pub.num == 0, DPGO_ERR_INVALID_ARG, "null send buffer");
+  DPGO_CUDA(dpgo::launch_pack_tiles(p->ts, p->pub.num, p->pub.pose.get(), p->vec[dpgo::V_X0].get(), send_dev, p->stream, p->gate));
   return DPGO_OK;
 }
 
@@ -1471,68 +1437,63 @@ int dpgo_agent_set_shared_edges(dpgo_problem_t *p, int num_edges, const int32_t 
     std::memcpy(&oms[(size_t)q * dh], omega + (size_t)e * dh, sizeof(double) * dh);
   }
   pose_ptr.push_back(num_edges);
-  free_dev(p->d_pose_ids); free_dev(p->d_pose_ptr); free_dev(p->d_edge_slot); free_dev(p->d_edge_out);
-  free_dev(p->d_edge_T); free_dev(p->d_edge_om);
-  p->num_edges = num_edges;
+  p->shared = {};
+  p->shared.num_edges = num_edges;
   p->G_dirty = true;
-  p->num_shared_poses = (int)pose_ids.size();
-  p->max_slot = -1;
-  for (int e = 0; e < num_edges; ++e) p->max_slot = std::max(p->max_slot, (int)nbr_slot[e]);
+  p->shared.num_poses = (int)pose_ids.size();
+  for (int e = 0; e < num_edges; ++e) p->shared.max_slot = std::max(p->shared.max_slot, (int)nbr_slot[e]);
   if (num_edges) {
-    DPGO_CUDA(cudaMalloc(&p->d_pose_ids, sizeof(int) * pose_ids.size()));
-    DPGO_CUDA(cudaMalloc(&p->d_pose_ptr, sizeof(int) * pose_ptr.size()));
-    DPGO_CUDA(cudaMalloc(&p->d_edge_slot, sizeof(int) * num_edges));
-    DPGO_CUDA(cudaMalloc(&p->d_edge_out, sizeof(int) * num_edges));
-    DPGO_CUDA(cudaMalloc(&p->d_edge_T, sizeof(double) * Ts.size()));
-    DPGO_CUDA(cudaMalloc(&p->d_edge_om, sizeof(double) * oms.size()));
-    DPGO_CUDA(cudaMemcpy(p->d_pose_ids, pose_ids.data(), sizeof(int) * pose_ids.size(), cudaMemcpyHostToDevice));
-    DPGO_CUDA(cudaMemcpy(p->d_pose_ptr, pose_ptr.data(), sizeof(int) * pose_ptr.size(), cudaMemcpyHostToDevice));
-    DPGO_CUDA(cudaMemcpy(p->d_edge_slot, slot.data(), sizeof(int) * num_edges, cudaMemcpyHostToDevice));
-    DPGO_CUDA(cudaMemcpy(p->d_edge_out, outg.data(), sizeof(int) * num_edges, cudaMemcpyHostToDevice));
-    DPGO_CUDA(cudaMemcpy(p->d_edge_T, Ts.data(), sizeof(double) * Ts.size(), cudaMemcpyHostToDevice));
-    DPGO_CUDA(cudaMemcpy(p->d_edge_om, oms.data(), sizeof(double) * oms.size(), cudaMemcpyHostToDevice));
+    DPGO_CUDA(p->shared.pose_ids.assign(pose_ids.data(), pose_ids.size(), p->stream));
+    DPGO_CUDA(p->shared.pose_ptr.assign(pose_ptr.data(), pose_ptr.size(), p->stream));
+    DPGO_CUDA(p->shared.slot.assign(slot.data(), slot.size(), p->stream));
+    DPGO_CUDA(p->shared.out.assign(outg.data(), outg.size(), p->stream));
+    DPGO_CUDA(p->shared.T.assign(Ts.data(), Ts.size(), p->stream));
+    DPGO_CUDA(p->shared.om.assign(oms.data(), oms.size(), p->stream));
   }
+  DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
 }
 
 int dpgo_agent_build_G(dpgo_problem_t *p, const double *gathered_dev, int64_t num_slots) {
   DPGO_CHECK_HANDLE(p);
-  DPGO_REQUIRE(gathered_dev || p->num_edges == 0, DPGO_ERR_INVALID_ARG, "null gathered buffer");
-  DPGO_REQUIRE((int64_t)p->max_slot < num_slots || p->num_edges == 0, DPGO_ERR_INVALID_ARG,
+  DPGO_REQUIRE(gathered_dev || p->shared.num_edges == 0, DPGO_ERR_INVALID_ARG, "null gathered buffer");
+  DPGO_REQUIRE((int64_t)p->shared.max_slot < num_slots || p->shared.num_edges == 0, DPGO_ERR_INVALID_ARG,
                "a shared edge refers to a slot beyond the gathered buffer (exchange plan / slot table mismatch)");
   // k_build_G assigns every tile of a pose with shared edges; the other tiles of G are zero and stay zero, so G is cleared
   // only when something else may have written it (set_G, a new edge table)
   if (p->G_dirty) {
-    DPGO_CUDA(cudaMemsetAsync(p->d_G, 0, p->vec_bytes(), p->stream));
+    DPGO_CUDA(cudaMemsetAsync(p->G.get(), 0, p->vec_bytes(), p->stream));
     p->G_dirty = false;
   }
-  if (p->num_edges)
-    DPGO_CUDA(dpgo::launch_build_G(p->r, p->dh, p->num_shared_poses, p->d_pose_ids, p->d_pose_ptr, p->d_edge_slot,
-                                   p->d_edge_out, p->d_edge_T, p->d_edge_om, gathered_dev, p->d_G, p->stream, p->gate));
+  const dpgo_problem::Shared &S = p->shared;
+  if (S.num_edges)
+    DPGO_CUDA(dpgo::launch_build_G(p->r, p->dh, S.num_poses, S.pose_ids.get(), S.pose_ptr.get(), S.slot.get(), S.out.get(),
+                                   S.T.get(), S.om.get(), gathered_dev, p->G.get(), p->stream, p->gate));
   return DPGO_OK;
 }
 
 // ---- Nesterov acceleration on the resident iterate ----------------------------------------------------
-#define DPGO_ACC_READY(p) DPGO_REQUIRE((p)->d_acc[0], DPGO_ERR_STATE, "dpgo_agent_accel_init has not been called")
+#define DPGO_ACC_READY(p) DPGO_REQUIRE((p)->acc.vec[0], DPGO_ERR_STATE, "dpgo_agent_accel_init has not been called")
 int dpgo_agent_accel_init(dpgo_problem_t *p) {
   DPGO_CHECK_HANDLE(p);
+  // allocated once: captured round graphs keep these addresses
   for (int i = 0; i < 3; ++i) {
-    if (!p->d_acc[i]) DPGO_CUDA(cudaMalloc(&p->d_acc[i], p->vec_bytes()));
-    DPGO_CUDA(cudaMemcpyAsync(p->d_acc[i], p->d_vec[dpgo::V_X0], p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
+    if (!p->acc.vec[i]) DPGO_CUDA(p->acc.vec[i].alloc((size_t)p->r * p->N));
+    DPGO_CUDA(cudaMemcpyAsync(p->acc.vec[i].get(), p->vec[dpgo::V_X0].get(), p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
   }
-  if (!p->d_acc_state) DPGO_CUDA(cudaMalloc(&p->d_acc_state, sizeof(double) * dpgo::ACCEL_STATE_DOUBLES));
-  if (!p->d_acc_part) DPGO_CUDA(cudaMalloc(&p->d_acc_part, sizeof(double) * (size_t)dpgo::accel_ctas(p->n)));
-  if (!p->d_acc_ticket) DPGO_CUDA(cudaMalloc(&p->d_acc_ticket, 2 * sizeof(unsigned)));
-  DPGO_CUDA(cudaMemsetAsync(p->d_acc_state, 0, sizeof(double) * dpgo::ACCEL_STATE_DOUBLES, p->stream));
-  DPGO_CUDA(cudaMemsetAsync(p->d_acc_ticket, 0, 2 * sizeof(unsigned), p->stream));
-  p->acc_rounds = 0;
-  p->acc_restart_due = false;
+  if (!p->acc.state) DPGO_CUDA(p->acc.state.alloc(dpgo::ACCEL_STATE_DOUBLES));
+  if (!p->acc.part) DPGO_CUDA(p->acc.part.alloc((size_t)dpgo::accel_ctas(p->n)));
+  if (!p->acc.ticket) DPGO_CUDA(p->acc.ticket.alloc(2));
+  DPGO_CUDA(cudaMemsetAsync(p->acc.state.get(), 0, sizeof(double) * dpgo::ACCEL_STATE_DOUBLES, p->stream));
+  DPGO_CUDA(cudaMemsetAsync(p->acc.ticket.get(), 0, 2 * sizeof(unsigned), p->stream));
+  p->acc.rounds = 0;
+  p->acc.restart_due = false;
   return DPGO_OK;
 }
 int dpgo_agent_accel_begin(dpgo_problem_t *p, double alpha) {
   DPGO_CHECK_HANDLE(p);
   DPGO_ACC_READY(p);
-  double *X = p->d_vec[dpgo::V_X0], *Y = p->d_acc[0], *V = p->d_acc[1], *XP = p->d_acc[2];
+  double *X = p->vec[dpgo::V_X0].get(), *Y = p->acc.vec[0].get(), *V = p->acc.vec[1].get(), *XP = p->acc.vec[2].get();
   DPGO_CUDA(cudaMemcpyAsync(XP, X, p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
   DPGO_CUDA(dpgo::launch_stiefel_project(p->r, p->dh, p->n, X, Y, p->stream, 1.0 - alpha, V, alpha));
   return DPGO_OK;
@@ -1540,7 +1501,7 @@ int dpgo_agent_accel_begin(dpgo_problem_t *p, double alpha) {
 int dpgo_agent_accel_end(dpgo_problem_t *p, double gamma, int optimized) {
   DPGO_CHECK_HANDLE(p);
   DPGO_ACC_READY(p);
-  double *X = p->d_vec[dpgo::V_X0], *Y = p->d_acc[0], *V = p->d_acc[1];
+  double *X = p->vec[dpgo::V_X0].get(), *Y = p->acc.vec[0].get(), *V = p->acc.vec[1].get();
   if (!optimized) DPGO_CUDA(cudaMemcpyAsync(X, Y, p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
   DPGO_CUDA(dpgo::launch_stiefel_project(p->r, p->dh, p->n, V, V, p->stream, 1.0, X, gamma, Y, -gamma));
   return DPGO_OK;
@@ -1548,27 +1509,27 @@ int dpgo_agent_accel_end(dpgo_problem_t *p, double gamma, int optimized) {
 int dpgo_agent_accel_restart_begin(dpgo_problem_t *p) {
   DPGO_CHECK_HANDLE(p);
   DPGO_ACC_READY(p);
-  DPGO_CUDA(cudaMemcpyAsync(p->d_vec[dpgo::V_X0], p->d_acc[2], p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(p->vec[dpgo::V_X0].get(), p->acc.vec[2].get(), p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
   return DPGO_OK;
 }
 int dpgo_agent_accel_restart_end(dpgo_problem_t *p) {
   DPGO_CHECK_HANDLE(p);
   DPGO_ACC_READY(p);
   for (int i = 0; i < 2; ++i)
-    DPGO_CUDA(cudaMemcpyAsync(p->d_acc[i], p->d_vec[dpgo::V_X0], p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
+    DPGO_CUDA(cudaMemcpyAsync(p->acc.vec[i].get(), p->vec[dpgo::V_X0].get(), p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
   return DPGO_OK;
 }
 int dpgo_agent_pack_public_aux(dpgo_problem_t *p, double *send_dev) {
   DPGO_CHECK_HANDLE(p);
   DPGO_ACC_READY(p);
-  DPGO_REQUIRE(send_dev || p->num_public == 0, DPGO_ERR_INVALID_ARG, "null send buffer");
-  DPGO_CUDA(dpgo::launch_pack_tiles(p->ts, p->num_public, p->d_public, p->d_acc[0], send_dev, p->stream));
+  DPGO_REQUIRE(send_dev || p->pub.num == 0, DPGO_ERR_INVALID_ARG, "null send buffer");
+  DPGO_CUDA(dpgo::launch_pack_tiles(p->ts, p->pub.num, p->pub.pose.get(), p->acc.vec[0].get(), send_dev, p->stream));
   return DPGO_OK;
 }
 int dpgo_optimize_resident_from_aux_async(dpgo_problem_t *p, const dpgo_opt_params_t *params) {
   DPGO_CHECK_HANDLE(p);
   DPGO_ACC_READY(p);
-  DPGO_CUDA(cudaMemcpyAsync(p->d_vec[dpgo::V_X0], p->d_acc[0], p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(p->vec[dpgo::V_X0].get(), p->acc.vec[0].get(), p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
   return dpgo_optimize_resident_async(p, params);
 }
 
@@ -1596,7 +1557,7 @@ template <class Issue> int replay_or_issue(dpgo_problem *lead, const std::vector
     entry->key = key;
   }
   if (entry->exec) {
-    DPGO_CUDA(cudaGraphLaunch(entry->exec, main));
+    DPGO_CUDA(cudaGraphLaunch(entry->exec.get(), main));
     return DPGO_OK;
   }
   if (entry->failed || entry->uses++ == 0) return issue();
@@ -1614,15 +1575,16 @@ template <class Issue> int replay_or_issue(dpgo_problem *lead, const std::vector
     entry->failed = true;
     return issue();
   }
-  const cudaError_t ie = cudaGraphInstantiate(&entry->exec, graph, 0);
+  cudaGraphExec_t exec = nullptr;
+  const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
   cudaGraphDestroy(graph);
   if (ie != cudaSuccess) {
     cudaGetLastError();
-    entry->exec = nullptr;
     entry->failed = true;
     return issue();
   }
-  DPGO_CUDA(cudaGraphLaunch(entry->exec, main));
+  entry->exec.reset(exec);
+  DPGO_CUDA(cudaGraphLaunch(exec, main));
   return DPGO_OK;
 }
 
@@ -1643,15 +1605,15 @@ int round_preamble(dpgo_problem_t *const *agents, int num_active, const dpgo_opt
     DPGO_CHECK_HANDLE(p);
     DPGO_REQUIRE(p->device == agents[0]->device, DPGO_ERR_INVALID_ARG, "the agents of a round must live on one device");
     DPGO_TRY(check_params(p, params));
-    if (!p->ev_done) DPGO_CUDA(cudaEventCreateWithFlags(&p->ev_done, cudaEventDisableTiming));
+    if (!p->ev_done) DPGO_CUDA(dpgo::create_event(p->ev_done));
     // a cooperative launch does not capture; a pending G clear or an unbuilt factorisation must run eagerly first
-    if (!p->cluster || p->G_dirty || p->d_phase_ns || ((p->precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)) && !p->nd_ready))
+    if (!p->cluster || p->G_dirty || p->phase_ns || ((p->bsr.precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)) && !p->nd.ready))
       graph = false;
   }
   dpgo_problem *lead = agents[0];
   main = main_stream ? (cudaStream_t)main_stream : lead->stream;
   DPGO_CUDA(cudaSetDevice(lead->device));
-  if (!lead->ev_fork) DPGO_CUDA(cudaEventCreateWithFlags(&lead->ev_fork, cudaEventDisableTiming));
+  if (!lead->ev_fork) DPGO_CUDA(dpgo::create_event(lead->ev_fork));
   if (main == cudaStreamLegacy || main == nullptr) graph = false;   // the legacy default stream cannot be captured
   return DPGO_OK;
 }
@@ -1681,19 +1643,19 @@ static int issue_round(dpgo_problem_t *const *agents, int num_active, const dpgo
   dpgo_problem *lead = agents[0];
   const int passes = pack_after_join ? 2 : 1;
   for (int pass = 0; pass < passes; ++pass) {
-    DPGO_CUDA(cudaEventRecord(lead->ev_fork, main));
+    DPGO_CUDA(cudaEventRecord(lead->ev_fork.get(), main));
     for (int i = 0; i < num_active; ++i) {
       dpgo_problem *p = agents[i];
-      StreamSwap swap(p, p->cluster ? p->own_stream : main);   // cluster steps side by side, full-grid steps in order
-      if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork, 0));
+      StreamSwap swap(p, p->cluster ? p->own_stream.get() : main);   // cluster steps side by side, full-grid steps in order
+      if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork.get(), 0));
       if (pass == 0) {
         DPGO_TRY(dpgo_agent_build_G(p, gathered_dev, num_slots));
         DPGO_TRY(dpgo_optimize_resident_async(p, params));
       }
       if (pass == passes - 1) DPGO_TRY(dpgo_agent_pack_public(p, send_dev[i]));
       if (p->stream != main) {
-        DPGO_CUDA(cudaEventRecord(p->ev_done, p->stream));
-        DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done, 0));
+        DPGO_CUDA(cudaEventRecord(p->ev_done.get(), p->stream));
+        DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done.get(), 0));
       }
     }
   }
@@ -1743,17 +1705,17 @@ int dpgo_agents_host_io_async(dpgo_problem_t *const *agents, int count, double *
   dpgo_problem *lead = agents[0];
   cudaStream_t main = stream ? (cudaStream_t)stream : lead->stream;
   DPGO_CUDA(cudaSetDevice(lead->device));
-  if (!lead->ev_fork) DPGO_CUDA(cudaEventCreateWithFlags(&lead->ev_fork, cudaEventDisableTiming));
+  if (!lead->ev_fork) DPGO_CUDA(dpgo::create_event(lead->ev_fork));
   for (int i = 0; i < count; ++i)
-    if (!agents[i]->ev_done) DPGO_CUDA(cudaEventCreateWithFlags(&agents[i]->ev_done, cudaEventDisableTiming));
+    if (!agents[i]->ev_done) DPGO_CUDA(dpgo::create_event(agents[i]->ev_done));
   auto issue = [&]() -> int {
     // every agent's copy (+ pack) on its own stream between a fork from and a join into `main`: the copies of different
     // agents overlap each other and the packs
-    DPGO_CUDA(cudaEventRecord(lead->ev_fork, main));
+    DPGO_CUDA(cudaEventRecord(lead->ev_fork.get(), main));
     for (int i = 0; i < count; ++i) {
       dpgo_problem *p = agents[i];
-      StreamSwap swap(p, p->own_stream);
-      if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork, 0));
+      StreamSwap swap(p, p->own_stream.get());
+      if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork.get(), 0));
       if (direction == 0) {
         DPGO_TRY(upload_vec(p, dpgo::V_X0, X_host[i]));
         if (send_dev && send_dev[i]) DPGO_TRY(dpgo_agent_pack_public(p, send_dev[i]));
@@ -1761,8 +1723,8 @@ int dpgo_agents_host_io_async(dpgo_problem_t *const *agents, int count, double *
         DPGO_TRY(download_vec(p, dpgo::V_X0, X_host[i]));
       }
       if (p->stream != main) {
-        DPGO_CUDA(cudaEventRecord(p->ev_done, p->stream));
-        DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done, 0));
+        DPGO_CUDA(cudaEventRecord(p->ev_done.get(), p->stream));
+        DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done.get(), 0));
       }
     }
     return DPGO_OK;
@@ -1798,28 +1760,27 @@ int dpgo_agent_f_rgradnorm_resident(dpgo_problem_t *p, double *f_out, double *no
 namespace {
 int ensure_jobs(dpgo_problem *p, int jobs, int ready) {
   if (jobs > p->jobs_cap) {
-    free_dev(p->d_jobs);
-    DPGO_CUDA(cudaMalloc(&p->d_jobs, sizeof(dpgo::AlignJob) * jobs));
+    DPGO_CUDA(p->align_jobs.alloc((size_t)jobs));
     p->jobs_cap = jobs;
   }
   if (ready > p->ready_cap) {
-    free_dev(p->d_ready);
-    DPGO_CUDA(cudaMalloc(&p->d_ready, sizeof(int) * ready));
+    DPGO_CUDA(p->ready.alloc((size_t)ready));
     p->ready_cap = ready;
   }
   return DPGO_OK;
 }
 
 dpgo::AlignJob align_job(const dpgo_problem *p) {
+  const dpgo_problem::Align &A = p->align;
   dpgo::AlignJob J = {};
-  J.ngroups = p->align_groups;
+  J.ngroups = A.groups;
   J.n = p->n;
-  J.grp_nbr = p->d_grp_nbr; J.grp_ptr = p->d_grp_ptr;
-  J.cand_local = p->d_cand_local; J.cand_slot = p->d_cand_slot; J.cand_out = p->d_cand_out; J.cand_T = p->d_cand_T;
+  J.grp_nbr = A.grp_nbr.get(); J.grp_ptr = A.grp_ptr.get();
+  J.cand_local = A.cand_local.get(); J.cand_slot = A.cand_slot.get(); J.cand_out = A.cand_out.get(); J.cand_T = A.cand_T.get();
   J.kappa = nullptr;
-  J.cand_R = p->d_cand_R; J.cand_t = p->d_cand_t; J.w = p->d_cand_w;
-  J.Tloc = p->d_Tloc; J.ylift = p->d_ylift; J.X = p->d_vec[dpgo::V_X0];
-  J.T_align = p->d_T_align; J.info = p->d_align_info;
+  J.cand_R = A.cand_R.get(); J.cand_t = A.cand_t.get(); J.w = A.cand_w.get();
+  J.Tloc = p->Tloc.get(); J.ylift = p->ylift.get(); J.X = p->vec[dpgo::V_X0].get();
+  J.T_align = p->T_align.get(); J.info = p->align_info.get();
   return J;
 }
 }  // namespace
@@ -1828,16 +1789,16 @@ int dpgo_agent_set_local_trajectory(dpgo_problem_t *p, const double *T_host, con
   DPGO_CHECK_HANDLE(p);
   DPGO_REQUIRE(T_host && YLift_host, DPGO_ERR_INVALID_ARG, "null trajectory or lifting matrix");
   const size_t tn = (size_t)p->d * p->dh * p->n, yn = (size_t)p->r * p->d;
-  if (!p->d_Tloc) DPGO_CUDA(cudaMalloc(&p->d_Tloc, sizeof(double) * tn));
-  if (!p->d_ylift) DPGO_CUDA(cudaMalloc(&p->d_ylift, sizeof(double) * yn));
-  DPGO_CUDA(cudaMemcpyAsync(p->d_Tloc, T_host, sizeof(double) * tn, cudaMemcpyHostToDevice, p->stream));
-  DPGO_CUDA(cudaMemcpyAsync(p->d_ylift, YLift_host, sizeof(double) * yn, cudaMemcpyHostToDevice, p->stream));
+  if (!p->Tloc) DPGO_CUDA(p->Tloc.alloc(tn));
+  if (!p->ylift) DPGO_CUDA(p->ylift.alloc(yn));
+  DPGO_CUDA(p->Tloc.upload(T_host, tn, p->stream));
+  DPGO_CUDA(p->ylift.upload(YLift_host, yn, p->stream));
   DPGO_TRY(ensure_jobs(p, 1, 0));
   dpgo::AlignJob J = align_job(p);
   J.T_align = nullptr;                     // identity: X = YLift T
   J.info = nullptr;
-  DPGO_CUDA(cudaMemcpyAsync(p->d_jobs, &J, sizeof(J), cudaMemcpyHostToDevice, p->stream));
-  DPGO_CUDA(dpgo::launch_frame_lift(p->d, p->r, 1, p->n, p->d_jobs, p->stream));
+  DPGO_CUDA(p->align_jobs.upload(&J, 1, p->stream));
+  DPGO_CUDA(dpgo::launch_frame_lift(p->d, p->r, 1, p->n, p->align_jobs.get(), p->stream));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
 }
@@ -1860,33 +1821,27 @@ int dpgo_agent_set_align_candidates(dpgo_problem_t *p, int num_groups, const int
                  "candidate index out of range");
     max_slot = std::max(max_slot, (int)nbr_slot[q]);
   }
-  free_dev(p->d_grp_nbr); free_dev(p->d_grp_ptr); free_dev(p->d_cand_local); free_dev(p->d_cand_slot); free_dev(p->d_cand_out);
-  free_dev(p->d_cand_T); free_dev(p->d_cand_R); free_dev(p->d_cand_t); free_dev(p->d_cand_w);
-  p->align_groups = num_groups;
-  p->align_cands = m;
-  p->align_max_slot = max_slot;
-  p->align_max_nbr = num_groups ? group_neighbor[num_groups - 1] : -1;
-  if (!p->d_T_align) DPGO_CUDA(cudaMalloc(&p->d_T_align, sizeof(double) * p->d * p->dh));
-  if (!p->d_align_info) DPGO_CUDA(cudaMalloc(&p->d_align_info, sizeof(int) * 4));
+  p->align = {};
+  p->align.groups = num_groups;
+  p->align.cands = m;
+  p->align.max_slot = max_slot;
+  p->align.max_nbr = num_groups ? group_neighbor[num_groups - 1] : -1;
+  if (!p->T_align) DPGO_CUDA(p->T_align.alloc((size_t)p->d * p->dh));
+  if (!p->align_info) DPGO_CUDA(p->align_info.alloc(4));
   if (!num_groups) return DPGO_OK;
   const int dh = p->dh;
-  DPGO_CUDA(cudaMalloc(&p->d_grp_nbr, sizeof(int) * num_groups));
-  DPGO_CUDA(cudaMalloc(&p->d_grp_ptr, sizeof(int) * (num_groups + 1)));
-  DPGO_CUDA(cudaMalloc(&p->d_cand_local, sizeof(int) * m));
-  DPGO_CUDA(cudaMalloc(&p->d_cand_slot, sizeof(int) * m));
-  DPGO_CUDA(cudaMalloc(&p->d_cand_out, sizeof(int) * m));
-  DPGO_CUDA(cudaMalloc(&p->d_cand_T, sizeof(double) * m * dh * dh));
-  DPGO_CUDA(cudaMalloc(&p->d_cand_R, sizeof(double) * m * p->d * p->d));
-  DPGO_CUDA(cudaMalloc(&p->d_cand_t, sizeof(double) * m * p->d));
-  DPGO_CUDA(cudaMalloc(&p->d_cand_w, sizeof(double) * m));
-  DPGO_CUDA(cudaMemcpy(p->d_grp_nbr, group_neighbor, sizeof(int) * num_groups, cudaMemcpyHostToDevice));
-  DPGO_CUDA(cudaMemcpy(p->d_grp_ptr, group_ptr, sizeof(int) * (num_groups + 1), cudaMemcpyHostToDevice));
-  DPGO_CUDA(cudaMemcpy(p->d_cand_local, local_pose, sizeof(int) * m, cudaMemcpyHostToDevice));
-  DPGO_CUDA(cudaMemcpy(p->d_cand_slot, nbr_slot, sizeof(int) * m, cudaMemcpyHostToDevice));
   std::vector<int> outg(m);
   for (int q = 0; q < m; ++q) outg[q] = outgoing[q] ? 1 : 0;
-  DPGO_CUDA(cudaMemcpy(p->d_cand_out, outg.data(), sizeof(int) * m, cudaMemcpyHostToDevice));
-  DPGO_CUDA(cudaMemcpy(p->d_cand_T, T, sizeof(double) * m * dh * dh, cudaMemcpyHostToDevice));
+  DPGO_CUDA(p->align.grp_nbr.assign(group_neighbor, (size_t)num_groups, p->stream));
+  DPGO_CUDA(p->align.grp_ptr.assign(group_ptr, (size_t)num_groups + 1, p->stream));
+  DPGO_CUDA(p->align.cand_local.assign(local_pose, (size_t)m, p->stream));
+  DPGO_CUDA(p->align.cand_slot.assign(nbr_slot, (size_t)m, p->stream));
+  DPGO_CUDA(p->align.cand_out.assign(outg.data(), outg.size(), p->stream));
+  DPGO_CUDA(p->align.cand_T.assign(T, (size_t)m * dh * dh, p->stream));
+  DPGO_CUDA(p->align.cand_R.alloc((size_t)m * p->d * p->d));
+  DPGO_CUDA(p->align.cand_t.alloc((size_t)m * p->d));
+  DPGO_CUDA(p->align.cand_w.alloc((size_t)m));
+  DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
 }
 
@@ -1902,35 +1857,36 @@ int dpgo_agents_align_async(dpgo_problem_t *const *agents, int count, const doub
     dpgo_problem *p = agents[i];
     DPGO_REQUIRE(p && p->device == lead->device && p->d == lead->d && p->r == lead->r, DPGO_ERR_INVALID_ARG,
                  "the agents of one align call must share the device, d and r");
-    DPGO_REQUIRE(p->d_Tloc && p->d_T_align, DPGO_ERR_STATE,
+    DPGO_REQUIRE(p->Tloc && p->T_align, DPGO_ERR_STATE,
                  "dpgo_agent_set_local_trajectory and dpgo_agent_set_align_candidates must be called first");
-    DPGO_REQUIRE(p->align_cands == 0 || (gathered_dev && p->align_max_slot < num_slots), DPGO_ERR_INVALID_ARG,
+    DPGO_REQUIRE(p->align.cands == 0 || (gathered_dev && p->align.max_slot < num_slots), DPGO_ERR_INVALID_ARG,
                  "a candidate refers to a slot beyond the gathered buffer");
-    DPGO_REQUIRE(p->align_max_nbr < num_agents, DPGO_ERR_INVALID_ARG, "a candidate group names an agent beyond the ready flags");
-    if (!p->ev_align) DPGO_CUDA(cudaEventCreateWithFlags(&p->ev_align, cudaEventDisableTiming));
+    DPGO_REQUIRE(p->align.max_nbr < num_agents, DPGO_ERR_INVALID_ARG, "a candidate group names an agent beyond the ready flags");
+    if (!p->ev_align) DPGO_CUDA(dpgo::create_event(p->ev_align));
     jobs[(size_t)i] = align_job(p);
-    max_cands = std::max(max_cands, p->align_cands);
+    max_cands = std::max(max_cands, p->align.cands);
     max_poses = std::max(max_poses, p->n);
   }
   cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
   DPGO_TRY(ensure_jobs(lead, count, num_agents));
-  DPGO_CUDA(cudaMemcpyAsync(lead->d_jobs, jobs.data(), sizeof(dpgo::AlignJob) * count, cudaMemcpyHostToDevice, st));
-  DPGO_CUDA(cudaMemcpyAsync(lead->d_ready, ready_host, sizeof(int) * num_agents, cudaMemcpyHostToDevice, st));
-  DPGO_CUDA(dpgo::launch_align_candidates(lead->d, lead->r, count, max_cands, lead->d_jobs, gathered_dev, st));
-  DPGO_CUDA(dpgo::launch_robust_rotation_average(lead->d, count, lead->d_jobs, lead->d_ready, 2.0 * std::sqrt(2.0) * std::sin(0.25), st));
-  DPGO_CUDA(dpgo::launch_frame_lift(lead->d, lead->r, count, max_poses, lead->d_jobs, st));
-  for (int i = 0; i < count; ++i) DPGO_CUDA(cudaEventRecord(agents[i]->ev_align, st));   // dpgo_agent_align_result waits on it
+  DPGO_CUDA(lead->align_jobs.upload(jobs.data(), jobs.size(), st));
+  DPGO_CUDA(lead->ready.upload(ready_host, (size_t)num_agents, st));
+  DPGO_CUDA(dpgo::launch_align_candidates(lead->d, lead->r, count, max_cands, lead->align_jobs.get(), gathered_dev, st));
+  DPGO_CUDA(dpgo::launch_robust_rotation_average(lead->d, count, lead->align_jobs.get(), lead->ready.get(),
+                                                 2.0 * std::sqrt(2.0) * std::sin(0.25), st));
+  DPGO_CUDA(dpgo::launch_frame_lift(lead->d, lead->r, count, max_poses, lead->align_jobs.get(), st));
+  for (int i = 0; i < count; ++i) DPGO_CUDA(cudaEventRecord(agents[i]->ev_align.get(), st));   // dpgo_agent_align_result waits on it
   return DPGO_OK;
 }
 
 int dpgo_agent_align_result(dpgo_problem_t *p, double *T_align_host, int32_t *info4) {
   DPGO_CHECK_HANDLE(p);
-  DPGO_REQUIRE(p->d_T_align, DPGO_ERR_STATE, "dpgo_agent_set_align_candidates has not been called");
+  DPGO_REQUIRE(p->T_align, DPGO_ERR_STATE, "dpgo_agent_set_align_candidates has not been called");
   DPGO_REQUIRE(info4, DPGO_ERR_INVALID_ARG, "null info");
-  if (p->ev_align) DPGO_CUDA(cudaEventSynchronize(p->ev_align));     // the align call may have run on another stream
+  if (p->ev_align) DPGO_CUDA(cudaEventSynchronize(p->ev_align.get()));     // the align call may have run on another stream
   if (T_align_host)
-    DPGO_CUDA(cudaMemcpyAsync(T_align_host, p->d_T_align, sizeof(double) * p->d * p->dh, cudaMemcpyDeviceToHost, p->stream));
-  DPGO_CUDA(cudaMemcpyAsync(info4, p->d_align_info, sizeof(int) * 4, cudaMemcpyDeviceToHost, p->stream));
+    DPGO_CUDA(cudaMemcpyAsync(T_align_host, p->T_align.get(), sizeof(double) * p->d * p->dh, cudaMemcpyDeviceToHost, p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(info4, p->align_info.get(), sizeof(int) * 4, cudaMemcpyDeviceToHost, p->stream));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
 }
@@ -1944,42 +1900,34 @@ int dpgo_robust_single_rotation_averaging(int device, int d, int m, const double
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count)
     return fail(DPGO_ERR_NO_DEVICE, "no such CUDA device: the GPU path has no CPU fallback");
   DPGO_CUDA(cudaSetDevice(device));
-  struct Bufs {
-    double *R = nullptr, *k = nullptr, *w = nullptr, *T = nullptr;
-    int *grp = nullptr, *info = nullptr;
-    dpgo::AlignJob *job = nullptr;
-    ~Bufs() { free_dev(R); free_dev(k); free_dev(w); free_dev(T); free_dev(grp); free_dev(info); free_dev(job); }
-  } b;
-  DPGO_CUDA(cudaMalloc(&b.R, sizeof(double) * m * d * d));
-  DPGO_CUDA(cudaMalloc(&b.w, sizeof(double) * m));
-  DPGO_CUDA(cudaMalloc(&b.T, sizeof(double) * d * (d + 1)));
-  DPGO_CUDA(cudaMalloc(&b.grp, sizeof(int) * 4));
-  DPGO_CUDA(cudaMalloc(&b.info, sizeof(int) * 4));
-  DPGO_CUDA(cudaMalloc(&b.job, sizeof(dpgo::AlignJob)));
-  DPGO_CUDA(cudaMemcpy(b.R, R_host, sizeof(double) * m * d * d, cudaMemcpyHostToDevice));
-  if (kappa_host) {
-    DPGO_CUDA(cudaMalloc(&b.k, sizeof(double) * m));
-    DPGO_CUDA(cudaMemcpy(b.k, kappa_host, sizeof(double) * m, cudaMemcpyHostToDevice));
-  }
-  const int grp[4] = {0, 0, m, 1};         // neighbour 0, candidates [0, m), ready flag of neighbour 0
-  DPGO_CUDA(cudaMemcpy(b.grp, grp, sizeof(grp), cudaMemcpyHostToDevice));
+  // everything on the legacy default stream: the synchronous reads at the end follow the launch
+  DevBuf<double> R, k, w, T;
+  DevBuf<int> grp, info;
+  DevBuf<dpgo::AlignJob> job;
+  DPGO_CUDA(R.assign(R_host, (size_t)m * d * d, nullptr));
+  DPGO_CUDA(w.alloc((size_t)m));
+  DPGO_CUDA(T.alloc((size_t)d * (d + 1)));
+  DPGO_CUDA(info.alloc(4));
+  if (kappa_host) DPGO_CUDA(k.assign(kappa_host, (size_t)m, nullptr));
+  const int grp_host[4] = {0, 0, m, 1};    // neighbour 0, candidates [0, m), ready flag of neighbour 0
+  DPGO_CUDA(grp.assign(grp_host, 4, nullptr));
   dpgo::AlignJob J = {};
   J.ngroups = 1;
-  J.grp_nbr = b.grp; J.grp_ptr = b.grp + 1;
-  J.kappa = b.k; J.cand_R = b.R; J.w = b.w;
-  J.T_align = b.T; J.info = b.info;
-  DPGO_CUDA(cudaMemcpy(b.job, &J, sizeof(J), cudaMemcpyHostToDevice));
-  DPGO_CUDA(dpgo::launch_robust_rotation_average(d, 1, b.job, b.grp + 3, threshold, nullptr));
-  std::vector<double> T((size_t)d * (d + 1)), w((size_t)m);
-  int info[4];
-  DPGO_CUDA(cudaMemcpy(T.data(), b.T, sizeof(double) * T.size(), cudaMemcpyDeviceToHost));
-  DPGO_CUDA(cudaMemcpy(w.data(), b.w, sizeof(double) * m, cudaMemcpyDeviceToHost));
-  DPGO_CUDA(cudaMemcpy(info, b.info, sizeof(info), cudaMemcpyDeviceToHost));
+  J.grp_nbr = grp.get(); J.grp_ptr = grp.get() + 1;
+  J.kappa = k.get(); J.cand_R = R.get(); J.w = w.get();
+  J.T_align = T.get(); J.info = info.get();
+  DPGO_CUDA(job.assign(&J, 1, nullptr));
+  DPGO_CUDA(dpgo::launch_robust_rotation_average(d, 1, job.get(), grp.get() + 3, threshold, nullptr));
+  std::vector<double> T_host((size_t)d * (d + 1)), w_host((size_t)m);
+  int info_host[4];
+  DPGO_CUDA(cudaMemcpy(T_host.data(), T.get(), sizeof(double) * T_host.size(), cudaMemcpyDeviceToHost));
+  DPGO_CUDA(cudaMemcpy(w_host.data(), w.get(), sizeof(double) * m, cudaMemcpyDeviceToHost));
+  DPGO_CUDA(cudaMemcpy(info_host, info.get(), sizeof(info_host), cudaMemcpyDeviceToHost));
   for (int a = 0; a < d; ++a)
-    for (int c = 0; c < d; ++c) R_out[a * d + c] = T[(size_t)c * d + a];
+    for (int c = 0; c < d; ++c) R_out[a * d + c] = T_host[(size_t)c * d + a];
   if (inlier_flags)
-    for (int q = 0; q < m; ++q) inlier_flags[q] = w[(size_t)q] > 1.0 - 1e-8 ? 1 : 0;
-  if (iterations) *iterations = info[3];
+    for (int q = 0; q < m; ++q) inlier_flags[q] = w_host[(size_t)q] > 1.0 - 1e-8 ? 1 : 0;
+  if (iterations) *iterations = info_host[3];
   return DPGO_OK;
 }
 
@@ -2007,15 +1955,13 @@ int job_table(std::vector<dpgo_problem::JobTable<Job>> &tables, std::vector<uint
     if (t.key == key) { tab = &t; return DPGO_OK; }
   if (tables.size() >= STATUS_TABLES_MAX) {                // a table may still be read by a launch in flight
     DPGO_CUDA(cudaDeviceSynchronize());
-    free_dev(tables.front().d_jobs);
     tables.erase(tables.begin());
   }
   std::vector<Job> jobs((size_t)count);
   const int ctas = fill(jobs);
-  Job *d_jobs = nullptr;
-  DPGO_CUDA(cudaMalloc(&d_jobs, sizeof(Job) * (size_t)count));
-  DPGO_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(Job) * (size_t)count, cudaMemcpyHostToDevice, st));
-  tables.push_back({std::move(key), d_jobs, ctas});
+  DevBuf<Job> d_jobs;
+  DPGO_CUDA(d_jobs.assign(jobs.data(), jobs.size(), st));
+  tables.push_back({std::move(key), std::move(d_jobs), ctas});
   tab = &tables.back();
   return DPGO_OK;
 }
@@ -2048,24 +1994,24 @@ int dpgo_agents_status_async(dpgo_problem_t *const *agents, int count, const int
   DPGO_CUDA(cudaSetDevice(lead->device));
   cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
   const dpgo_problem::JobTable<dpgo::StatusJob> *tab = nullptr;
-  DPGO_TRY(job_table(lead->status_tables, key, count, st, [&](std::vector<dpgo::StatusJob> &jobs) {
+  DPGO_TRY(job_table(lead->status.tables, key, count, st, [&](std::vector<dpgo::StatusJob> &jobs) {
     int ctas = 0;
     for (int i = 0; i < count; ++i) {
       const dpgo_problem *p = agents[i];
       dpgo::StatusJob &J = jobs[(size_t)i];
       J.n = p->n;
       J.cta0 = ctas;
-      J.rowptr = p->d_rowptr; J.bcol = p->d_bcol; J.bval = p->d_bval;
-      J.X = p->d_vec[dpgo::V_X0]; J.G = p->d_G;
-      J.opt_record = p->d_opt_record;
-      J.partials = p->d_status_part;
-      J.ticket = p->d_status_ticket;
+      J.rowptr = p->bsr.rowptr.get(); J.bcol = p->bsr.bcol.get(); J.bval = p->bsr.bval.get();
+      J.X = p->vec[dpgo::V_X0].get(); J.G = p->G.get();
+      J.opt_record = p->status.opt_record.get();
+      J.partials = p->status.part.get();
+      J.ticket = p->status.ticket.get();
       J.out = status_dev + (size_t)slot[i] * DPGO_STATUS_DOUBLES;
       ctas += dpgo::status_ctas(p->n);
     }
     return ctas;
   }, tab));
-  DPGO_CUDA(dpgo::launch_agents_status(lead->r, lead->dh, count, tab->ctas, tab->d_jobs, st));
+  DPGO_CUDA(dpgo::launch_agents_status(lead->r, lead->dh, count, tab->ctas, tab->jobs.get(), st));
   return DPGO_OK;
 }
 
@@ -2073,11 +2019,11 @@ int dpgo_agent_trajectory_global(dpgo_problem_t *p, const double *anchor_host, d
   DPGO_TRY(require_device());
   DPGO_REQUIRE(anchor_host && T_host, DPGO_ERR_INVALID_ARG, "null anchor or trajectory");
   DPGO_CHECK_HANDLE(p);
-  if (!p->d_anchor) DPGO_CUDA(cudaMalloc(&p->d_anchor, sizeof(double) * p->ts));
-  if (!p->d_traj) DPGO_CUDA(cudaMalloc(&p->d_traj, sizeof(double) * (size_t)p->d * p->N));
-  DPGO_CUDA(cudaMemcpyAsync(p->d_anchor, anchor_host, sizeof(double) * p->ts, cudaMemcpyHostToDevice, p->stream));
-  DPGO_CUDA(dpgo::launch_trajectory_global(p->r, p->dh, p->n, p->d_anchor, p->d_vec[dpgo::V_X0], p->d_traj, p->stream));
-  DPGO_CUDA(cudaMemcpyAsync(T_host, p->d_traj, sizeof(double) * (size_t)p->d * p->N, cudaMemcpyDeviceToHost, p->stream));
+  if (!p->anchor) DPGO_CUDA(p->anchor.alloc((size_t)p->ts));
+  if (!p->traj) DPGO_CUDA(p->traj.alloc((size_t)p->d * p->N));
+  DPGO_CUDA(p->anchor.upload(anchor_host, (size_t)p->ts, p->stream));
+  DPGO_CUDA(dpgo::launch_trajectory_global(p->r, p->dh, p->n, p->anchor.get(), p->vec[dpgo::V_X0].get(), p->traj.get(), p->stream));
+  DPGO_CUDA(cudaMemcpyAsync(T_host, p->traj.get(), sizeof(double) * (size_t)p->d * p->N, cudaMemcpyDeviceToHost, p->stream));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
 }
@@ -2121,9 +2067,9 @@ int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, cons
     DPGO_REQUIRE(p->device == lead->device && p->d == lead->d && p->r == lead->r, DPGO_ERR_INVALID_ARG,
                  "the agents of one accelerated call must share the device, d and r");
     DPGO_ACC_READY(p);
-    DPGO_REQUIRE(p->d_pub_slot && p->pub_slot_unique, DPGO_ERR_STATE,
+    DPGO_REQUIRE(p->pub.slot && p->pub.slot_unique, DPGO_ERR_STATE,
                  "the agent needs a public pose list without duplicates (dpgo_agent_set_public_poses)");
-    DPGO_REQUIRE(p->num_public == 0 || (send_dev[i] && send_aux_dev[i]), DPGO_ERR_INVALID_ARG, "null send buffer");
+    DPGO_REQUIRE(p->pub.num == 0 || (send_dev[i] && send_aux_dev[i]), DPGO_ERR_INVALID_ARG, "null send buffer");
     key.push_back((uint64_t)(uintptr_t)p);
     key.push_back(p->generation);
     key.push_back((uint64_t)(active_flags[i] != 0));
@@ -2133,7 +2079,7 @@ int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, cons
   DPGO_CUDA(cudaSetDevice(lead->device));
   cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
   const dpgo_problem::JobTable<dpgo::AccelJob> *tab = nullptr;
-  DPGO_TRY(job_table(lead->accel_tables, key, count, st, [&](std::vector<dpgo::AccelJob> &jobs) {
+  DPGO_TRY(job_table(lead->acc.tables, key, count, st, [&](std::vector<dpgo::AccelJob> &jobs) {
     int ctas = 0;
     for (int i = 0; i < count; ++i) {
       const dpgo_problem *p = agents[i];
@@ -2141,21 +2087,21 @@ int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, cons
       J.n = p->n;
       J.cta0 = ctas;
       J.active = active_flags[i] != 0;
-      J.X = p->d_vec[dpgo::V_X0]; J.Y = p->d_acc[0]; J.V = p->d_acc[1]; J.XP = p->d_acc[2];
-      J.state = p->d_acc_state;
-      J.opt_record = p->d_opt_record;
-      J.pub_slot = p->d_pub_slot;
+      J.X = p->vec[dpgo::V_X0].get(); J.Y = p->acc.vec[0].get(); J.V = p->acc.vec[1].get(); J.XP = p->acc.vec[2].get();
+      J.state = p->acc.state.get();
+      J.opt_record = p->status.opt_record.get();
+      J.pub_slot = p->pub.slot.get();
       J.send_x = send_dev[i]; J.send_y = send_aux_dev[i];
-      J.ticket = p->d_acc_ticket;
+      J.ticket = p->acc.ticket.get();
       ctas += dpgo::accel_ctas(p->n);
     }
     return ctas;
   }, tab));
-  DPGO_CUDA(dpgo::launch_accel_agents(lead->r, lead->dh, count, tab->ctas, tab->d_jobs, momentum_N, restart_interval, st));
+  DPGO_CUDA(dpgo::launch_accel_agents(lead->r, lead->dh, count, tab->ctas, tab->jobs.get(), momentum_N, restart_interval, st));
   for (int i = 0; i < count; ++i) {
     dpgo_problem *p = agents[i];
-    ++p->acc_rounds;
-    p->acc_restart_due = (p->acc_rounds + 1) % restart_interval == 0;
+    ++p->acc.rounds;
+    p->acc.restart_due = (p->acc.rounds + 1) % restart_interval == 0;
   }
   return DPGO_OK;
 }
@@ -2163,27 +2109,27 @@ int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, cons
 static int issue_accel_round(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
                              const double *gathered_dev, const double *gathered_aux_dev, int64_t num_slots, cudaStream_t main) {
   dpgo_problem *lead = agents[0];
-  DPGO_CUDA(cudaEventRecord(lead->ev_fork, main));
+  DPGO_CUDA(cudaEventRecord(lead->ev_fork.get(), main));
   for (int i = 0; i < num_active; ++i) {
     dpgo_problem *p = agents[i];
-    StreamSwap swap(p, p->cluster ? p->own_stream : main);   // cluster steps side by side, full-grid steps in order
-    double *X = p->d_vec[dpgo::V_X0], *Y = p->d_acc[0], *V = p->d_acc[1], *XP = p->d_acc[2];
-    if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork, 0));
+    StreamSwap swap(p, p->cluster ? p->own_stream.get() : main);   // cluster steps side by side, full-grid steps in order
+    double *X = p->vec[dpgo::V_X0].get(), *Y = p->acc.vec[0].get(), *V = p->acc.vec[1].get(), *XP = p->acc.vec[2].get();
+    if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork.get(), 0));
     DPGO_TRY(dpgo_agent_build_G(p, gathered_aux_dev, num_slots));
     DPGO_CUDA(cudaMemcpyAsync(X, Y, p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
     DPGO_TRY(dpgo_optimize_resident_async(p, params));
-    DPGO_CUDA(dpgo::launch_accel_finish(p->r, p->dh, p->n, X, Y, V, XP, p->d_acc_state,
-                                        p->acc_restart_due ? dpgo::ACCEL_FINISH_V_RESTART : dpgo::ACCEL_FINISH_V, p->d_acc_part,
-                                        p->d_acc_ticket + 1, p->d_opt_record, p->stream));
-    if (p->acc_restart_due) {
+    DPGO_CUDA(dpgo::launch_accel_finish(p->r, p->dh, p->n, X, Y, V, XP, p->acc.state.get(),
+                                        p->acc.restart_due ? dpgo::ACCEL_FINISH_V_RESTART : dpgo::ACCEL_FINISH_V, p->acc.part.get(),
+                                        p->acc.ticket.get() + 1, p->status.opt_record.get(), p->stream));
+    if (p->acc.restart_due) {
       DPGO_TRY(dpgo_agent_build_G(p, gathered_dev, num_slots));
       DPGO_TRY(dpgo_optimize_resident_async(p, params));
-      DPGO_CUDA(dpgo::launch_accel_finish(p->r, p->dh, p->n, X, Y, V, XP, p->d_acc_state, dpgo::ACCEL_FINISH_RESTART_END,
-                                          p->d_acc_part, p->d_acc_ticket + 1, p->d_opt_record, p->stream));
+      DPGO_CUDA(dpgo::launch_accel_finish(p->r, p->dh, p->n, X, Y, V, XP, p->acc.state.get(), dpgo::ACCEL_FINISH_RESTART_END,
+                                          p->acc.part.get(), p->acc.ticket.get() + 1, p->status.opt_record.get(), p->stream));
     }
     if (p->stream != main) {
-      DPGO_CUDA(cudaEventRecord(p->ev_done, p->stream));
-      DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done, 0));
+      DPGO_CUDA(cudaEventRecord(p->ev_done.get(), p->stream));
+      DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done.get(), 0));
     }
   }
   return DPGO_OK;
@@ -2198,9 +2144,9 @@ int dpgo_agents_accel_round_async(dpgo_problem_t *const *agents, int num_active,
   for (int i = 0; i < num_active; ++i) {
     DPGO_CHECK_HANDLE(agents[i]);
     DPGO_ACC_READY(agents[i]);
-    DPGO_REQUIRE(agents[i]->d_acc_state && agents[i]->acc_rounds > 0, DPGO_ERR_STATE,
+    DPGO_REQUIRE(agents[i]->acc.state && agents[i]->acc.rounds > 0, DPGO_ERR_STATE,
                  "dpgo_agents_accel_begin_async has not been called");
-    DPGO_REQUIRE(gathered_aux_dev || agents[i]->num_edges == 0, DPGO_ERR_INVALID_ARG, "null gathered buffer");
+    DPGO_REQUIRE(gathered_aux_dev || agents[i]->shared.num_edges == 0, DPGO_ERR_INVALID_ARG, "null gathered buffer");
   }
   cudaStream_t main = nullptr;
   bool graph = false;
@@ -2209,7 +2155,7 @@ int dpgo_agents_accel_round_async(dpgo_problem_t *const *agents, int num_active,
   if (!graph) return issue();
   std::vector<uint64_t> key = round_key(0x6163630000ull, agents, num_active, params, main, num_slots);   // "acc"
   for (int i = 0; i < num_active; ++i)
-    key.push_back((uint64_t)agents[i]->acc_restart_due);    // two variants per active set: plain and restart rounds
+    key.push_back((uint64_t)agents[i]->acc.restart_due);    // two variants per active set: plain and restart rounds
   key.push_back((uint64_t)(uintptr_t)gathered_dev);
   key.push_back((uint64_t)(uintptr_t)gathered_aux_dev);
   return replay_or_issue(agents[0], key, main, issue);
@@ -2230,19 +2176,16 @@ int dpgo_agents_set_agent_graph(dpgo_problem_t *lead, int num_agents, const int3
   }
   DPGO_CUDA(cudaSetDevice(lead->device));
   DPGO_CUDA(cudaDeviceSynchronize());                       // the old buffers may still be read by a round in flight
-  free_dev(lead->d_sel_ptr); free_dev(lead->d_sel_adj); free_dev(lead->d_sel_mask); free_dev(lead->d_sel_log);
-  for (auto *b : lead->sel_retired) cudaFree(b);
-  lead->sel_retired.clear();
+  lead->sel = {};
+  dpgo_problem::Select &S = lead->sel;
   const int m = adj_ptr[num_agents];
-  DPGO_CUDA(cudaMalloc(&lead->d_sel_ptr, sizeof(int) * (size_t)(num_agents + 1)));
-  DPGO_CUDA(cudaMalloc(&lead->d_sel_adj, sizeof(int) * (size_t)std::max(m, 1)));
-  DPGO_CUDA(cudaMalloc(&lead->d_sel_mask, (size_t)num_agents));
-  if (!lead->d_sel_count) DPGO_CUDA(cudaMalloc(&lead->d_sel_count, sizeof(unsigned long long)));
-  DPGO_CUDA(cudaMemcpy(lead->d_sel_ptr, adj_ptr, sizeof(int) * (size_t)(num_agents + 1), cudaMemcpyHostToDevice));
-  if (m) DPGO_CUDA(cudaMemcpy(lead->d_sel_adj, adj, sizeof(int) * (size_t)m, cudaMemcpyHostToDevice));
-  DPGO_CUDA(cudaMemset(lead->d_sel_count, 0, sizeof(unsigned long long)));
-  lead->sel_k = num_agents;
-  lead->sel_rounds = lead->sel_cap = 0;
+  DPGO_CUDA(S.ptr.assign(adj_ptr, (size_t)num_agents + 1, lead->stream));
+  DPGO_CUDA(S.adj.assign(adj, (size_t)m, lead->stream));
+  DPGO_CUDA(S.mask.alloc((size_t)num_agents));
+  DPGO_CUDA(S.count.alloc(1));
+  DPGO_CUDA(cudaMemsetAsync(S.count.get(), 0, sizeof(unsigned long long), lead->stream));
+  DPGO_CUDA(cudaStreamSynchronize(lead->stream));
+  S.k = num_agents;
   ++lead->generation;
   return DPGO_OK;
 }
@@ -2267,31 +2210,32 @@ int dpgo_agents_select_round_async(dpgo_problem_t *const *agents, int count, con
   DPGO_REQUIRE(count > 0 && agents && agent_index && params && records_dev && send_dev, DPGO_ERR_INVALID_ARG, "bad arguments");
   dpgo_problem *lead = agents[0];
   DPGO_CHECK_HANDLE(lead);
-  DPGO_REQUIRE(lead->sel_k > 0, DPGO_ERR_STATE, "dpgo_agents_set_agent_graph has not been called for the first agent");
-  std::vector<char> seen((size_t)lead->sel_k, 0);
+  DPGO_REQUIRE(lead->sel.k > 0, DPGO_ERR_STATE, "dpgo_agents_set_agent_graph has not been called for the first agent");
+  std::vector<char> seen((size_t)lead->sel.k, 0);
   for (int i = 0; i < count; ++i) {
-    DPGO_REQUIRE(agent_index[i] >= 0 && agent_index[i] < lead->sel_k && !seen[(size_t)agent_index[i]], DPGO_ERR_INVALID_ARG,
+    DPGO_REQUIRE(agent_index[i] >= 0 && agent_index[i] < lead->sel.k && !seen[(size_t)agent_index[i]], DPGO_ERR_INVALID_ARG,
                  "agent indices must be distinct and below the agent graph's size");
     seen[(size_t)agent_index[i]] = 1;
   }
   cudaStream_t main = nullptr;
   bool graph = false;
   DPGO_TRY(round_preamble(agents, count, params, stream, main, graph));
-  if (lead->sel_rounds == lead->sel_cap) {                  // the log doubles; the old buffer is freed after the next read
-    const long long cap = std::max(64LL, 2 * lead->sel_cap);
-    unsigned char *grown = nullptr;
-    DPGO_CUDA(cudaMalloc(&grown, (size_t)cap * lead->sel_k));
-    if (lead->d_sel_log) {
-      DPGO_CUDA(cudaMemcpyAsync(grown, lead->d_sel_log, (size_t)lead->sel_rounds * lead->sel_k, cudaMemcpyDeviceToDevice, main));
-      lead->sel_retired.push_back(lead->d_sel_log);
+  dpgo_problem::Select &S = lead->sel;
+  if (S.rounds == S.cap) {                                  // the log doubles; the old buffer is freed after the next read
+    const long long cap = std::max(64LL, 2 * S.cap);
+    DevBuf<unsigned char> grown;
+    DPGO_CUDA(grown.alloc((size_t)cap * S.k));
+    if (S.log) {
+      DPGO_CUDA(cudaMemcpyAsync(grown.get(), S.log.get(), (size_t)S.rounds * S.k, cudaMemcpyDeviceToDevice, main));
+      S.retired.push_back(std::move(S.log));
     }
-    lead->d_sel_log = grown;
-    lead->sel_cap = cap;
+    S.log = std::move(grown);
+    S.cap = cap;
   }
   auto issue = [&]() -> int {
-    DPGO_CUDA(dpgo::launch_select_independent(lead->sel_k, records_dev, lead->d_sel_ptr, lead->d_sel_adj, lead->d_sel_mask,
-                                              lead->d_sel_log, lead->d_sel_count, main));
-    GateSet gates(agents, count, lead->d_sel_mask, agent_index);
+    DPGO_CUDA(dpgo::launch_select_independent(S.k, records_dev, S.ptr.get(), S.adj.get(), S.mask.get(), S.log.get(),
+                                              S.count.get(), main));
+    GateSet gates(agents, count, S.mask.get(), agent_index);
     return issue_round(agents, count, params, gathered_dev, num_slots, send_dev, main, 0);
   };
   int rc = DPGO_OK;
@@ -2305,10 +2249,10 @@ int dpgo_agents_select_round_async(dpgo_problem_t *const *agents, int count, con
     }
     key.push_back((uint64_t)(uintptr_t)gathered_dev);
     key.push_back((uint64_t)(uintptr_t)records_dev);
-    key.push_back((uint64_t)(uintptr_t)lead->d_sel_log);
+    key.push_back((uint64_t)(uintptr_t)S.log.get());
     rc = replay_or_issue(lead, key, main, issue);
   }
-  if (rc == DPGO_OK) ++lead->sel_rounds;
+  if (rc == DPGO_OK) ++S.rounds;
   return rc;
 }
 
@@ -2316,16 +2260,15 @@ int dpgo_agents_selection_log(dpgo_problem_t *lead, int64_t first_round, int64_t
                               int64_t *total_rounds) {
   DPGO_TRY(require_device());
   DPGO_CHECK_HANDLE(lead);
-  DPGO_REQUIRE(lead->sel_k > 0, DPGO_ERR_STATE, "dpgo_agents_set_agent_graph has not been called for this agent");
+  DPGO_REQUIRE(lead->sel.k > 0, DPGO_ERR_STATE, "dpgo_agents_set_agent_graph has not been called for this agent");
   DPGO_REQUIRE(first_round >= 0 && max_rounds >= 0 && (max_rounds == 0 || out_host), DPGO_ERR_INVALID_ARG, "bad log range");
   DPGO_CUDA(cudaSetDevice(lead->device));
   DPGO_CUDA(cudaDeviceSynchronize());                       // the log is written on the streams of the round calls
-  for (auto *b : lead->sel_retired) cudaFree(b);
-  lead->sel_retired.clear();
-  if (total_rounds) *total_rounds = lead->sel_rounds;
-  const int64_t rows = std::max<int64_t>(0, std::min<int64_t>(max_rounds, lead->sel_rounds - first_round));
+  lead->sel.retired.clear();
+  if (total_rounds) *total_rounds = lead->sel.rounds;
+  const int64_t rows = std::max<int64_t>(0, std::min<int64_t>(max_rounds, lead->sel.rounds - first_round));
   if (rows > 0)
-    DPGO_CUDA(cudaMemcpy(out_host, lead->d_sel_log + (size_t)first_round * lead->sel_k, (size_t)rows * lead->sel_k,
+    DPGO_CUDA(cudaMemcpy(out_host, lead->sel.log.get() + (size_t)first_round * lead->sel.k, (size_t)rows * lead->sel.k,
                          cudaMemcpyDeviceToHost));
   return DPGO_OK;
 }
@@ -2334,9 +2277,9 @@ int dpgo_agent_accel_state(dpgo_problem_t *p, double *out3) {
   DPGO_TRY(require_device());
   DPGO_REQUIRE(out3, DPGO_ERR_INVALID_ARG, "null output");
   DPGO_CHECK_HANDLE(p);
-  DPGO_REQUIRE(p->d_acc_state, DPGO_ERR_STATE, "dpgo_agent_accel_init has not been called");
+  DPGO_REQUIRE(p->acc.state, DPGO_ERR_STATE, "dpgo_agent_accel_init has not been called");
   DPGO_CUDA(cudaDeviceSynchronize());                       // the record is written on the stream of the begin calls
-  DPGO_CUDA(cudaMemcpy(out3, p->d_acc_state, 3 * sizeof(double), cudaMemcpyDeviceToHost));
+  DPGO_CUDA(cudaMemcpy(out3, p->acc.state.get(), 3 * sizeof(double), cudaMemcpyDeviceToHost));
   return DPGO_OK;
 }
 

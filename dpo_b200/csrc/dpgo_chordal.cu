@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../../include/dpgo_b200.h"
+#include "dpgo_devbuf.cuh"
 #include "dpgo_rotation.cuh"
 
 namespace {
@@ -82,12 +83,6 @@ template <int D> __global__ void k_project_rotations(int n, const double *__rest
     for (int a = 0; a < D; ++a) out[(size_t)j * TS9 + c * B3 + a] = Rm[a][c];
 }
 
-struct DevBuf {
-  double *p = nullptr;
-  ~DevBuf() { if (p) cudaFree(p); }
-  cudaError_t alloc(size_t n) { return cudaMalloc(&p, sizeof(double) * std::max<size_t>(n, 1)); }
-};
-
 struct ProblemGuard {
   dpgo_problem_t *h = nullptr;
   ~ProblemGuard() { if (h) dpgo_problem_destroy(h); }
@@ -109,35 +104,35 @@ struct ProblemGuard {
 int pcg(dpgo_problem_t *h, int n, const double *diag_host, double *x, const double *b, double tol, int max_iter, int *iters,
         cudaStream_t st, std::string &err) {
   const int len = TS9 * n;
-  DevBuf r, z, p, q, dinv, sc;
+  dpgo::DevBuf<double> r, z, p, q, dinv, sc;
   CH_CUDA(r.alloc(len)); CH_CUDA(z.alloc(len)); CH_CUDA(p.alloc(len)); CH_CUDA(q.alloc(len)); CH_CUDA(dinv.alloc(3 * (size_t)n)); CH_CUDA(sc.alloc(8));
   std::vector<double> dh((size_t)3 * n);
   for (int i = 0; i < 3 * n; ++i) dh[(size_t)i] = (diag_host[i] > 0.0) ? 1.0 / diag_host[i] : 0.0;
   for (int k = 0; k < 3; ++k) dh[(size_t)k] = 0.0;                         // anchored tile
-  CH_CUDA(cudaMemcpyAsync(dinv.p, dh.data(), sizeof(double) * dh.size(), cudaMemcpyHostToDevice, st));
+  CH_CUDA(cudaMemcpyAsync(dinv.get(), dh.data(), sizeof(double) * dh.size(), cudaMemcpyHostToDevice, st));
   CH_CUDA(cudaMemsetAsync(x, 0, sizeof(double) * len, st));
-  CH_CUDA(cudaMemcpyAsync(r.p, b, sizeof(double) * len, cudaMemcpyDeviceToDevice, st));
+  CH_CUDA(cudaMemcpyAsync(r.get(), b, sizeof(double) * len, cudaMemcpyDeviceToDevice, st));
   const int TB = 256, GB = (len + TB - 1) / TB;
-  k_jacobi<<<GB, TB, 0, st>>>(len, r.p, dinv.p, z.p, p.p);
-  k_dot<<<1, 1024, 0, st>>>(len, r.p, z.p, sc.p + 0);
+  k_jacobi<<<GB, TB, 0, st>>>(len, r.get(), dinv.get(), z.get(), p.get());
+  k_dot<<<1, 1024, 0, st>>>(len, r.get(), z.get(), sc.get() + 0);
   double rz0 = 0.0;
-  CH_CUDA(cudaMemcpyAsync(&rz0, sc.p, sizeof(double), cudaMemcpyDeviceToHost, st));
+  CH_CUDA(cudaMemcpyAsync(&rz0, sc.get(), sizeof(double), cudaMemcpyDeviceToHost, st));
   CH_CUDA(cudaStreamSynchronize(st));
   *iters = 0;
   if (!(rz0 > 0.0)) return DPGO_OK;
   const int CHECK = 25;
   for (int it = 0; it < max_iter; ++it) {
-    CH_TRY(dpgo_spmv_device(h, p.p, q.p, 0));                               // q = p Q  (k_spmv_tma)
-    k_mask_anchor<<<1, 32, 0, st>>>(q.p);
-    k_dot<<<1, 1024, 0, st>>>(len, p.p, q.p, sc.p + 1);
-    k_update_xrz<<<GB, TB, 0, st>>>(len, sc.p, p.p, q.p, dinv.p, x, r.p, z.p);
-    k_dot<<<1, 1024, 0, st>>>(len, r.p, z.p, sc.p + 2);
-    k_update_p<<<GB, TB, 0, st>>>(len, sc.p, z.p, p.p);
-    k_rotate_scalars<<<1, 1, 0, st>>>(sc.p);
+    CH_TRY(dpgo_spmv_device(h, p.get(), q.get(), 0));                           // q = p Q  (k_spmv_tma)
+    k_mask_anchor<<<1, 32, 0, st>>>(q.get());
+    k_dot<<<1, 1024, 0, st>>>(len, p.get(), q.get(), sc.get() + 1);
+    k_update_xrz<<<GB, TB, 0, st>>>(len, sc.get(), p.get(), q.get(), dinv.get(), x, r.get(), z.get());
+    k_dot<<<1, 1024, 0, st>>>(len, r.get(), z.get(), sc.get() + 2);
+    k_update_p<<<GB, TB, 0, st>>>(len, sc.get(), z.get(), p.get());
+    k_rotate_scalars<<<1, 1, 0, st>>>(sc.get());
     *iters = it + 1;
     if ((it + 1) % CHECK == 0) {
       double rz = 0.0;
-      CH_CUDA(cudaMemcpyAsync(&rz, sc.p, sizeof(double), cudaMemcpyDeviceToHost, st));
+      CH_CUDA(cudaMemcpyAsync(&rz, sc.get(), sizeof(double), cudaMemcpyDeviceToHost, st));
       CH_CUDA(cudaStreamSynchronize(st));
       if (!(rz == rz)) { err = "chordal initialisation: conjugate gradients broke down"; return DPGO_ERR_CUDA; }
       if (rz <= tol * tol * rz0) break;
@@ -146,11 +141,6 @@ int pcg(dpgo_problem_t *h, int n, const double *diag_host, double *x, const doub
   CH_CUDA(cudaStreamSynchronize(st));
   return DPGO_OK;
 }
-
-struct StreamGuard {
-  cudaStream_t s = nullptr;
-  ~StreamGuard() { if (s) cudaStreamDestroy(s); }
-};
 
 thread_local std::string g_chordal_error;
 
@@ -208,10 +198,10 @@ int dpgo_chordal_initialization(int n, int d, int64_t m, const int32_t *p1, cons
     push(i, i, kAAt); push(j, j, kI); push(i, j, Rt); push(j, i, RtT);
     for (int c = 0; c < 3; ++c) { diag[(size_t)3 * i + c] += kAAt[c * 3 + c]; diag[(size_t)3 * j + c] += k; }
   }
-  StreamGuard sg;
-  CH_CUDA(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-  cudaStream_t st = sg.s;
-  DevBuf x, b, y;
+  cudaStream_t st = nullptr;
+  CH_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  const dpgo::Stream own(st);
+  dpgo::DevBuf<double> x, b, y;
   CH_CUDA(x.alloc(len)); CH_CUDA(b.alloc(len)); CH_CUDA(y.alloc(len));
   std::vector<double> tiles((size_t)len);                   // projected rotations, 3 x 3 tiles (column-major)
   {
@@ -222,18 +212,18 @@ int dpgo_chordal_initialization(int n, int d, int64_t m, const int32_t *p1, cons
     // right-hand side: X0 = [I, 0, ...];  b = -(X0 Q) on the free tiles
     std::vector<double> x0((size_t)len, 0.0);
     for (int k = 0; k < 3; ++k) x0[(size_t)k * 3 + k] = 1.0;
-    CH_CUDA(cudaMemcpyAsync(y.p, x0.data(), sizeof(double) * len, cudaMemcpyHostToDevice, st));
-    CH_TRY(dpgo_spmv_device(pr.h, y.p, x.p, 0));
-    k_scale_neg_mask<<<(len + 255) / 256, 256, 0, st>>>(len, x.p, b.p);
+    CH_CUDA(cudaMemcpyAsync(y.get(), x0.data(), sizeof(double) * len, cudaMemcpyHostToDevice, st));
+    CH_TRY(dpgo_spmv_device(pr.h, y.get(), x.get(), 0));
+    k_scale_neg_mask<<<(len + 255) / 256, 256, 0, st>>>(len, x.get(), b.get());
     int it = 0;
-    const int rc = pcg(pr.h, n, diag.data(), x.p, b.p, tol, max_iter, &it, st, err);
+    const int rc = pcg(pr.h, n, diag.data(), x.get(), b.get(), tol, max_iter, &it, st, err);
     if (rc != DPGO_OK) return rc;
     if (iterations2) iterations2[0] = it;
     // anchored tile = identity, then the projection onto SO(d) (pose 0 stays I)
-    CH_CUDA(cudaMemcpyAsync(x.p, x0.data(), sizeof(double) * TS9, cudaMemcpyHostToDevice, st));
-    if (d == 3) k_project_rotations<3><<<(n + 127) / 128, 128, 0, st>>>(n, x.p, y.p);
-    else k_project_rotations<2><<<(n + 127) / 128, 128, 0, st>>>(n, x.p, y.p);
-    CH_CUDA(cudaMemcpyAsync(tiles.data(), y.p, sizeof(double) * len, cudaMemcpyDeviceToHost, st));
+    CH_CUDA(cudaMemcpyAsync(x.get(), x0.data(), sizeof(double) * TS9, cudaMemcpyHostToDevice, st));
+    if (d == 3) k_project_rotations<3><<<(n + 127) / 128, 128, 0, st>>>(n, x.get(), y.get());
+    else k_project_rotations<2><<<(n + 127) / 128, 128, 0, st>>>(n, x.get(), y.get());
+    CH_CUDA(cudaMemcpyAsync(tiles.data(), y.get(), sizeof(double) * len, cudaMemcpyDeviceToHost, st));
     CH_CUDA(cudaStreamSynchronize(st));
   }
   // ---- translations: tau-weighted graph Laplacian (x I_3), right-hand side from the rotations:  gradient of
@@ -262,12 +252,12 @@ int dpgo_chordal_initialization(int n, int d, int64_t m, const int32_t *p1, cons
     CH_TRY(dpgo_problem_create(n, 2, 3, device, &pr.h));
     CH_TRY(dpgo_problem_set_stream(pr.h, (void *)st));
     CH_TRY(dpgo_problem_set_Q_blocks(pr.h, (int64_t)brow.size(), brow.data(), bcol.data(), blocks.data(), 0u));
-    CH_CUDA(cudaMemcpyAsync(b.p, rhs.data(), sizeof(double) * len, cudaMemcpyHostToDevice, st));
+    CH_CUDA(cudaMemcpyAsync(b.get(), rhs.data(), sizeof(double) * len, cudaMemcpyHostToDevice, st));
     int it = 0;
-    const int rc = pcg(pr.h, n, diag.data(), x.p, b.p, tol, max_iter, &it, st, err);
+    const int rc = pcg(pr.h, n, diag.data(), x.get(), b.get(), tol, max_iter, &it, st, err);
     if (rc != DPGO_OK) return rc;
     if (iterations2) iterations2[1] = it;
-    CH_CUDA(cudaMemcpyAsync(tsol.data(), x.p, sizeof(double) * len, cudaMemcpyDeviceToHost, st));
+    CH_CUDA(cudaMemcpyAsync(tsol.data(), x.get(), sizeof(double) * len, cudaMemcpyDeviceToHost, st));
     CH_CUDA(cudaStreamSynchronize(st));
   }
   // ---- T = [R_0 t_0 | R_1 t_1 | ...], d x (d+1) n column-major ----
