@@ -128,9 +128,12 @@ __global__ void __launch_bounds__(TMA_THREADS, 2)
         const unsigned ibytes = (unsigned)(((b1 - ib) + 3) & ~3) * 4u;
         const int rb = r0 & ~3;                                   // rowptr[r0 .. r1] inclusive
         const unsigned rbytes = (unsigned)(((r1 + 1 - rb) + 3) & ~3) * 4u;
+        // a group of empty rows whose first block index is a multiple of 4 has no index window (ibytes = 0).  The PTX ISA
+        // asks cp.async.bulk for a size that is a multiple of 16 and does not say what a size of 0 does, so no zero-size
+        // copy is issued; expect_tx counts the bytes of the copies that are
         mbar_expect_tx(&full[s], qbytes + ibytes + rbytes);
         if (qbytes) tma_load_1d(sq + (size_t)s * BT * 16, bval + (size_t)b0 * 16, qbytes, &full[s], pol);
-        tma_load_1d(sidx + s * IDX_CAP, bcol + ib, ibytes, &full[s], pol);
+        if (ibytes) tma_load_1d(sidx + s * IDX_CAP, bcol + ib, ibytes, &full[s], pol);
         tma_load_1d(srp + s * RP_CAP, rowptr + rb, rbytes, &full[s], pol);
       }
     }
