@@ -340,6 +340,15 @@ void nd_fill_info(const dpgo::nd::Hierarchy &H, const dpgo::nd::Plan &P, int64_t
   info[0] = H.nstages; info[1] = (int64_t)H.nodes.size(); info[2] = (int64_t)P.phases.size(); info[3] = H.blob_doubles * 8;
   info[4] = P.bytes_per_apply; info[5] = smax; info[6] = bmax; info[7] = H.nd_depth; info[8] = (int64_t)P.steps.size();
   info[9] = (int64_t)P.jobs.size(); info[10] = (int64_t)P.epis.size(); info[11] = P.max_ytiles; info[12] = P.max_slots;
+  info[13] = P.resident_bytes; info[14] = (int64_t)P.max_resident_doubles * 8;
+}
+
+// shared-memory sizes of the kernel's view of a plan (the staged areas the resident budget is what is left of)
+void nd_kernel_sizes(const dpgo::nd::Plan &plan, dpgo::KNd &K) {
+  K.max_ytiles = std::max(plan.max_ytiles, 1);
+  K.max_slots = std::max(plan.max_slots, 1);
+  K.max_gathers = K.max_ytiles;          // a step gathers at most what its shared-memory tiles hold
+  K.resident_doubles = 0;
 }
 
 dpgo::nd::Options nd_options(int grid, int r, bool cluster = false) {
@@ -389,15 +398,21 @@ int ensure_nd(dpgo_problem *p) {
   if (plan.max_ytiles > dpgo::ND_YCAP_TILES || plan.max_slots > dpgo::ND_SLOT_CAP)
     return fail(DPGO_ERR_UNSUPPORTED, "sparse exact preconditioner: plan exceeds the shared-memory capacities");
   dpgo_problem::Nd &F = p->nd;
-  nd_fill_info(*H, plan, F.info);
   if ((int)plan.phases.size() > dpgo::nd::MAX_PHASES)
     return fail(DPGO_ERR_UNSUPPORTED, "sparse exact preconditioner: too many phases");
-  F.H = std::move(H);
   dpgo::KNd &K = F.k;
+  nd_kernel_sizes(plan, K);
+  try {
+    // grid mode only: agents stepped side by side as clusters are slower with the resident columns than with L1 (16-agent
+    // sphere2500 / torus3D on one H100 80GB HBM3 at 400 W: 6818-6878 / 7689-7729 rounds/s against 7177-7222 / 7819-7855)
+    nd::assign_residency(plan, dpgo::OPT_THREADS / 32, p->cluster ? 0 : dpgo::nd_resident_budget(p->r, p->dh, K));
+  } catch (const std::exception &e) {
+    return fail(DPGO_ERR_UNSUPPORTED, std::string("sparse exact preconditioner setup: ") + e.what());
+  }
+  K.resident_doubles = plan.max_resident_doubles;
+  nd_fill_info(*H, plan, F.info);
+  F.H = std::move(H);
   for (size_t k = 0; k < plan.phases.size(); ++k) { K.dir[k] = plan.phases[k].dir; K.cta0[k] = plan.phases[k].cta0; }
-  K.max_ytiles = std::max(plan.max_ytiles, 1);
-  K.max_slots = std::max(plan.max_slots, 1);
-  K.max_gathers = K.max_ytiles;          // a step gathers at most what its shared-memory tiles hold
   DPGO_CUDA(F.cta_phase.assign(plan.cta_phase.data(), plan.cta_phase.size(), p->stream));
   DPGO_CUDA(F.steps.assign(plan.steps.data(), plan.steps.size(), p->stream));
   DPGO_CUDA(F.gathers.assign(plan.gathers.data(), plan.gathers.size(), p->stream));
@@ -1198,6 +1213,12 @@ int dpgo_nd_debug_emulate(int n, int d, int r, int64_t nb, const int32_t *brow, 
     nd::build_plan(H, opt, plan);
     if (plan.max_ytiles > opt.ycap_tiles || plan.max_slots > opt.slot_cap)
       return fail(DPGO_ERR_UNSUPPORTED, "plan exceeds the shared-memory capacities");
+    // residency as a launch of this plan would have it, or with DPGO_ND_RESIDENT_BYTES per CTA (verification)
+    dpgo::KNd K = {};
+    nd_kernel_sizes(plan, K);
+    int64_t budget = dpgo::nd_resident_budget(r, dh, K);
+    if (const char *e = std::getenv("DPGO_ND_RESIDENT_BYTES")) budget = std::atoll(e);
+    nd::assign_residency(plan, opt.warps, budget);
     nd::emulate_apply(H, plan, blob, r, V_host, Z_host);
     if (info16) nd_fill_info(H, plan, info16);
     if (const char *dump = std::getenv("DPGO_ND_DUMP_PLAN")) {            // per (phase, CTA) work statistics, CSV
@@ -1215,6 +1236,22 @@ int dpgo_nd_debug_emulate(int n, int d, int r, int64_t nb, const int32_t *brow, 
               mw += *std::max_element(w.begin(), w.end());
             }
             std::fprintf(fp, "%zu,%d,%d,%d,%d,%ld,%ld,%ld,%ld,%ld\n", ph, plan.phases[ph].dir, plan.phases[ph].stage, c, cp.s1 - cp.s0, gt, nj, jc, mw, ne);
+          }
+        std::fclose(fp);
+      }
+    }
+    if (const char *dump = std::getenv("DPGO_ND_DUMP_JOBS")) {            // residency of every job, CSV
+      if (FILE *fp = std::fopen(dump, "w")) {
+        std::fprintf(fp, "phase,cta,step,warp,ncols,nres,soff,budget\n");
+        for (size_t ph = 0; ph < plan.phases.size(); ++ph)
+          for (int c = 0; c < plan.grid; ++c) {
+            const nd::CtaPhase &cp = plan.cta_phase[(size_t)plan.phases[ph].cta0 + c];
+            for (int si = cp.s0; si < cp.s1; ++si)
+              for (int j = plan.steps[(size_t)si].j0; j < plan.steps[(size_t)si].j1; ++j) {
+                const nd::Job &jb = plan.jobs[(size_t)j];
+                std::fprintf(fp, "%zu,%d,%d,%d,%d,%d,%d,%lld\n", ph, c, si, (j - plan.steps[(size_t)si].j0) % opt.warps, jb.ncols,
+                             jb.nres, jb.soff, (long long)budget);
+              }
           }
         std::fclose(fp);
       }

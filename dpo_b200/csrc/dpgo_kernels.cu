@@ -746,7 +746,7 @@ __device__ __forceinline__ int4 ld_int4(const void *p) { return __ldg(reinterpre
 
 template <int R, int DH, bool CLOCK>
 __device__ void phase_nd(const KParams &kp, int ph, const double *V, int cb, double *Zout, double *ys, double *slots,
-                         int4 *grec, double (&acc)[NRED]) {
+                         int4 *grec, double *sres, bool fill, double (&acc)[NRED]) {
   constexpr int TS = R * DH;
   constexpr int SG = SubGroup<R>::SG;
   constexpr int SGW = 32 / SG;
@@ -814,7 +814,9 @@ __device__ void phase_nd(const KParams &kp, int ph, const double *V, int cb, dou
     // ---- jobs: DMMA m8n8k4 -- A = 8 panel rows x 4 columns (one coalesced 256-byte warp load), B = 4 columns x r
     //      right-hand sides from shared memory, D = 8 x 8 accumulators (r columns used): 1 LDG + 1 LDS + 1 DMMA per
     //      4 columns instead of 1 LDG + r LDS + r DFMA per lane, and no shuffle reduction.  Two accumulator chains;
-    //      the next job's record is fetched ahead.
+    //      the next job's record is fetched ahead.  The rounds of the job's resident columns (nd::Job) read A from the
+    //      CTA's region in shared memory, one 256-byte group per load in lane order; the launch's first application
+    //      (fill) still streams them and leaves them there.  Either way every DMMA gets the same operands.
     {
       const int r8 = lane >> 2, k4 = lane & 3;
       const bool bval_lane = (r8 < R);
@@ -826,13 +828,20 @@ __device__ void phase_nd(const KParams &kp, int ph, const double *V, int cb, dou
         int4 na = make_int4(0, 0, 0, 0), nb = make_int4(0, 0, 0, 0);
         if (jn < j1) { na = ld_int4(N.jobs + jn); nb = ld_int4(reinterpret_cast<const int4 *>(N.jobs + jn) + 1); }
         const long long mat = ((long long)(unsigned)ja.x) | ((long long)ja.y << 32);
-        const int ncols = ja.z, ycol = ja.w, slot = jb.x, accum = jb.y;
+        const int ncols = ja.z, ycol = ja.w, slot = jb.x, accum = jb.y, nres = jb.w;
         const double *mp = N.blob + mat + (size_t)k4 * nd::PANEL_ROWS + r8;      // A[r8][k4] of the first column group
         const double *yp = ys + (size_t)(ycol + k4) * R + (bval_lane ? r8 : 0);    // B[k4][r8]
+        double *rp = sres + jb.z + lane;                                           // A[r8][k4] of resident group 0
         double d0 = 0.0, d1 = 0.0, f0 = 0.0, f1 = 0.0;
         for (int j = 0; j < ncols; j += 32) {                                        // 8 column groups (32 columns) per round
           double am[8], bm[8];
-          if (j + 32 <= ncols) {
+          const bool res = j < nres;                                                 // whole rounds are resident
+          if (res && !fill) {
+#pragma unroll
+            for (int u = 0; u < 8; ++u) am[u] = (j + 4 * u < ncols) ? rp[(size_t)(j + 4 * u) * nd::PANEL_ROWS] : 0.0;
+#pragma unroll
+            for (int u = 0; u < 8; ++u) bm[u] = (bval_lane && j + 4 * u + k4 < ncols) ? yp[(size_t)(j + 4 * u) * R] : 0.0;
+          } else if (j + 32 <= ncols) {
 #pragma unroll
             for (int u = 0; u < 8; ++u) am[u] = ld_stream(mp + (size_t)(j + 4 * u) * nd::PANEL_ROWS);
 #pragma unroll
@@ -842,6 +851,11 @@ __device__ void phase_nd(const KParams &kp, int ph, const double *V, int cb, dou
             for (int u = 0; u < 8; ++u) am[u] = (j + 4 * u + k4 < ncols) ? ld_stream(mp + (size_t)(j + 4 * u) * nd::PANEL_ROWS) : 0.0;
 #pragma unroll
             for (int u = 0; u < 8; ++u) bm[u] = (bval_lane && j + 4 * u + k4 < ncols) ? yp[(size_t)(j + 4 * u) * R] : 0.0;
+          }
+          if (res && fill) {
+#pragma unroll
+            for (int u = 0; u < 8; ++u)
+              if (j + 4 * u < ncols) rp[(size_t)(j + 4 * u) * nd::PANEL_ROWS] = am[u];
           }
 #pragma unroll
           for (int u = 0; u < 8; u += 2) {
@@ -1083,17 +1097,25 @@ template <int R, int DH, bool FULL> __global__ void __launch_bounds__(OPT_THREAD
   const dpgo_opt_params_t prm = kp.prm;
   const int precond = prm.precond;
   const bool exact = (precond == DPGO_PRECOND_DENSE_EXACT) || (precond == DPGO_PRECOND_SPARSE_EXACT);
+  dpgo_opt_result_t res;
+  res.success = 0; res.tcg_status = DPGO_TCG_NOT_RUN; res.tcg_iterations = 0; res.outer_iterations = 0;
+  res.rejections = 0; res.spmv_passes = 0; res.precond_applies = 0; res.reserved0 = 0;
+  res.f_init = res.gradnorm_init = res.f_opt = res.gradnorm_opt = res.relative_change = res.elapsed_ms = 0.0;
+  res.quad_init = res.lin_init = 0.0;
   double acc[NRED];
   // sparse exact preconditioner: shared memory = gathered input tiles + partial-sum slots (aliases the dense ring)
   double *nd_ys = sV;
   double *nd_slots = sV + (size_t)kp.nd.max_ytiles * R * DH;
   int4 *nd_grec = reinterpret_cast<int4 *>((reinterpret_cast<uintptr_t>(nd_slots + (size_t)kp.nd.max_slots * nd::PANEL_ROWS * R) + 15) & ~(uintptr_t)15);
+  // the CTA's resident panel columns, aliased by nothing; the launch's first application (no application counted yet:
+  // z0 of the first outer iteration, or the single-operation entry point) fills them
+  double *nd_res = reinterpret_cast<double *>(nd_grec + 2 * (size_t)kp.nd.max_gathers);
   // Z = P_X( (Q + 0.1 I)^-1 V ), returns <Z, V> in acc[0]; every phase ends with a grid barrier
   auto apply_exact = [&](const double *Vv, int cbx, double *Zout) {
     if (!FULL || precond == DPGO_PRECOND_SPARSE_EXACT) {     // the lean variant is never launched with the dense one
       zero(acc);
       for (int ph = 0; ph < kp.nd.nphases; ++ph) {
-        phase_nd<R, DH, FULL>(kp, ph, Vv, cbx, Zout, nd_ys, nd_slots, nd_grec, acc);
+        phase_nd<R, DH, FULL>(kp, ph, Vv, cbx, Zout, nd_ys, nd_slots, nd_grec, nd_res, res.precond_applies == 0, acc);
         if (ph + 1 < kp.nd.nphases) { phase_end<0>(kp, bc, acc); tick(8 + min(ph, 15)); }
       }
       phase_end<1>(kp, bc, acc);
@@ -1109,11 +1131,6 @@ template <int R, int DH, bool FULL> __global__ void __launch_bounds__(OPT_THREAD
       tick(2);
     }
   };
-  dpgo_opt_result_t res;
-  res.success = 0; res.tcg_status = DPGO_TCG_NOT_RUN; res.tcg_iterations = 0; res.outer_iterations = 0;
-  res.rejections = 0; res.spmv_passes = 0; res.precond_applies = 0; res.reserved0 = 0;
-  res.f_init = res.gradnorm_init = res.f_opt = res.gradnorm_opt = res.relative_change = res.elapsed_ms = 0.0;
-  res.quad_init = res.lin_init = 0.0;
 
   int cur = 0;   // which X buffer holds the current iterate
 
@@ -1495,15 +1512,29 @@ __global__ void k_edge_weights(int64_t m, const int *__restrict__ p1, const int 
 // launchers
 // ---------------------------------------------------------------------------------------------
 // Dynamic shared memory of one launch: the reduction scratch, plus what the launch's preconditioner stages (the dense
-// ring or the sparse plan's tiles and slots).  Asking for no more than needed leaves the rest of the SM's 228 KB to L1,
-// which now keeps the constant data (block-CSR, plan records) across phases.
-template <int R, int DH> static size_t optimize_smem_doubles(const KParams &kp, bool max_only) {
+// ring or the sparse plan's tiles, slots and resident panel columns).  Launches without the sparse plan ask for no more
+// than they stage and leave the rest of the SM's 228 KB to L1; the sparse plan's resident columns take what it leaves.
+template <int R, int DH> static size_t nd_staged_doubles(const KNd &nd) {
+  return (OPT_THREADS / 32) * NRED + 2 * NRED + SP_CACHE_INTS / 2 + (size_t)nd.max_ytiles * R * DH +
+         (size_t)(nd.max_slots + 1) * nd::PANEL_ROWS * R + 4 * (size_t)nd.max_gathers + 8;
+}
+
+template <int R, int DH> static size_t optimize_smem_doubles(const KParams &kp) {
   const size_t base = (OPT_THREADS / 32) * NRED + 2 * NRED + SP_CACHE_INTS / 2;
   const size_t dense = (size_t)DENSE_PER_MAX * R + (size_t)DENSE_RING_DOUBLES + 2 * DENSE_NST + (size_t)SYM_META_DOUBLES;
-  if (max_only || kp.prm.precond == DPGO_PRECOND_DENSE_EXACT) return base + dense;
-  if (kp.prm.precond == DPGO_PRECOND_SPARSE_EXACT)
-    return base + (size_t)kp.nd.max_ytiles * R * DH + (size_t)(kp.nd.max_slots + 1) * nd::PANEL_ROWS * R + 4 * (size_t)kp.nd.max_gathers + 8;
+  if (kp.prm.precond == DPGO_PRECOND_DENSE_EXACT) return base + dense;
+  if (kp.prm.precond == DPGO_PRECOND_SPARSE_EXACT) return nd_staged_doubles<R, DH>(kp.nd) + (size_t)kp.nd.resident_doubles;
   return base + 8;
+}
+
+// Everything a CTA may ask for beyond what the plan stages.  No L1 reserve: the step is faster with every resident round
+// than with L1 for the block-CSR values and plan records.  sphere2500, 1 agent, H100 80GB HBM3 at 400 W, two alternating
+// bench.py runs each: 2023 / 2041 it/s with no reserve, 1987 / 1998 with 32 KB and 1988 / 2009 with 64 KB kept for L1,
+// against 1920 / 1924 without resident columns.
+int64_t nd_resident_budget(int r, int dh, const KNd &nd) {
+  int64_t staged = 0;
+  DPGO_DISPATCH(r, dh, staged = (int64_t)nd_staged_doubles<R, DH>(nd) * (int64_t)sizeof(double));
+  return std::max<int64_t>(0, (int64_t)OPT_SMEM_LIMIT - staged);
 }
 
 // The full kernel (dense preconditioner, phase clock) or the lean one (everything else).
@@ -1515,18 +1546,17 @@ template <int R, int DH> static cudaError_t launch_optimize_t(const KParams &kp_
   KParams kp = kp_in;
   const bool full = (kp.phase_ns != nullptr) || (kp.prm.precond == DPGO_PRECOND_DENSE_EXACT);
   const void *kern = optimize_kernel<R, DH>(full);
-  const size_t smem_max = optimize_smem_doubles<R, DH>(kp, true) * sizeof(double);
   static_assert((size_t)ND_YCAP_TILES * R * DH + (size_t)(ND_SLOT_CAP + 1) * nd::PANEL_ROWS * R + 4 * (size_t)ND_YCAP_TILES + 8 <=
                     (size_t)DENSE_PER_MAX * R + (size_t)DENSE_RING_DOUBLES + 2 * DENSE_NST + (size_t)SYM_META_DOUBLES,
                 "the sparse plan's capacities must fit the kernel's maximum shared memory");
-  kp.smem_doubles = (int)optimize_smem_doubles<R, DH>(kp, false);
+  kp.smem_doubles = (int)optimize_smem_doubles<R, DH>(kp);
   const size_t smem = (size_t)kp.smem_doubles * sizeof(double);
   // per device and kernel variant
   static bool attr_set[2][64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr_set[full][dev]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, OPT_SMEM_LIMIT);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr_set[full][dev] = true;
   }
@@ -1568,9 +1598,13 @@ template <int R, int DH> static cudaError_t launch_optimize_t(const KParams &kp_
   return cudaLaunchCooperativeKernel(kern, dim3(kp.grid), dim3(OPT_THREADS), args, smem, stream);
 }
 
+// Both checks ask for the largest request a launch may make (OPT_SMEM_LIMIT), so that no plan can exceed what they allowed.
 template <int R, int DH> static int max_cluster_t(int device) {
-  const size_t smem = ((OPT_THREADS / 32) * NRED + 2 * NRED + SP_CACHE_INTS / 2 + (size_t)ND_SMEM_NEED_SMALL) * sizeof(double);
-  for (int f = 0; f < 2; ++f) cudaFuncSetAttribute(optimize_kernel<R, DH>(f != 0), cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+  const size_t smem = OPT_SMEM_LIMIT;
+  for (int f = 0; f < 2; ++f) {
+    cudaFuncSetAttribute(optimize_kernel<R, DH>(f != 0), cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    cudaFuncSetAttribute(optimize_kernel<R, DH>(f != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, OPT_SMEM_LIMIT);
+  }
   for (int cs : {16, 8}) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(cs);
@@ -1593,8 +1627,11 @@ template <int R, int DH> static int max_cluster_t(int device) {
 }
 
 template <int R, int DH> static int max_grid_t(int device) {
-  const size_t smem = ((OPT_THREADS / 32) * NRED + 2 * NRED + SP_CACHE_INTS / 2 + (size_t)DENSE_PER_MAX * R + (size_t)DENSE_RING_DOUBLES + 2 * DENSE_NST + (size_t)SYM_META_DOUBLES) * sizeof(double);
-  int per_sm = 1, sms = 0;
+  const size_t smem = OPT_SMEM_LIMIT;
+  int per_sm = 1, sms = 0, optin = 0;
+  // the sparse plan's budget assumes the H100's opt-in limit: a device with less cannot run the kernel as planned
+  if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess || optin < OPT_SMEM_LIMIT)
+    return 0;
   for (int f = 0; f < 2; ++f) {
     const void *kern = optimize_kernel<R, DH>(f != 0);
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

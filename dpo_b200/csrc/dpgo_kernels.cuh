@@ -36,7 +36,7 @@ constexpr int OPT_THREADS = 512;   // persistent kernel block size
 constexpr int SPMV_GROUP_BLOCKS = 192;  // blocks per row group of the TMA-fed SpMV (24 KB of Q per smem stage)
 constexpr int ND_YCAP_TILES = 600;  // sparse exact preconditioner: pose tiles of a phase's input vector staged in shared memory per step
 constexpr int ND_SLOT_CAP = 240;    // ... and partial-sum slots (8 rows x r doubles) per step
-constexpr int ND_SMEM_NEED_SMALL = 16000;   // doubles a small agent's sparse plan needs at most (occupancy query of the cluster launch)
+constexpr int OPT_SMEM_LIMIT = 227 * 1024;  // dynamic shared memory one CTA of an H100 may ask for (checked by optimize_max_grid)
 constexpr int SP_CACHE_INTS = 2048;  // shared-memory copy of a CTA's block-CSR structure (row pointers + block columns), 8 KB
 constexpr int DENSE_PER_MAX = 512;  // max rows of the dense inverse one CTA owns (smem staging of V): N <= 67k at 132 CTAs
 
@@ -45,6 +45,7 @@ struct KNd {
   int nphases;
   int max_ytiles, max_slots;       // shared-memory tiles / partial-sum slots the plan needs per step
   int max_gathers;                 // gather records staged per step (<= max_ytiles)
+  int resident_doubles;            // shared-memory region of the resident panel columns (largest over the CTAs)
   int dir[nd::MAX_PHASES];         // per phase: 0 forward (input = residual), 1 backward (input = ancestors' solution)
   int cta0[nd::MAX_PHASES];        // per phase: first (phase, CTA) record
   const nd::CtaPhase *cta_phase;
@@ -125,6 +126,8 @@ cudaError_t launch_spmv_tma(int r, int dh, int ngroups, const int2 *groups, cons
                             cudaStream_t stream);
 int spmv_group_blocks();                            // blocks per row group of the TMA-fed SpMV in use
 int optimize_max_grid(int r, int dh, int device);   // co-resident CTA count for the persistent kernel
+// bytes of resident panel columns (nd::assign_residency) a CTA may keep next to what the sparse plan stages
+int64_t nd_resident_budget(int r, int dh, const KNd &nd);
 int optimize_max_cluster(int r, int dh, int device); // largest single-cluster grid (16, 8 or 0) the kernel can be launched with
 cudaError_t launch_stiefel_project(int r, int dh, int n, const double *M, double *out, cudaStream_t stream, double c0 = 1.0,
                                    const double *B = nullptr, double c1 = 0.0, const double *C = nullptr, double c2 = 0.0);

@@ -919,10 +919,115 @@ void build_plan(const Hierarchy &H, const Options &opt, Plan &P) {
   }
 }
 
+// A step's phase time is set by its slowest warp, and a round of the job loop that streams from L2 costs an L2 round
+// trip where a resident round costs a shared-memory one.  So residency is handed out in rounds, per (CTA, phase): a level
+// L caps the rounds every warp of every step of the phase streams, the first rounds of a warp's job sequence are the
+// resident ones.  Lowering a phase's level by one saves one L2 round trip in each step that reaches it; the CTA's budget
+// goes, one level at a time, to the phase where that saving costs the fewest bytes.
+void assign_residency(Plan &P, int warps, int64_t budget_bytes) {
+  const int G = P.grid;
+  for (Job &j : P.jobs) { j.soff = 0; j.nres = 0; }
+  P.resident_doubles.assign((size_t)G, 0);
+  P.max_resident_doubles = 0;
+  P.resident_bytes = 0;
+  const int64_t budget = std::max<int64_t>(0, budget_bytes / 8);
+  const int nph = (int)P.phases.size();
+  auto nrounds = [](int ncols) { return (ncols + RES_ROUND - 1) / RES_ROUND; };
+  for (int c = 0; c < G; ++c) {
+    // per phase: the rounds (shared-memory doubles of each, in order) of every (step, warp), and the step of each
+    std::vector<std::vector<std::vector<int>>> seq((size_t)nph);
+    std::vector<std::vector<int>> seq_step((size_t)nph);
+    std::vector<int> level((size_t)nph, 0);
+    for (int ph = 0; ph < nph; ++ph) {
+      const CtaPhase &cp = P.cta_phase[(size_t)P.phases[(size_t)ph].cta0 + c];
+      for (int si = cp.s0; si < cp.s1; ++si) {
+        const Step &st = P.steps[(size_t)si];
+        for (int w = 0; w < warps && st.j0 + w < st.j1; ++w) {
+          std::vector<int> rd;
+          for (int ji = st.j0 + w; ji < st.j1; ji += warps) {
+            const int nc = P.jobs[(size_t)ji].ncols;
+            for (int k = 0; k < nrounds(nc); ++k)
+              rd.push_back(resident_doubles(std::min(nc, (k + 1) * RES_ROUND)) - resident_doubles(k * RES_ROUND));
+          }
+          level[(size_t)ph] = std::max(level[(size_t)ph], (int)rd.size());
+          seq[(size_t)ph].push_back(std::move(rd));
+          seq_step[(size_t)ph].push_back(si);
+        }
+      }
+    }
+    int64_t used = 0;
+    while (true) {
+      int best = -1;
+      int64_t best_cost = 0;
+      double best_score = 0.0;
+      for (int ph = 0; ph < nph; ++ph) {
+        const int L = level[(size_t)ph];
+        if (L == 0) continue;
+        int64_t cost = 0;
+        std::vector<int> steps_hit;
+        for (size_t q = 0; q < seq[(size_t)ph].size(); ++q) {
+          const std::vector<int> &rd = seq[(size_t)ph][q];
+          if ((int)rd.size() < L) continue;
+          cost += rd[rd.size() - (size_t)L];
+          steps_hit.push_back(seq_step[(size_t)ph][q]);
+        }
+        if (used + cost > budget) continue;
+        std::sort(steps_hit.begin(), steps_hit.end());
+        const double saved = (double)(std::unique(steps_hit.begin(), steps_hit.end()) - steps_hit.begin());
+        const double score = (double)cost / saved;
+        if (best < 0 || score < best_score) { best = ph; best_cost = cost; best_score = score; }
+      }
+      if (best < 0) break;
+      --level[(size_t)best];
+      used += best_cost;
+    }
+    // the region: the resident rounds of every (phase, step, warp) in job order, one after the other
+    int off = 0;
+    for (int ph = 0; ph < nph; ++ph) {
+      const CtaPhase &cp = P.cta_phase[(size_t)P.phases[(size_t)ph].cta0 + c];
+      for (int si = cp.s0; si < cp.s1; ++si) {
+        const Step &st = P.steps[(size_t)si];
+        for (int w = 0; w < warps && st.j0 + w < st.j1; ++w) {
+          int total = 0;
+          for (int ji = st.j0 + w; ji < st.j1; ji += warps) total += nrounds(P.jobs[(size_t)ji].ncols);
+          int left = std::max(0, total - level[(size_t)ph]);
+          for (int ji = st.j0 + w; ji < st.j1 && left > 0; ji += warps) {
+            Job &jb = P.jobs[(size_t)ji];
+            const int take = std::min(left, nrounds(jb.ncols));
+            left -= take;
+            jb.nres = std::min(jb.ncols, take * RES_ROUND);
+            jb.soff = off;
+            off += resident_doubles(jb.nres);
+            P.resident_bytes += (int64_t)jb.nres * PANEL_ROWS * 8;
+          }
+        }
+      }
+    }
+    if (off > budget) throw std::runtime_error("nd: resident region exceeds its budget");
+    P.resident_doubles[(size_t)c] = off;
+    P.max_resident_doubles = std::max(P.max_resident_doubles, off);
+  }
+}
+
 // =================================================================================================================
 // host emulation of the plan (verification only)
 // =================================================================================================================
+static void emulate_pass(const Hierarchy &H, const Plan &P, const std::vector<double> &blob, int r, const double *V, double *Z,
+                         std::vector<std::vector<double>> &region, bool fill);
+
 void emulate_apply(const Hierarchy &H, const Plan &P, const std::vector<double> &blob, int r, const double *V, double *Z) {
+  const bool resident = P.resident_bytes > 0;
+  std::vector<std::vector<double>> region((size_t)P.grid);
+  for (int c = 0; c < P.grid && resident; ++c) region[(size_t)c].assign((size_t)P.resident_doubles[(size_t)c], std::nan(""));
+  std::vector<double> Zfill;
+  if (resident) Zfill.assign((size_t)r * H.dh * H.n, 0.0);
+  for (int pass = resident ? 0 : 1; pass < 2; ++pass)
+    emulate_pass(H, P, blob, r, V, pass == 0 ? Zfill.data() : Z, region, resident && pass == 0);
+}
+
+// one application; fill: resident columns are read from the panels and copied to the region, else read from the region
+static void emulate_pass(const Hierarchy &H, const Plan &P, const std::vector<double> &blob, int r, const double *V, double *Z,
+                         std::vector<std::vector<double>> &region, bool fill) {
   const int dh = H.dh, ts = r * dh;
   std::vector<double> TX((size_t)H.n * ts, 0.0), C((size_t)H.cbuf_tiles * ts, 0.0);
   std::vector<double> ys((size_t)std::max(P.max_ytiles, 1) * ts), slots((size_t)std::max(P.max_slots, 1) * PANEL_ROWS * r);
@@ -955,10 +1060,20 @@ void emulate_apply(const Hierarchy &H, const Plan &P, const std::vector<double> 
           const Job &jb = P.jobs[(size_t)ji];
           const double *mat = blob.data() + jb.mat;
           double *sl = slots.data() + (size_t)jb.slot * PANEL_ROWS * r;
+          // column j of a resident piece: group j / 4, lane 4 row + j % 4 (dpgo_kernels.cu phase_nd)
+          auto rslot = [&](int j, int row) -> double & {
+            return region[(size_t)c].at((size_t)jb.soff + (size_t)(j / 4) * 32 + (size_t)(row * 4 + (j & 3)));
+          };
+          if (fill)
+            for (int j = 0; j < jb.nres; ++j)
+              for (int row = 0; row < PANEL_ROWS; ++row) rslot(j, row) = mat[(size_t)j * PANEL_ROWS + row];
           for (int row = 0; row < PANEL_ROWS; ++row)
             for (int a = 0; a < r; ++a) {
               double acc = 0.0;
-              for (int j = 0; j < jb.ncols; ++j) acc += mat[(size_t)j * PANEL_ROWS + row] * ys[(size_t)(jb.ycol + j) * r + a];
+              for (int j = 0; j < jb.ncols; ++j) {
+                const double m = (j < jb.nres && !fill) ? rslot(j, row) : mat[(size_t)j * PANEL_ROWS + row];
+                acc += m * ys[(size_t)(jb.ycol + j) * r + a];
+              }
               if (jb.accum) sl[row * r + a] += acc; else sl[row * r + a] = acc;
             }
         }
@@ -998,7 +1113,9 @@ std::string describe(const Hierarchy &H, const Plan &P) {
   for (size_t k = 0; k < H.cuts.size(); ++k) os << (k ? "," : "") << H.cuts[k];
   os << "] stages=" << H.nstages << " nodes=" << H.nodes.size() << " blob=" << (H.blob_doubles * 8) / 1e6 << "MB phases=" << P.phases.size()
      << " bytes/apply=" << P.bytes_per_apply / 1e6 << "MB steps=" << P.steps.size() << " jobs=" << P.jobs.size() << " epis=" << P.epis.size()
-     << " max_ytiles=" << P.max_ytiles << " max_slots=" << P.max_slots;
+     << " max_ytiles=" << P.max_ytiles << " max_slots=" << P.max_slots
+     << " resident=" << (P.bytes_per_apply > 0 ? (double)P.resident_bytes / (double)P.bytes_per_apply : 0.0)
+     << " max_resident_KB=" << P.max_resident_doubles * 8 / 1024.0;
   for (int st = 0; st < H.nstages; ++st) {
     int cnt = 0, smax = 0, bmax = 0;
     for (const MacroNode &m : H.nodes)

@@ -34,13 +34,19 @@ struct Step { int g0, g1, j0, j1, e0, e1, pad0, pad1; };              // ranges 
 struct CtaPhase { int s0, s1; int g0, g1, j0, j1, e0, e1; };          // steps [s0, s1) of one CTA in one phase + step s0 inline
 constexpr int INLINE_CONTRIB = 4;
 struct Gather { int ytile; int src; int nc; int cext; int ci[INLINE_CONTRIB]; };   // smem tile <- source tile - sum of nc contribution tiles
-struct Job { long long mat; int ncols; int ycol; int slot; int accum; int pad0, pad1; };   // one warp: panel piece x y
+// one warp: panel piece x y.  The first nres columns (0, a multiple of RES_ROUND, or all ncols) are resident: the first
+// application of a launch copies them to the CTA's shared-memory region at double offset soff, later ones read them there
+// (groups of 4 columns x 8 rows, 32 doubles each, in lane order: lane 4 row + k holds column 4 g + k)
+struct Job { long long mat; int ncols; int ycol; int slot; int accum; int soff, nres; };
 struct Epi { int kind; int slot0; int nslots; int half; int out; int aux; int nc; int cext; int ci[INLINE_CONTRIB]; };   // one pose (dh rows of a panel)
 enum EpiKind { EPI_F_OWN = 0, EPI_F_BND = 1, EPI_B_OWN = 2, EPI_ROOT = 3 };
 struct Phase { int dir; int stage; int cta0; int pad; };              // dir 0 forward (source = V, pose ids), 1 backward (source = TX); cta0 = first CtaPhase record
 constexpr int MAX_PHASES = 16;
 
 constexpr int PANEL_ROWS = 8;
+constexpr int RES_ROUND = 32;     // columns per round of the job loop (8 independent loads of 4 columns)
+// shared-memory doubles of a job's resident columns
+inline int resident_doubles(int nres) { return (nres + 3) / 4 * 32; }
 
 struct Options {
   int grid = 132;            // CTAs of the persistent kernel (one per SM of an H100 SXM)
@@ -92,6 +98,9 @@ struct Plan {
   int grid = 0, r = 0;
   int max_ytiles = 0, max_slots = 0;
   int64_t bytes_per_apply = 0;     // matrix bytes streamed by one application (all phases)
+  std::vector<int> resident_doubles;   // per CTA: shared-memory region of its resident columns (assign_residency)
+  int max_resident_doubles = 0;
+  int64_t resident_bytes = 0;      // matrix bytes of one application read from shared memory after the first
 };
 
 // block-CSR input: rowptr[n+1], bcol[nb], bval[nb*16] with bval[b][k][c] = Q[dh*bcol[b]+k, dh*j+c] for b in row j
@@ -110,8 +119,13 @@ void build_numeric(const BsrView &Q, const Options &opt, Hierarchy &H, std::vect
                    int big_threshold = 1 << 30);
 // 3. static work plan of every phase
 void build_plan(const Hierarchy &H, const Options &opt, Plan &P);
+// 4. residency: annotates the jobs (soff, nres) so that every CTA keeps at most budget_bytes of its panels in shared
+//    memory for the whole launch.  Only an annotation: the jobs, their order and their arithmetic stay as they are.
+//    Within a (CTA, phase) every warp streams the same number of rounds per step (or all of its own, if fewer).
+void assign_residency(Plan &P, int warps, int64_t budget_bytes);
 // host emulation of the plan exactly as the kernel interprets it (verification only; never on a product path):
-// V, Z are r x (dh n) column-major (pose tiles), Z = (Q + shift I)^-1 V   (no tangent projection)
+// V, Z are r x (dh n) column-major (pose tiles), Z = (Q + shift I)^-1 V   (no tangent projection).  With resident
+// columns, a first pass fills a simulated per-CTA region and the result is that of a second pass reading from it.
 void emulate_apply(const Hierarchy &H, const Plan &P, const std::vector<double> &blob, int r, const double *V, double *Z);
 
 std::string describe(const Hierarchy &H, const Plan &P);

@@ -288,8 +288,11 @@ class QuadraticProblem:
         info = (C.c_int64 * 16)()
         capi.check(self._lib.dpgo_nd_info(self._h, info))
         keys = ("levels", "nodes", "phases", "block_bytes", "bytes_per_apply", "max_own", "max_bnd", "nd_depth", "steps",
-                "jobs", "epilogues", "max_ytiles", "max_slots")
-        return {k: int(info[i]) for i, k in enumerate(keys)}
+                "jobs", "epilogues", "max_ytiles", "max_slots", "resident_bytes", "max_resident_bytes_per_cta")
+        out = {k: int(info[i]) for i, k in enumerate(keys)}
+        # share of the panel bytes of an application read from shared memory (every application of a launch but the first)
+        out["resident_fraction"] = out["resident_bytes"] / max(out["bytes_per_apply"], 1)
+        return out
 
     def precond_algorithmic_bytes(self, preconditioner: int) -> int:
         return int(self._lib.dpgo_precond_algorithmic_bytes(self._h, int(preconditioner)))
