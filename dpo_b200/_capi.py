@@ -67,6 +67,10 @@ SIGNATURES = {
     "dpgo_problem_set_edges": (C.c_int, [_vp, C.c_int64, _ip, _ip, _dp, _dp, _dp, _dp, _dp, _ip, C.c_int64, _ip, _dp, C.c_uint]),
     "dpgo_problem_robust_reweight": (C.c_int, [_vp, C.c_int, C.c_double, C.c_double, _dp, _dp]),
     "dpgo_problem_set_edge_weights": (C.c_int, [_vp, _dp]),
+    "dpgo_problem_set_edge_weights_async": (C.c_int, [_vp, _vp]),
+    "dpgo_problem_robust_reweight_async": (C.c_int, [_vp, C.c_int, C.c_double, C.c_double]),
+    "dpgo_problem_device_edge_weights": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_vp)]),
+    "dpgo_problem_gnc_counts": (C.c_int, [_vp, C.POINTER(C.c_int64)]),
     "dpgo_problem_set_G_dense": (C.c_int, [_vp, _dp]),
     "dpgo_problem_set_G_csr": (C.c_int, [_vp, _ip, _ip, _dp]),
     "dpgo_problem_f": (C.c_int, [_vp, _dp, _dp]),
@@ -95,6 +99,7 @@ SIGNATURES = {
     "dpgo_sym_plan_sizes": (C.c_int, [C.c_int, _ip, _ip]),
     "dpgo_sym_plan": (C.c_int, [C.c_int, C.c_int, C.c_double, _ip, _ip, _ip, _ip, C.POINTER(C.c_int64)]),
     "dpgo_nd_info": (C.c_int, [_vp, C.POINTER(C.c_int64)]),
+    "dpgo_nd_node_sizes": (C.c_int, [_vp, C.c_int64, _ip, _ip, _ip, C.POINTER(C.c_int64)]),
     "dpgo_nd_debug_emulate": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int64, _ip, _ip, _dp, C.c_double, C.c_int, C.c_int,
                                         C.c_int, _dp, _dp, C.POINTER(C.c_int64)]),
     "dpgo_debug_phase_latency": (C.c_int, [_vp, C.c_int, _dp, _dp]),

@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdpgo_b200.so")
 SOURCES = ["dpgo_kernels.cu", "dpgo_spmv_tma.cu", "dense_inverse.cu", "dpgo_capi.cu", "dpgo_chordal.cu", "dpgo_align.cu",
-           "dpgo_status.cu", "dpgo_accel.cu", "dpgo_select.cu"]
+           "dpgo_status.cu", "dpgo_accel.cu", "dpgo_select.cu", "nd_refactor.cu"]
 HOST_ONLY_SOURCES = ["nd_precond.cpp"]          # host planning code inside libdpgo_b200.so (g++, OpenMP)
 HEADERS = ["dpgo_device.cuh", "dpgo_devbuf.cuh", "dpgo_kernels.cuh", "dpgo_rotation.cuh", "nd_precond.h", os.path.join("..", "..", "include", "dpgo_b200.h")]
 HOST_ONLY_FLAGS = ["-O3", "-std=c++17", "-fPIC", "-fvisibility=hidden", "-fopenmp", "-mavx2", "-mfma", "-Wall"]

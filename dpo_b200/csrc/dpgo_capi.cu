@@ -70,6 +70,7 @@ struct dpgo_problem {
     DevBuf<double> bval, dinv, partials;
     std::vector<int> h_rowptr, h_bcol;
     std::vector<double> h_bval;
+    bool h_stale = false;        // an asynchronous re-weight changed bval on the device only (sync_host_bval)
   } bsr;
   // the dense exact preconditioner (ensure_dense); dropped whenever Q changes
   struct Dense {
@@ -92,6 +93,13 @@ struct dpgo_problem {
     DevBuf<double> blob, TX, C;
     std::unique_ptr<dpgo::nd::Hierarchy> H;
     int64_t info[16] = {};
+    // device refactorisation of the blob (ensure_refactor): scatter maps, fronts, sweep workspace and jobs of H
+    std::unique_ptr<dpgo::nd::Refactor> R;
+    DevBuf<dpgo::nd::RefactorNode> rnodes;
+    DevBuf<dpgo::nd::RefactorChild> rchild;
+    DevBuf<int> rposes, rcmap;
+    DevBuf<double> arena, ws;
+    DevBuf<dpgo::GjJob> rjobs;
   } nd;
   // edge records for the device-side Q assembly / robust re-weighting (dpgo_problem_set_edges)
   struct Edges {
@@ -99,6 +107,9 @@ struct dpgo_problem {
     DevBuf<int> p1, p2, fixed, cptr;
     DevBuf<int2> contrib;
     DevBuf<double> T, om, w, sblk, res;
+    DevBuf<unsigned long long> gnc;   // GNC counts of the last re-weight: weight 1, 0, in between (non-fixed edges)
+    DevBuf<int> fail;                 // set by a device refactorisation whose matrix was not positive definite
+    bool fail_armed = false;          // an asynchronous re-weight ran since the flag was last read
   } edges;
   // vectors
   DevBuf<double> G, vec[dpgo::V_COUNT], S[2];
@@ -375,6 +386,17 @@ void free_nd(dpgo_problem *p) {
   p->nd = {};
 }
 
+// The host copy of Q's values after an asynchronous re-weight changed them on the device only: downloaded before any
+// host-side use (synchronises).
+int sync_host_bval(dpgo_problem *p) {
+  if (!p->bsr.h_stale) return DPGO_OK;
+  DPGO_CUDA(cudaMemcpyAsync(p->bsr.h_bval.data(), p->bsr.bval.get(), sizeof(double) * 16 * (size_t)p->bsr.nb,
+                            cudaMemcpyDeviceToHost, p->stream));
+  DPGO_CUDA(cudaStreamSynchronize(p->stream));
+  p->bsr.h_stale = false;
+  return DPGO_OK;
+}
+
 // The nested-dissection block factorisation of Q + 0.1 I is built on first use (host: ordering, symbolic, plan; the
 // dense algebra of large blocks on the device), like the dense inverse.
 int ensure_nd(dpgo_problem *p) {
@@ -383,6 +405,7 @@ int ensure_nd(dpgo_problem *p) {
     return fail(DPGO_ERR_STATE, "sparse exact preconditioner was not requested in set_Q (precond_mask)");
   namespace nd = dpgo::nd;
   free_nd(p);
+  DPGO_TRY(sync_host_bval(p));
   nd::Plan plan;
   std::vector<double> blob;
   auto H = std::make_unique<nd::Hierarchy>();
@@ -625,10 +648,23 @@ int download_vec(dpgo_problem *p, int id, double *host) {
   DPGO_CUDA(cudaMemcpyAsync(host, p->vec[id].get(), p->vec_bytes(), cudaMemcpyDeviceToHost, p->stream));
   return DPGO_OK;
 }
+// After the stream has been synchronised: report (once) a device refactorisation that met a matrix that was not positive
+// definite.  Only read when an asynchronous re-weight ran since the last read.
+int check_refactor_fail(dpgo_problem *p) {
+  dpgo_problem::Edges &E = p->edges;
+  if (!E.fail_armed) return DPGO_OK;
+  E.fail_armed = false;
+  int flag = 0;
+  DPGO_CUDA(cudaMemcpy(&flag, E.fail.get(), sizeof(int), cudaMemcpyDeviceToHost));
+  if (!flag) return DPGO_OK;
+  DPGO_CUDA(cudaMemset(E.fail.get(), 0, sizeof(int)));
+  return fail(DPGO_ERR_CUDA, "device refactorisation: Q + 0.1 I is not positive definite (negative edge weight?)");
+}
+
 int fetch_result(dpgo_problem *p) {
   DPGO_CUDA(cudaMemcpyAsync(p->h_result.get(), p->result.get(), sizeof(dpgo_opt_result_t), cudaMemcpyDeviceToHost, p->stream));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
-  return DPGO_OK;
+  return check_refactor_fail(p);
 }
 
 #define DPGO_CHECK_HANDLE(p)                                                         \
@@ -752,7 +788,7 @@ int dpgo_problem_set_stream(dpgo_problem_t *p, void *cuda_stream) {
 int dpgo_problem_sync(dpgo_problem_t *p) {
   DPGO_CHECK_HANDLE(p);
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
-  return DPGO_OK;
+  return check_refactor_fail(p);
 }
 
 int dpgo_problem_set_launch_mode(dpgo_problem_t *p, int mode) {
@@ -1263,6 +1299,15 @@ int dpgo_nd_debug_emulate(int n, int d, int r, int64_t nb, const int32_t *brow, 
 }
 
 // ---- Q from edge records on the device, robust re-weighting -----------------------------------------------------
+// weights (and the GNC counts) of the non-fixed edges at the resident iterate
+static int launch_reweight(dpgo_problem *p, int cost, double mu, double param) {
+  const dpgo_problem::Edges &E = p->edges;
+  DPGO_CUDA(cudaMemsetAsync(E.gnc.get(), 0, 3 * sizeof(unsigned long long), p->stream));
+  DPGO_CUDA(dpgo::launch_edge_weights(p->r, p->dh, E.ne, E.p1.get(), E.p2.get(), E.T.get(), E.om.get(), E.fixed.get(),
+                                      p->vec[dpgo::V_X0].get(), cost, mu, param, E.w.get(), E.res.get(), E.gnc.get(), p->stream));
+  return DPGO_OK;
+}
+
 static int reassemble_Q(dpgo_problem *p) {
   const dpgo_problem::Edges &E = p->edges;
   DPGO_CUDA(dpgo::launch_assemble_Q(p->bsr.nb, E.cptr.get(), E.contrib.get(), E.T.get(), E.om.get(), E.w.get(), E.sblk.get(),
@@ -1271,6 +1316,7 @@ static int reassemble_Q(dpgo_problem *p) {
   DPGO_CUDA(cudaMemcpyAsync(p->bsr.h_bval.data(), p->bsr.bval.get(), sizeof(double) * 16 * (size_t)p->bsr.nb,
                             cudaMemcpyDeviceToHost, p->stream));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
+  p->bsr.h_stale = false;
   if (p->bsr.dinv) {
     std::vector<double> dinv;
     jacobi_blocks(p->n, p->dh, p->bsr.h_rowptr, p->bsr.h_bcol, p->bsr.h_bval, dinv);
@@ -1356,6 +1402,10 @@ int dpgo_problem_set_edges(dpgo_problem_t *p, int64_t m, const int32_t *p1, cons
   DPGO_CUDA(E.w.assign(ew.data(), ew.size(), p->stream));
   DPGO_CUDA(E.sblk.assign(sb.data(), sb.size(), p->stream));
   DPGO_CUDA(E.res.alloc((size_t)m));
+  DPGO_CUDA(E.gnc.alloc(3));
+  DPGO_CUDA(cudaMemsetAsync(E.gnc.get(), 0, 3 * sizeof(unsigned long long), p->stream));
+  DPGO_CUDA(E.fail.alloc(1));
+  DPGO_CUDA(cudaMemsetAsync(E.fail.get(), 0, sizeof(int), p->stream));
   return reassemble_Q(p);
 }
 
@@ -1372,14 +1422,146 @@ int dpgo_problem_robust_reweight(dpgo_problem_t *p, int cost, double mu, double 
   DPGO_REQUIRE(p->edges.cptr, DPGO_ERR_STATE, "dpgo_problem_set_edges has not been called");
   DPGO_REQUIRE(cost >= 0 && cost <= 5, DPGO_ERR_INVALID_ARG, "unknown robust cost");
   DPGO_REQUIRE(cost != 5 || mu > 0, DPGO_ERR_INVALID_ARG, "GNC needs mu > 0");
+  DPGO_TRY(launch_reweight(p, cost, mu, param));
   const dpgo_problem::Edges &E = p->edges;
-  DPGO_CUDA(dpgo::launch_edge_weights(p->r, p->dh, E.ne, E.p1.get(), E.p2.get(), E.T.get(), E.om.get(), E.fixed.get(),
-                                      p->vec[dpgo::V_X0].get(), cost, mu, param, E.w.get(), E.res.get(), p->stream));
   if (weights_host && E.ne)
     DPGO_CUDA(cudaMemcpyAsync(weights_host, E.w.get(), sizeof(double) * (size_t)E.ne, cudaMemcpyDeviceToHost, p->stream));
   if (residuals2_host && E.ne)
     DPGO_CUDA(cudaMemcpyAsync(residuals2_host, E.res.get(), sizeof(double) * (size_t)E.ne, cudaMemcpyDeviceToHost, p->stream));
   return reassemble_Q(p);
+}
+
+// ---- stream-ordered re-weighting: the preconditioners are refactorised on the device --------------------------------
+// The sparse exact preconditioner's device refactorisation: scatter maps, fronts and sweep jobs of its hierarchy, built
+// once per hierarchy on the host (synchronises).
+static int ensure_refactor(dpgo_problem *p) {
+  namespace nd = dpgo::nd;
+  dpgo_problem::Nd &F = p->nd;
+  if (F.R) return DPGO_OK;
+  auto R = std::make_unique<nd::Refactor>();
+  try {
+    nd::build_refactor(*F.H, *R);
+  } catch (const std::exception &e) {
+    return fail(DPGO_ERR_UNSUPPORTED, std::string("sparse exact preconditioner refactorisation: ") + e.what());
+  }
+  for (size_t st = 0; st + 1 < R->stage0.size(); ++st)
+    if (R->stage0[st + 1] - R->stage0[st] > 65535)
+      return fail(DPGO_ERR_UNSUPPORTED, "sparse exact preconditioner refactorisation: more than 65535 nodes in one stage");
+  if (R->child.empty()) R->child.push_back({0, 0});        // one macro level: no children, nothing reads these
+  if (R->cmap.empty()) R->cmap.push_back(-1);
+  DPGO_CUDA(F.rnodes.assign(R->nodes.data(), R->nodes.size(), p->stream));
+  DPGO_CUDA(F.rchild.assign(R->child.data(), R->child.size(), p->stream));
+  DPGO_CUDA(F.rposes.assign(R->poses.data(), R->poses.size(), p->stream));
+  DPGO_CUDA(F.rcmap.assign(R->cmap.data(), R->cmap.size(), p->stream));
+  DPGO_CUDA(F.arena.alloc((size_t)R->arena_doubles));
+  DPGO_CUDA(F.ws.alloc((size_t)R->ws_doubles));
+  std::vector<dpgo::GjJob> jobs(R->nodes.size());
+  constexpr int B = nd::REFACTOR_PIVOT_BLOCK;
+  for (size_t q = 0; q < jobs.size(); ++q) {
+    const nd::RefactorNode &rn = R->nodes[q];
+    const int M = p->dh * (rn.no + rn.nb);
+    double *w = F.ws.get() + rn.ws;
+    jobs[q] = {F.arena.get() + rn.front, w, w + B * B, w + B * B + (size_t)B * M, M, p->dh * rn.no};
+  }
+  DPGO_CUDA(F.rjobs.assign(jobs.data(), jobs.size(), p->stream));
+  DPGO_CUDA(cudaStreamSynchronize(p->stream));
+  F.R = std::move(R);
+  return DPGO_OK;
+}
+
+// After k_assemble_Q on the stream: block-Jacobi and the sparse exact preconditioner refactorised on the device, the dense
+// inverse dropped (rebuilt synchronously on its next use).  Only the first call after the sparse exact structure was
+// dropped (or never built) runs host work and synchronises.
+static int refresh_preconditioners_async(dpgo_problem *p) {
+  p->bsr.h_stale = true;
+  if (p->dense.pinv) {                                  // its buffers go: a round captured with them must be re-captured
+    p->dense = {};
+    ++p->generation;
+  }
+  dpgo_problem::Edges &E = p->edges;
+  E.fail_armed = true;
+  if (p->bsr.dinv)
+    DPGO_CUDA(dpgo::launch_jacobi_blocks(p->n, p->dh, p->bsr.rowptr.get(), p->bsr.bcol.get(), p->bsr.bval.get(), 0.1,
+                                         p->bsr.dinv.get(), E.fail.get(), p->stream));
+  if (!(p->bsr.precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT))) return DPGO_OK;
+  DPGO_TRY(ensure_nd(p));
+  DPGO_TRY(ensure_refactor(p));
+  dpgo_problem::Nd &F = p->nd;
+  dpgo::KRefactor k;
+  k.dh = p->dh;
+  k.shift = 0.1;
+  k.nodes = F.rnodes.get();
+  k.child = F.rchild.get();
+  k.poses = F.rposes.get();
+  k.cmap = F.rcmap.get();
+  k.rowptr = p->bsr.rowptr.get();
+  k.bcol = p->bsr.bcol.get();
+  k.bval = p->bsr.bval.get();
+  k.arena = F.arena.get();
+  k.jobs = F.rjobs.get();
+  k.blob = F.blob.get();
+  k.fail = E.fail.get();
+  DPGO_CUDA(dpgo::launch_nd_refactor(k, *F.R, p->stream));
+  return DPGO_OK;
+}
+
+int dpgo_problem_set_edge_weights_async(dpgo_problem_t *p, const double *weights_dev) {
+  DPGO_CHECK_HANDLE(p);
+  DPGO_REQUIRE(weights_dev || p->edges.ne == 0, DPGO_ERR_INVALID_ARG, "null weights");
+  DPGO_REQUIRE(p->edges.cptr, DPGO_ERR_STATE, "dpgo_problem_set_edges has not been called");
+  const dpgo_problem::Edges &E = p->edges;
+  if (E.ne)
+    DPGO_CUDA(cudaMemcpyAsync(E.w.get(), weights_dev, sizeof(double) * (size_t)E.ne, cudaMemcpyDeviceToDevice, p->stream));
+  DPGO_CUDA(dpgo::launch_assemble_Q(p->bsr.nb, E.cptr.get(), E.contrib.get(), E.T.get(), E.om.get(), E.w.get(), E.sblk.get(),
+                                    p->bsr.bval.get(), p->stream));
+  return refresh_preconditioners_async(p);
+}
+
+int dpgo_problem_robust_reweight_async(dpgo_problem_t *p, int cost, double mu, double param) {
+  DPGO_CHECK_HANDLE(p);
+  DPGO_REQUIRE(p->edges.cptr, DPGO_ERR_STATE, "dpgo_problem_set_edges has not been called");
+  DPGO_REQUIRE(cost >= 0 && cost <= 5, DPGO_ERR_INVALID_ARG, "unknown robust cost");
+  DPGO_REQUIRE(cost != 5 || mu > 0, DPGO_ERR_INVALID_ARG, "GNC needs mu > 0");
+  DPGO_TRY(launch_reweight(p, cost, mu, param));
+  const dpgo_problem::Edges &E = p->edges;
+  DPGO_CUDA(dpgo::launch_assemble_Q(p->bsr.nb, E.cptr.get(), E.contrib.get(), E.T.get(), E.om.get(), E.w.get(), E.sblk.get(),
+                                    p->bsr.bval.get(), p->stream));
+  return refresh_preconditioners_async(p);
+}
+
+int dpgo_problem_device_edge_weights(dpgo_problem_t *p, double **w_dev, double **res2_dev) {
+  DPGO_REQUIRE(p && w_dev && res2_dev, DPGO_ERR_INVALID_ARG, "null argument");
+  DPGO_REQUIRE(p->edges.cptr, DPGO_ERR_STATE, "dpgo_problem_set_edges has not been called");
+  *w_dev = p->edges.w.get();
+  *res2_dev = p->edges.res.get();
+  return DPGO_OK;
+}
+
+int dpgo_problem_gnc_counts(dpgo_problem_t *p, int64_t *out3) {
+  DPGO_CHECK_HANDLE(p);
+  DPGO_REQUIRE(out3, DPGO_ERR_INVALID_ARG, "null argument");
+  DPGO_REQUIRE(p->edges.cptr, DPGO_ERR_STATE, "dpgo_problem_set_edges has not been called");
+  unsigned long long c[3] = {0, 0, 0};
+  DPGO_CUDA(cudaMemcpyAsync(c, p->edges.gnc.get(), sizeof(c), cudaMemcpyDeviceToHost, p->stream));
+  DPGO_CUDA(cudaStreamSynchronize(p->stream));
+  DPGO_TRY(check_refactor_fail(p));
+  for (int q = 0; q < 3; ++q) out3[q] = (int64_t)c[q];
+  return DPGO_OK;
+}
+
+int dpgo_nd_node_sizes(dpgo_problem_t *p, int64_t cap, int32_t *own, int32_t *bnd, int32_t *stage, int64_t *count) {
+  DPGO_CHECK_HANDLE(p);
+  DPGO_REQUIRE(count && cap >= 0 && (cap == 0 || (own && bnd && stage)), DPGO_ERR_INVALID_ARG, "null argument");
+  DPGO_REQUIRE(p->bsr.have, DPGO_ERR_STATE, "set_Q has not been called");
+  DPGO_TRY(ensure_nd(p));
+  const auto &nodes = p->nd.H->nodes;
+  *count = (int64_t)nodes.size();
+  for (size_t q = 0; q < nodes.size() && (int64_t)q < cap; ++q) {
+    own[q] = (int32_t)nodes[q].own.size();
+    bnd[q] = (int32_t)nodes[q].bnd.size();
+    stage[q] = nodes[q].stage;
+  }
+  return DPGO_OK;
 }
 
 // ---- plain device helpers ----------------------------------------------------------------------

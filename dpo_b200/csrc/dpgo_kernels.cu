@@ -1478,7 +1478,8 @@ __global__ void k_assemble_Q(int64_t nb, const int *__restrict__ cptr, const int
 template <int R, int DH>
 __global__ void k_edge_weights(int64_t m, const int *__restrict__ p1, const int *__restrict__ p2, const double *__restrict__ eT,
                                const double *__restrict__ eom, const int *__restrict__ fixed, const double *__restrict__ X, int cost,
-                               double mu, double param, double *__restrict__ w, double *__restrict__ resid) {
+                               double mu, double param, double *__restrict__ w, double *__restrict__ resid,
+                               unsigned long long *__restrict__ gnc) {
   constexpr int D = DH - 1, TS = R * DH;
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= m) return;
@@ -1506,6 +1507,8 @@ __global__ void k_edge_weights(int64_t m, const int *__restrict__ p1, const int 
   else if (cost == 4) { const double s = 1.0 + r2; wt = 1.0 / (s * s); }
   else if (cost == 5) wt = gnc_tls_weight(r2, mu, param);
   w[e] = wt;
+  // the counts of the reference's computeConvergedLoopClosureRatio (src/PGOAgent.cpp:1247-1289); integers, so deterministic
+  if (gnc) atomicAdd(gnc + (wt == 1.0 ? 0 : (wt == 0.0 ? 1 : 2)), 1ULL);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1771,11 +1774,12 @@ cudaError_t launch_assemble_Q(int64_t nb, const int *cptr, const int2 *contrib, 
 
 cudaError_t launch_edge_weights(int r, int dh, int64_t m, const int *p1, const int *p2, const double *eT, const double *eom,
                                 const int *fixed, const double *X, int cost, double mu, double param, double *w, double *resid,
-                                cudaStream_t stream) {
+                                unsigned long long *gnc, cudaStream_t stream) {
   if (m <= 0) return cudaSuccess;
   bool ok = false;
   DPGO_DISPATCH(r, dh, {
-    k_edge_weights<R, DH><<<(unsigned)((m + 127) / 128), 128, 0, stream>>>(m, p1, p2, eT, eom, fixed, X, cost, mu, param, w, resid);
+    k_edge_weights<R, DH><<<(unsigned)((m + 127) / 128), 128, 0, stream>>>(m, p1, p2, eT, eom, fixed, X, cost, mu, param, w, resid,
+                                                                            gnc);
     ok = true;
   });
   if (!ok) return cudaErrorInvalidValue;

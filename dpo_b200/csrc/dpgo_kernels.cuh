@@ -139,9 +139,10 @@ cudaError_t launch_build_G(int r, int dh, int nposes, const int *pose_ids, const
                            double *G, cudaStream_t stream, const unsigned char *gate = nullptr);
 cudaError_t launch_assemble_Q(int64_t nb, const int *cptr, const int2 *contrib, const double *eT, const double *eom, const double *ew,
                               const double *sblk, double *bval, cudaStream_t stream);
+// gnc (nullable, zeroed by the caller): counts over the non-fixed edges of weight exactly 1, exactly 0, and in between
 cudaError_t launch_edge_weights(int r, int dh, int64_t m, const int *p1, const int *p2, const double *eT, const double *eom,
                                 const int *fixed, const double *X, int cost, double mu, double param, double *w, double *resid,
-                                cudaStream_t stream);
+                                unsigned long long *gnc, cudaStream_t stream);
 cudaError_t launch_pack_sym(const double *pinv, int N, int nchunks, const int *segptr, int nseg, const long long *off, double *ppack,
                             cudaStream_t stream);
 cudaError_t launch_bsr_to_dense(int n, int dh, int64_t nb, const int *rowptr, const int *bcol, const double *bval,
@@ -149,6 +150,38 @@ cudaError_t launch_bsr_to_dense(int n, int dh, int64_t nb, const int *rowptr, co
 
 // dense SPD inverse in place (dense_inverse.cu); A is N x N, ld = N, symmetric positive definite
 cudaError_t dense_spd_inverse(double *A, int N, cudaStream_t stream);
+// One matrix of a batched Gauss-Jordan sweep (dense_inverse.cu): A is M x M column-major (ld = M), swept over its pivots
+// [0, s); piv (32 x 32), Rw (32 x M) and C (M x 32) are its workspace.
+struct GjJob {
+  double *A, *piv, *Rw, *C;
+  int M, s;
+};
+// Sweeps every job of jobs_dev (njobs <= 65535; max_M / max_s bound the jobs' sizes): 3 launches per 32 pivots, no
+// synchronisation.  A non-positive pivot sets *fail (nullable).
+cudaError_t gj_sweep_batch(const GjJob *jobs_dev, int njobs, int max_M, int max_s, int *fail, cudaStream_t stream);
+
+// ---- numeric refactorisation of the sparse exact preconditioner on the device (nd_refactor.cu) ----
+// Device view of an nd::Refactor plus the buffers it fills; see nd_precond.h.
+struct KRefactor {
+  int dh;
+  double shift;
+  const nd::RefactorNode *nodes;
+  const nd::RefactorChild *child;
+  const int *poses, *cmap;
+  const int *rowptr, *bcol;          // block-CSR pattern of Q
+  const double *bval;                // Q values
+  double *arena;                     // fronts (nd::Refactor::arena_doubles)
+  const GjJob *jobs;                 // one sweep job per node, nodes order
+  double *blob;                      // the panel blob, rewritten in place
+  int *fail;                         // set when a front is not positive definite
+};
+// Every stage of R (deepest first): assemble the fronts, sweep them, pack the panels.  Ordinary launches on `stream`, none
+// synchronising; the sequence captures into a CUDA graph.
+cudaError_t launch_nd_refactor(const KRefactor &k, const nd::Refactor &R, cudaStream_t stream);
+// block-Jacobi inverse blocks (Q_jj + shift I)^-1 of every pose, 4x4 padded (the host's jacobi_blocks in dpgo_capi.cu);
+// a non-positive pivot sets *fail (nullable)
+cudaError_t launch_jacobi_blocks(int n, int dh, const int *rowptr, const int *bcol, const double *bval, double shift, double *dinv,
+                                 int *fail, cudaStream_t stream);
 
 // ---- frame alignment of the distributed initialisation (dpgo_align.cu) ----
 // One aligning agent.  Its candidates are grouped per neighbour (group g = candidates [grp_ptr[g], grp_ptr[g+1]) against

@@ -616,6 +616,69 @@ void build_numeric(const BsrView &Q, const Options &opt, Hierarchy &H, std::vect
   }
 }
 
+void build_refactor(const Hierarchy &H, Refactor &R) {
+  const int dh = H.dh;
+  const size_t nn = H.nodes.size();
+  R = Refactor();
+  std::vector<int> order(nn);
+  std::iota(order.begin(), order.end(), 0);
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return H.nodes[(size_t)a].stage < H.nodes[(size_t)b].stage; });
+  std::vector<int> idx(nn);
+  for (size_t q = 0; q < nn; ++q) idx[(size_t)order[q]] = (int)q;
+  R.stage0.assign((size_t)H.nstages + 1, 0);
+  R.max_nfr.assign((size_t)H.nstages, 0);
+  R.max_s.assign((size_t)H.nstages, 0);
+  R.max_blob.assign((size_t)H.nstages, 0);
+  std::vector<int64_t> stage_front((size_t)H.nstages, 0), stage_ws((size_t)H.nstages, 0);
+  std::vector<int> where((size_t)H.n, -1);                   // pose -> position in the child's bnd list
+  for (int m : order) {
+    const MacroNode &mn = H.nodes[(size_t)m];
+    const int st = mn.stage, no = (int)mn.own.size(), nb = (int)mn.bnd.size(), nfr = no + nb;
+    const int64_t M = (int64_t)dh * nfr, s = (int64_t)dh * no, b = (int64_t)dh * nb;
+    RefactorNode rn = {};
+    rn.front = stage_front[(size_t)st];
+    rn.ws = stage_ws[(size_t)st];
+    rn.gf = mn.gf_off;
+    rn.gb = mn.gb_off;
+    rn.no = no;
+    rn.nb = nb;
+    rn.pose0 = (int)R.poses.size();
+    rn.ch0 = (int)R.child.size();
+    rn.nch = (int)mn.children.size();
+    R.poses.insert(R.poses.end(), mn.own.begin(), mn.own.end());
+    R.poses.insert(R.poses.end(), mn.bnd.begin(), mn.bnd.end());
+    for (int c : mn.children) {
+      const MacroNode &ch = H.nodes[(size_t)c];
+      if (ch.stage != st - 1) throw std::runtime_error("nd: a child two stages below its parent");
+      R.child.push_back({idx[(size_t)c], (int)R.cmap.size()});
+      for (size_t k = 0; k < ch.bnd.size(); ++k) where[(size_t)ch.bnd[k]] = (int)k;
+      for (int q = 0; q < nfr; ++q) R.cmap.push_back(where[(size_t)R.poses[(size_t)rn.pose0 + q]]);
+      for (int p : ch.bnd) where[(size_t)p] = -1;
+    }
+    stage_front[(size_t)st] += M * M;
+    stage_ws[(size_t)st] += (int64_t)REFACTOR_PIVOT_BLOCK * (REFACTOR_PIVOT_BLOCK + 2 * M);
+    R.max_nfr[(size_t)st] = std::max(R.max_nfr[(size_t)st], nfr);
+    R.max_s[(size_t)st] = std::max(R.max_s[(size_t)st], (int)s);
+    R.max_blob[(size_t)st] = std::max<int64_t>(R.max_blob[(size_t)st], (int64_t)ceil_div(nfr, 2) * PANEL_ROWS * s +
+                                                                         (int64_t)ceil_div(no, 2) * PANEL_ROWS * b);
+    R.stage0[(size_t)st + 1]++;
+    R.nodes.push_back(rn);
+  }
+  for (int st = 0; st < H.nstages; ++st) R.stage0[(size_t)st + 1] += R.stage0[(size_t)st];
+  int64_t even = 0, odd = 0, ws = 0;
+  for (int st = 0; st < H.nstages; ++st) {
+    (st % 2 ? odd : even) = std::max(st % 2 ? odd : even, stage_front[(size_t)st]);
+    ws = std::max(ws, stage_ws[(size_t)st]);
+  }
+  for (RefactorNode &rn : R.nodes) {
+    const int st = H.nodes[(size_t)order[(size_t)(&rn - R.nodes.data())]].stage;
+    if (st % 2) rn.front += even;
+  }
+  R.arena_even = even;
+  R.arena_doubles = std::max<int64_t>(even + odd, 1);
+  R.ws_doubles = std::max<int64_t>(ws, 1);
+}
+
 // =================================================================================================================
 // 3. plan
 // =================================================================================================================

@@ -130,5 +130,35 @@ void emulate_apply(const Hierarchy &H, const Plan &P, const std::vector<double> 
 
 std::string describe(const Hierarchy &H, const Plan &P);
 
+// ---- numeric refactorisation on the device (nd_refactor.cu): the algorithm of build_numeric over the fronts of the macro
+// nodes, stage by stage, for a Q whose block pattern is unchanged.  The front of node v is the dense symmetric matrix
+// [Foo Fob; Fob^T Fbb] over its front poses (own, then bnd), column-major, leading dimension M = dh (own + bnd); a
+// Gauss-Jordan sweep over its first s = dh own pivots leaves W = Foo^-1, Fm = W Fob and U = Fbb - Fob^T Fm in place, and
+// U stays there until the parent's stage has added it.  Fronts of stage st live in the arena at base (st even: 0, odd:
+// arena_even), so a child's U (stage st - 1) is never overwritten while its parent (stage st) is assembled.
+constexpr int REFACTOR_PIVOT_BLOCK = 32;   // pivots per Gauss-Jordan step (dense_inverse.cu GJB)
+struct RefactorNode {
+  long long front;           // arena offset (doubles) of the front
+  long long ws;              // workspace offset (doubles): pivot block, row panel, column panel of the sweep
+  long long gf, gb;          // panel blob offsets (MacroNode::gf_off / gb_off)
+  int no, nb;                // own / boundary poses
+  int pose0;                 // first front pose in Refactor::poses
+  int ch0, nch;              // children in Refactor::child (mn.children order)
+  int pad;
+};
+struct RefactorChild { int node; int map0; };   // refactor-node index of the child; map0: Refactor::cmap offset (one entry per parent front pose)
+struct Refactor {
+  std::vector<RefactorNode> nodes;   // stage by stage, deepest first (the order build_numeric visits)
+  std::vector<int> stage0;           // nstages + 1: node range of every stage
+  std::vector<int> poses;            // front poses of every node, own then bnd
+  std::vector<RefactorChild> child;
+  std::vector<int> cmap;             // position of a parent front pose in the child's bnd list, -1 when absent
+  std::vector<int> max_nfr, max_s;   // per stage: largest front (poses), largest pivot count (scalars)
+  std::vector<int64_t> max_blob;     // per stage: largest panel region of one node (doubles)
+  int64_t arena_even = 0, arena_doubles = 0, ws_doubles = 0;
+};
+// Throws std::runtime_error when a child is not exactly one stage below its parent (the arena parity relies on it).
+void build_refactor(const Hierarchy &H, Refactor &R);
+
 }  // namespace nd
 }  // namespace dpgo

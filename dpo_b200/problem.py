@@ -18,6 +18,22 @@ from ._capi import (ALG_RGD, ALG_RTR, PRECOND_BLOCK_JACOBI, PRECOND_DENSE_EXACT,
                     OptParams, OptResult)
 
 
+class _DeviceArray:
+    """__cuda_array_interface__ of m float64 at a device address; keeps the owning problem alive while viewed."""
+
+    def __init__(self, ptr: int, m: int, owner):
+        self._owner = owner
+        self.__cuda_array_interface__ = {"shape": (m,), "typestr": "<f8", "data": (ptr or 0, False), "version": 3,
+                                         "strides": None, "stream": None}
+
+
+def _device_view(ptr: int, m: int, device: int, owner):
+    import torch
+    t = torch.as_tensor(_DeviceArray(ptr, m, owner), device=torch.device("cuda", device))
+    t._dpgo_owner = owner
+    return t
+
+
 class ROPTALG:
     """ref: include/DPGO/DPGO_types.h:29-35"""
     RTR = ALG_RTR
@@ -151,6 +167,49 @@ class QuadraticProblem:
     def setEdgeWeights(self, weights) -> None:
         w = np.ascontiguousarray(weights, dtype=np.float64)
         capi.check(self._lib.dpgo_problem_set_edge_weights(self._h, capi.dptr(w)))
+
+    # -- stream-ordered re-weighting (no host copy, no synchronisation; see dpgo_problem_robust_reweight_async) ---------
+    def robustReweightAsync(self, cost: str, mu: float = 1.0, param: float = 1.0) -> None:
+        """robustReweight on the handle's stream: weights, Q and the prepared preconditioners all refreshed on the device.
+        The first call after setEdges builds the sparse exact preconditioner's structure on the host and synchronises;
+        every later one can be captured into a CUDA graph."""
+        capi.check(self._lib.dpgo_problem_robust_reweight_async(self._h, self.ROBUST[cost], float(mu), float(param)))
+
+    def setEdgeWeightsAsync(self, weights) -> None:
+        """weights: a float64 CUDA tensor of the edge count on the problem's device, or a device pointer (int).  Read in
+        the handle's stream order."""
+        if isinstance(weights, int):
+            ptr = weights
+        else:
+            if not (getattr(weights, "is_cuda", False) and weights.dtype.is_floating_point and weights.element_size() == 8):
+                raise ValueError("weights must be a float64 CUDA tensor or a device pointer")
+            if weights.device.index != self.device or weights.numel() != getattr(self, "_num_edges", 0) or not weights.is_contiguous():
+                raise ValueError("weights must be a contiguous tensor of one weight per edge on the problem's device")
+            ptr = weights.data_ptr()
+        capi.check(self._lib.dpgo_problem_set_edge_weights_async(self._h, C.c_void_p(ptr)))
+
+    def edgeWeightsDevice(self):
+        """(weights, squared residuals): torch float64 views of the device arrays (one entry per edge), not copies."""
+        import torch
+        w, r2 = C.c_void_p(), C.c_void_p()
+        capi.check(self._lib.dpgo_problem_device_edge_weights(self._h, C.byref(w), C.byref(r2)))
+        m = getattr(self, "_num_edges", 0)
+        return _device_view(w.value, m, self.device, self), _device_view(r2.value, m, self.device, self)
+
+    def gncCounts(self):
+        """(weight 1, weight 0, in between) over the non-fixed edges at the last re-weight (synchronises)."""
+        out = (C.c_int64 * 3)()
+        capi.check(self._lib.dpgo_problem_gnc_counts(self._h, out))
+        return int(out[0]), int(out[1]), int(out[2])
+
+    def nd_node_sizes(self):
+        """(own poses, boundary poses, stage) of every macro node of the sparse exact preconditioner (prepares it)."""
+        cnt = C.c_int64()
+        capi.check(self._lib.dpgo_nd_node_sizes(self._h, 0, None, None, None, C.byref(cnt)))
+        own, bnd, st = (np.zeros(max(cnt.value, 1), dtype=np.int32) for _ in range(3))
+        capi.check(self._lib.dpgo_nd_node_sizes(self._h, cnt.value, capi.iptr(own), capi.iptr(bnd), capi.iptr(st), C.byref(cnt)))
+        n = cnt.value
+        return own[:n], bnd[:n], st[:n]
 
     def setG(self, G) -> None:
         """G: dense (r, (d+1)n) array, scipy sparse matrix, or None to clear.  ref: setG, .cpp:44-48."""

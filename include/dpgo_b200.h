@@ -155,6 +155,28 @@ DPGO_API int dpgo_problem_robust_reweight(dpgo_problem_t *p, int cost, double mu
                                           double *residuals2_host);
 /* replace the edge weights (m values) and re-assemble Q on the device */
 DPGO_API int dpgo_problem_set_edge_weights(dpgo_problem_t *p, const double *weights_host);
+/* Stream-ordered re-weighting: the reference re-weights the loop closures and rebuilds Q and its factorisation every
+ * robustOptInnerIters iterations (PGOAgent::iterate / updateLoopClosuresWeights / constructQMatrix + setQ,
+ * src/PGOAgent.cpp:653-667, 1109-1112, 1174-1289).  These calls do it without a host copy or a synchronisation, on the
+ * handle's stream: the same weights and the same k_assemble_Q as the synchronous calls above, then every prepared
+ * preconditioner is refactorised ON THE DEVICE -- block-Jacobi (one 4x4 SPD inverse per pose) and the sparse exact one
+ * (the multifrontal factorisation of its hierarchy, written into its panels in place).  Device buffers keep their
+ * addresses and the handle's generation is not bumped, so a round graph captured before stays valid, and the calls can
+ * themselves be captured into a CUDA graph, with two exceptions that synchronise (and so cannot be captured):
+ *  - the first call after the sparse exact preconditioner's structure was dropped (set_edges, a synchronous re-weight) or
+ *    never built builds its hierarchy and plan on the host, as its first use does;
+ *  - a prepared dense exact preconditioner (the A/B switch) is dropped and rebuilt synchronously on its next use.
+ * A front that is not positive definite (impossible for weights >= 0) sets a device flag that the next synchronising call
+ * (dpgo_problem_sync, dpgo_optimize_result, dpgo_problem_gnc_counts, ...) reports as DPGO_ERR_CUDA.
+ * weights_dev: m doubles in device memory on the handle's device, read in stream order. */
+DPGO_API int dpgo_problem_set_edge_weights_async(dpgo_problem_t *p, const double *weights_dev);
+DPGO_API int dpgo_problem_robust_reweight_async(dpgo_problem_t *p, int cost, double mu, double param);
+/* The device arrays of the edge weights and of the squared residuals of the last re-weight (m doubles each), for reading
+ * or for writing weights in place before dpgo_problem_set_edge_weights_async(p, *w_dev). */
+DPGO_API int dpgo_problem_device_edge_weights(dpgo_problem_t *p, double **w_dev, double **res2_dev);
+/* Counts of the last re-weight over the non-fixed edges: out3 = {weight exactly 1, exactly 0, in between} -- what the
+ * reference's PGOAgent::computeConvergedLoopClosureRatio counts (src/PGOAgent.cpp:1247-1289).  Synchronises. */
+DPGO_API int dpgo_problem_gnc_counts(dpgo_problem_t *p, int64_t *out3);
 /* ref: QuadraticProblem::setG, src/QuadraticProblem.cpp:44-48.  Dense r x (d+1)n column-major,
  * or the reference's sparse form (row-major CSR with r rows).  NULL / nnz == 0 clears G. */
 DPGO_API int dpgo_problem_set_G_dense(dpgo_problem_t *p, const double *G_host);
@@ -233,6 +255,9 @@ DPGO_API int dpgo_sym_plan(int N, int grid, double chunk_cost, int32_t *segptr, 
  * 3 bytes of all blocks, 4 matrix bytes streamed per application, 5 largest own block (scalars), 6 largest boundary
  * (scalars), 7 dissection depth, 8 steps, 9 jobs, 10 epilogues, 11.. reserved */
 DPGO_API int dpgo_nd_info(dpgo_problem_t *p, int64_t *info16);
+/* Sizes of the hierarchy's macro nodes (prepares it if needed): *count nodes; the first min(cap, count) get their own and
+ * boundary pose counts and their stage (0 = deepest).  The work of a refactorisation follows from them. */
+DPGO_API int dpgo_nd_node_sizes(dpgo_problem_t *p, int64_t cap, int32_t *own, int32_t *bnd, int32_t *stage, int64_t *count);
 /* HOST ONLY, verification of the planning code on machines without a GPU (never used by a product path): builds the
  * hierarchy, the blocks and the phase plan for the block matrix given as in dpgo_problem_set_Q_blocks and runs a host
  * emulation of the plan exactly as the kernel interprets it:  Z = (Q + shift I)^-1 V  (no projection), V and Z
