@@ -35,8 +35,14 @@ struct BlockCtx {
 // so a phase end has two bar.syncs, not four.  (A fused variant -- 16-byte {value, phase} packets polled all-to-all, barrier
 // and all-reduce in one round trip -- is not faster: scripts/barrier_bench3.cu compares the two; with gpu-scope "strong"
 // 16-byte accesses it is much slower.)
-template <int NUSED = NRED>
-__device__ __forceinline__ void phase_end(const KParams &kp, BlockCtx &bc, double (&acc)[NRED]) {
+// `update(totals)` runs in thread 0 between the two bar.syncs: it advances the CTA's SolverState (below), which every
+// thread reads after the second one.
+struct NoUpdate {
+  __device__ void operator()(const double *) const {}
+};
+
+template <int NUSED = NRED, class Update = NoUpdate>
+__device__ __forceinline__ void phase_end(const KParams &kp, BlockCtx &bc, double (&acc)[NRED], const Update &update = Update()) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
 #pragma unroll
   for (int q = 0; q < NUSED; ++q) {
@@ -89,12 +95,32 @@ __device__ __forceinline__ void phase_end(const KParams &kp, BlockCtx &bc, doubl
         if (lane == 0) outp[q] = v;
       }
     }
+    if (lane == 0) update(outp);
   }
   __syncthreads();
 #pragma unroll
   for (int q = 0; q < NUSED; ++q) acc[q] = outp[q];
   bc.parity ^= 1;
 }
+
+// The scalar state of the solver's control flow: trust region, tCG recurrences, the result record.  It is the same in
+// every thread of every CTA, so it lives once per CTA in shared memory rather than in registers of all 512 threads, where
+// it would stay live across every phase.  Thread 0 advances it inside phase_end (`update`) with the totals of the phase;
+// every thread reads it, and the branch it decided, after the phase end.
+struct SolverState {
+  dpgo_opt_result_t res;
+  double f1, gn, zr0;                      // cost, |RG| and <z0, RG> at the base point
+  double Delta, Delta_max;                 // trust-region radius
+  double z_r, d_Pd, e_Pd, e_Pe, n0, alpha, beta, tau;   // tCG recurrences
+  double denom;                            // model decrease of the candidate
+  int cb;                                  // base buffer
+  int pd;                                  // delta_old lives in V_D0 + pd
+  int zsrc_z;                              // the Hessian's operand is V_Z (else the base point's V_Z00)
+  int eta_zero, z0_valid, status, iter, total_steps;
+  int brk;                                 // the last update leaves its loop
+  unsigned long long tick_last;            // phase clock (FULL): thread 0 of CTA 0 only
+};
+constexpr int STATE_DOUBLES = (int)((sizeof(SolverState) + 15) / 16) * 2;   // keeps the following blocks 16-byte aligned
 
 // The CTA's row range and (when it fits) a shared-memory copy of its block-CSR structure, set up once per launch: the
 // sparse phases then start their X gathers without first waiting for two dependent global loads (row pointer, indices).
@@ -1035,8 +1061,16 @@ template <int R, int DH, bool FULL> __global__ void __launch_bounds__(OPT_THREAD
   BlockCtx bc;
   bc.sm_warp = smem;
   bc.sm_out = smem + (OPT_THREADS / 32) * NRED;
+  SolverState &S = *reinterpret_cast<SolverState *>(bc.sm_out + 2 * NRED);
+  if (threadIdx.x == 0) {                       // ordered before any read by the barrier below
+    dpgo_opt_result_t &res = S.res;
+    res.success = 0; res.tcg_status = DPGO_TCG_NOT_RUN; res.tcg_iterations = 0; res.outer_iterations = 0;
+    res.rejections = 0; res.spmv_passes = 0; res.precond_applies = 0; res.reserved0 = 0;
+    res.f_init = res.gradnorm_init = res.f_opt = res.gradnorm_opt = res.relative_change = res.elapsed_ms = 0.0;
+    res.quad_init = res.lin_init = 0.0;
+  }
   // the CTA's rows and, when they fit, its slice of the block-CSR structure in shared memory (SP_CACHE_INTS ints)
-  int *sp_ints = reinterpret_cast<int *>(bc.sm_out + 2 * NRED);
+  int *sp_ints = reinterpret_cast<int *>(bc.sm_out + 2 * NRED + STATE_DOUBLES);
   CtaRows cr;
   cr.r0 = ld_const(kp.cta_rows + blockIdx.x);
   cr.r1 = ld_const(kp.cta_rows + blockIdx.x + 1);
@@ -1083,25 +1117,17 @@ template <int R, int DH, bool FULL> __global__ void __launch_bounds__(OPT_THREAD
   bc.parity = 0;
   // diagnostic phase clock: CTA 0 / thread 0 charges the time since the previous tick to a phase kind
   // (0 eval, 1 dense apply, 2 partial sums + projection, 3 Hessian product, 4 tCG update, 5 retraction, 6 final)
-  unsigned long long tick_last = 0;
-  const bool ticking = FULL && (kp.phase_ns != nullptr) && blockIdx.x == 0 && threadIdx.x == 0;
   auto tick = [&](int kind) {
-    if (ticking) {
+    if (FULL && kp.phase_ns != nullptr && blockIdx.x == 0 && threadIdx.x == 0) {
       unsigned long long t;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      if (kind >= 0) kp.phase_ns[kind] += t - tick_last;
-      tick_last = t;
+      if (kind >= 0) kp.phase_ns[kind] += t - S.tick_last;
+      S.tick_last = t;
     }
   };
   tick(-1);
-  const dpgo_opt_params_t prm = kp.prm;
-  const int precond = prm.precond;
+  const int precond = kp.prm.precond;
   const bool exact = (precond == DPGO_PRECOND_DENSE_EXACT) || (precond == DPGO_PRECOND_SPARSE_EXACT);
-  dpgo_opt_result_t res;
-  res.success = 0; res.tcg_status = DPGO_TCG_NOT_RUN; res.tcg_iterations = 0; res.outer_iterations = 0;
-  res.rejections = 0; res.spmv_passes = 0; res.precond_applies = 0; res.reserved0 = 0;
-  res.f_init = res.gradnorm_init = res.f_opt = res.gradnorm_opt = res.relative_change = res.elapsed_ms = 0.0;
-  res.quad_init = res.lin_init = 0.0;
   double acc[NRED];
   // sparse exact preconditioner: shared memory = gathered input tiles + partial-sum slots (aliases the dense ring)
   double *nd_ys = sV;
@@ -1110,15 +1136,15 @@ template <int R, int DH, bool FULL> __global__ void __launch_bounds__(OPT_THREAD
   // the CTA's resident panel columns, aliased by nothing; the launch's first application (no application counted yet:
   // z0 of the first outer iteration, or the single-operation entry point) fills them
   double *nd_res = reinterpret_cast<double *>(nd_grec + 2 * (size_t)kp.nd.max_gathers);
-  // Z = P_X( (Q + 0.1 I)^-1 V ), returns <Z, V> in acc[0]; every phase ends with a grid barrier
-  auto apply_exact = [&](const double *Vv, int cbx, double *Zout) {
+  // Z = P_X( (Q + 0.1 I)^-1 V ), <Z, V> in acc[0] and to `update`; every phase ends with a grid barrier
+  auto apply_exact = [&](const double *Vv, int cbx, double *Zout, const auto &update) {
     if (!FULL || precond == DPGO_PRECOND_SPARSE_EXACT) {     // the lean variant is never launched with the dense one
       zero(acc);
       for (int ph = 0; ph < kp.nd.nphases; ++ph) {
-        phase_nd<R, DH, FULL>(kp, ph, Vv, cbx, Zout, nd_ys, nd_slots, nd_grec, nd_res, res.precond_applies == 0, acc);
+        phase_nd<R, DH, FULL>(kp, ph, Vv, cbx, Zout, nd_ys, nd_slots, nd_grec, nd_res, S.res.precond_applies == 0, acc);
         if (ph + 1 < kp.nd.nphases) { phase_end<0>(kp, bc, acc); tick(8 + min(ph, 15)); }
       }
-      phase_end<1>(kp, bc, acc);
+      phase_end<1>(kp, bc, acc, update);
       tick(8 + min(kp.nd.nphases - 1, 15));
     } else {
       if (dense_sym) phase_dense_sym<R>(kp, Vv, ring, sV, sMeta);
@@ -1127,7 +1153,7 @@ template <int R, int DH, bool FULL> __global__ void __launch_bounds__(OPT_THREAD
       zero(acc); phase_end<0>(kp, bc, acc);
       tick(1);
       zero(acc); phase_pz<R, DH>(kp, cr, cbx, Vv, Zout, sV, acc);
-      phase_end<1>(kp, bc, acc);
+      phase_end<1>(kp, bc, acc, update);
       tick(2);
     }
   };
@@ -1136,13 +1162,13 @@ template <int R, int DH, bool FULL> __global__ void __launch_bounds__(OPT_THREAD
 
   // ---- single-operation entry points -------------------------------------------------------
   if (kp.op == OP_PHASE_BENCH) {          // diagnostic: tr_max_inner empty phases (barrier + 1-scalar reduction)
-    for (int i = 0; i < prm.tr_max_inner; ++i) { zero(acc); acc[0] = 1.0; phase_end<1>(kp, bc, acc); }
-    if (blockIdx.x == 0 && threadIdx.x == 0) { res.f_init = acc[0]; *kp.result = res; *kp.bar_epoch = bc.epoch; }
+    for (int i = 0; i < kp.prm.tr_max_inner; ++i) { zero(acc); acc[0] = 1.0; phase_end<1>(kp, bc, acc); }
+    if (blockIdx.x == 0 && threadIdx.x == 0) { S.res.f_init = acc[0]; *kp.result = S.res; *kp.bar_epoch = bc.epoch; }
     return;
   }
   if (kp.op == OP_PRECON) {
     if (exact) {
-      apply_exact(kp.v[V_AUX], 0, kp.v[V_Z]);
+      apply_exact(kp.v[V_AUX], 0, kp.v[V_Z], NoUpdate());
     } else {
       // reuse phase_update with res := AUX (first = false, alpha = 0 would need RES); do it directly
       constexpr int TS = R * DH;
@@ -1176,171 +1202,195 @@ template <int R, int DH, bool FULL> __global__ void __launch_bounds__(OPT_THREAD
   }
 
   // ---- statistics at the input point (ref: src/QuadraticOptimizer.cpp:36-37) -------------------
+  const bool single = (kp.prm.tr_iterations == 1);      // ref :92-110 shrink-until-accepted mode
+  // thread 0: start a truncated CG solve (ROPTLIB SolversTR::tCG_TR; theta = 1, kappa = 0.1, Min_Inner_Iter = 0)
+  auto tcg_begin = [&]() {
+    S.z_r = S.zr0; S.d_Pd = S.zr0; S.e_Pd = 0.0; S.e_Pe = 0.0;
+    S.n0 = S.gn;
+    S.res.precond_applies++;                           // z0 = M^-1 g
+    S.beta = 0.0; S.tau = 0.0;
+    S.zsrc_z = 0; S.pd = 0; S.eta_zero = 1; S.status = DPGO_TCG_MAXITER;
+  };
+  // thread 0: the next tCG direction from the new <z, res>
+  auto tcg_next = [&](double zr_new) {
+    S.res.precond_applies++;
+    const double beta = zr_new / S.z_r;
+    S.beta = beta;
+    S.z_r = zr_new;
+    S.zsrc_z = 1;
+    S.e_Pd = beta * (S.e_Pd + S.alpha * S.d_Pd);
+    S.d_Pd = S.z_r + beta * beta * S.d_Pd;
+  };
   zero(acc);
   phase_eval<R, DH>(kp, cr, 0, true, precond, acc);
-  phase_end(kp, bc, acc);
+  phase_end(kp, bc, acc, [&](const double *t) {
+    dpgo_opt_result_t &res = S.res;
+    res.spmv_passes++;
+    const double f1 = 0.5 * t[0] + t[1];
+    const double gn = sqrt(t[2]);
+    S.f1 = f1; S.gn = gn; S.zr0 = t[3];
+    res.f_init = f1;
+    res.gradnorm_init = gn;
+    res.quad_init = t[0];
+    res.lin_init = t[1];
+    res.f_opt = f1;
+    res.gradnorm_opt = gn;
+    // the trust region's start (ref :80-81, :96-97); its first tCG solve starts here unless z0 is still to be applied
+    S.Delta = kp.prm.tr_initial_radius;
+    S.Delta_max = single ? S.Delta : 5.0 * kp.prm.tr_initial_radius;
+    S.total_steps = 0; S.cb = 0; S.iter = 0;
+    S.z0_valid = !exact;
+    if (kp.op != OP_EVAL && kp.op != OP_RHESS && kp.prm.algorithm != DPGO_ALG_RGD && gn >= kp.prm.tr_tolerance && !exact)
+      tcg_begin();
+  });
   tick(0);
-  res.spmv_passes++;
-  double f1 = 0.5 * acc[0] + acc[1];
-  double gn = sqrt(acc[2]);
-  double zr0 = acc[3];
-  res.f_init = f1;
-  res.gradnorm_init = gn;
-  res.quad_init = acc[0];
-  res.lin_init = acc[1];
-  res.f_opt = f1;
-  res.gradnorm_opt = gn;
 
   if (kp.op == OP_EVAL) {
-    res.success = 1;
-    if (blockIdx.x == 0 && threadIdx.x == 0) { *kp.result = res; *kp.bar_epoch = bc.epoch; }
+    if (blockIdx.x == 0 && threadIdx.x == 0) { S.res.success = 1; *kp.result = S.res; *kp.bar_epoch = bc.epoch; }
     return;
   }
   if (kp.op == OP_RHESS) {
     zero(acc);
     phase_hess<R, DH, FULL>(kp, cr, 0, kp.v[V_AUX], nullptr, nullptr, 0.0, false, acc);
     phase_end(kp, bc, acc);
-    if (blockIdx.x == 0 && threadIdx.x == 0) { *kp.result = res; *kp.bar_epoch = bc.epoch; }
+    if (blockIdx.x == 0 && threadIdx.x == 0) { *kp.result = S.res; *kp.bar_epoch = bc.epoch; }
     return;
   }
 
-  if (prm.algorithm == DPGO_ALG_RGD) {
+  if (kp.prm.algorithm == DPGO_ALG_RGD) {
     // ---- one fixed-step Riemannian gradient-descent step (ref :124-149) ----------------------
     zero(acc);
-    phase_retract<R, DH>(kp, cr, 0, 1, nullptr, 0.0, false, prm.rgd_stepsize, acc);
+    phase_retract<R, DH>(kp, cr, 0, 1, nullptr, 0.0, false, kp.prm.rgd_stepsize, acc);
     phase_end(kp, bc, acc);
     zero(acc);
     phase_eval<R, DH>(kp, cr, 1, false, DPGO_PRECOND_NONE, acc);
-    phase_end(kp, bc, acc);
-    res.spmv_passes++;
-    res.f_opt = 0.5 * acc[0] + acc[1];
-    res.gradnorm_opt = sqrt(acc[2]);
-    res.outer_iterations = 1;
+    phase_end(kp, bc, acc, [&](const double *t) {
+      S.res.spmv_passes++;
+      S.res.f_opt = 0.5 * t[0] + t[1];
+      S.res.gradnorm_opt = sqrt(t[2]);
+      S.res.outer_iterations = 1;
+    });
     cur = 1;
-  } else if (gn >= prm.tr_tolerance) {           // ref :67-70 early exit otherwise
+  } else if (S.gn >= kp.prm.tr_tolerance) {      // ref :67-70 early exit otherwise
     // ---- Riemannian trust region ------------------------------------------------------------
-    const bool single = (prm.tr_iterations == 1);      // ref :92-110 shrink-until-accepted mode
-    double Delta = prm.tr_initial_radius;
-    const double Delta_max = single ? Delta : 5.0 * prm.tr_initial_radius;   // ref :80-81,:96-97
-    int total_steps = 0;
-    int cb = 0;                      // base buffer
-    bool z0_valid = !exact;
-    int iter = 0;
     while (true) {
-      // -- z0 = M^-1 g for the dense preconditioner (pose-local ones were fused into phase E)
-      if (!z0_valid) {
-        apply_exact(kp.v[V_RG0 + cb], cb, kp.v[V_Z00 + cb]);
-        zr0 = acc[0];
-        z0_valid = true;
+      // -- z0 = M^-1 g for the exact preconditioners (pose-local ones were fused into phase E)
+      if (!S.z0_valid) {
+        const int cb = S.cb;
+        apply_exact(kp.v[V_RG0 + cb], cb, kp.v[V_Z00 + cb], [&](const double *t) {
+          S.zr0 = t[0];
+          S.z0_valid = 1;
+          tcg_begin();
+        });
       }
-      // -- truncated CG (ROPTLIB SolversTR::tCG_TR; theta = 1, kappa = 0.1, Min_Inner_Iter = 0)
-      double z_r = zr0, d_Pd = zr0, e_Pd = 0.0, e_Pe = 0.0;
-      const double n0 = gn;
-      res.precond_applies++;                       // z0 = M^-1 g
-      double beta = 0.0, tau = 0.0;
-      const double *zsrc = kp.v[V_Z00 + cb];
-      int pd = 0;                                  // delta_old lives in V_D0 + pd
-      bool eta_zero = true;
-      int status = DPGO_TCG_MAXITER;
-      const double *dcur = nullptr;
-      for (int j = 0; j < prm.tr_max_inner; ++j) {
-        double *dnew = kp.v[V_D0 + (1 - pd)];
-        zero(acc);
-        phase_hess<R, DH, FULL>(kp, cr, cb, zsrc, kp.v[V_D0 + pd], dnew, beta, true, acc);
-        phase_end<1>(kp, bc, acc);
+      // -- truncated CG
+      for (int j = 0; j < kp.prm.tr_max_inner; ++j) {
+        {
+          const int cb = S.cb, pd = S.pd;
+          zero(acc);
+          phase_hess<R, DH, FULL>(kp, cr, cb, S.zsrc_z ? kp.v[V_Z] : kp.v[V_Z00 + cb], kp.v[V_D0 + pd], kp.v[V_D0 + (1 - pd)],
+                                  S.beta, true, acc);
+        }
+        phase_end<1>(kp, bc, acc, [&](const double *t) {
+          S.res.spmv_passes++;
+          S.res.tcg_iterations++;
+          S.pd = 1 - S.pd;                               // delta_new becomes delta_old
+          const double d_Hd = t[0];
+          const double Delta = S.Delta, e_Pd = S.e_Pd, d_Pd = S.d_Pd, e_Pe = S.e_Pe;
+          const double alpha = S.z_r / d_Hd;
+          const double e_new = e_Pe + 2.0 * alpha * e_Pd + alpha * alpha * d_Pd;
+          S.alpha = alpha;
+          S.brk = d_Hd <= 0.0 || e_new >= Delta * Delta;
+          if (S.brk) {
+            S.tau = (-e_Pd + sqrt(e_Pd * e_Pd + d_Pd * (Delta * Delta - e_Pe))) / d_Pd;
+            S.status = (d_Hd <= 0.0) ? DPGO_TCG_NEGCURVTURE : DPGO_TCG_EXCREGION;
+          } else {
+            S.e_Pe = e_new;
+          }
+        });
         tick(3);
-        res.spmv_passes++;
-        res.tcg_iterations++;
-        pd = 1 - pd;
-        dcur = dnew;
-        const double d_Hd = acc[0];
-        const double alpha = z_r / d_Hd;
-        const double e_new = e_Pe + 2.0 * alpha * e_Pd + alpha * alpha * d_Pd;
-        if (d_Hd <= 0.0 || e_new >= Delta * Delta) {
-          tau = (-e_Pd + sqrt(e_Pd * e_Pd + d_Pd * (Delta * Delta - e_Pe))) / d_Pd;
-          status = (d_Hd <= 0.0) ? DPGO_TCG_NEGCURVTURE : DPGO_TCG_EXCREGION;
-          break;
-        }
-        e_Pe = e_new;
+        if (S.brk) break;
         zero(acc);
-        phase_update<R, DH>(kp, cr, cb, dcur, alpha, eta_zero, precond, acc);
-        phase_end<2>(kp, bc, acc);
+        phase_update<R, DH>(kp, cr, S.cb, kp.v[V_D0 + S.pd], S.alpha, S.eta_zero, precond, acc);
+        phase_end<2>(kp, bc, acc, [&](const double *t) {
+          S.eta_zero = 0;
+          const double nr = sqrt(t[0]);
+          const double n0 = S.n0;
+          const double n0t = n0;                         // n0^theta, theta = 1
+          S.brk = nr <= n0 * fmin(n0t, 0.1);
+          if (S.brk) S.status = (0.1 < n0t) ? DPGO_TCG_LCON : DPGO_TCG_SCON;
+          else if (!exact) tcg_next(t[1]);
+        });
         tick(4);
-        eta_zero = false;
-        const double nr = sqrt(acc[0]);
-        const double n0t = n0;                         // n0^theta, theta = 1
-        if (nr <= n0 * fmin(n0t, 0.1)) {
-          status = (0.1 < n0t) ? DPGO_TCG_LCON : DPGO_TCG_SCON;
-          break;
-        }
-        double zr_new = acc[1];
-        if (exact) {
-          apply_exact(kp.v[V_RES], cb, kp.v[V_Z]);
-          zr_new = acc[0];
-        }
-        res.precond_applies++;
-        beta = zr_new / z_r;
-        z_r = zr_new;
-        zsrc = kp.v[V_Z];
-        e_Pd = beta * (e_Pd + alpha * d_Pd);
-        d_Pd = z_r + beta * beta * d_Pd;
+        if (S.brk) break;
+        if (exact) apply_exact(kp.v[V_RES], S.cb, kp.v[V_Z], [&](const double *t) { tcg_next(t[0]); });
       }
-      res.tcg_status = status;
-      res.outer_iterations++;
       // -- candidate point, model decrease, actual decrease
       zero(acc);
-      phase_retract<R, DH>(kp, cr, cb, 0, dcur, tau, eta_zero, 0.0, acc);
-      phase_end<2>(kp, bc, acc);
+      phase_retract<R, DH>(kp, cr, S.cb, 0, kp.v[V_D0 + S.pd], S.tau, S.eta_zero, 0.0, acc);   // delta: read when tau != 0
+      phase_end<2>(kp, bc, acc, [&](const double *t) {
+        S.res.tcg_status = S.status;
+        S.res.outer_iterations++;
+        S.denom = -t[0] - 0.5 * t[1];
+      });
       tick(5);
-      const double denom = -acc[0] - 0.5 * acc[1];
       zero(acc);
-      phase_eval<R, DH>(kp, cr, 1 - cb, false, precond, acc);
-      phase_end(kp, bc, acc);
-      tick(0);
-      res.spmv_passes++;
-      const double f2 = 0.5 * acc[0] + acc[1];
-      const double gn2 = sqrt(acc[2]);
-      const double rho = (denom != 0.0) ? (f1 - f2) / denom : -1.0;
-      const bool accepted = rho > 0.1;                 // ROPTLIB Acceptence_Rho
-      if (single) {
-        if (accepted) {
-          cb = 1 - cb; res.f_opt = f2; res.gradnorm_opt = gn2;
-          break;
-        }
-        res.rejections++;
-        if (total_steps > 10) break;                   // ref :101-103 return the initial guess
-        Delta *= 0.25;                                 // ref :104-107
-        total_steps++;
-      } else {
-        // ROPTLIB SolversTR radius update (Shrinked_tau = 0.25, Magnified_tau = 2)
-        if (rho < 0.25) Delta *= 0.25;
-        else if (rho > 0.75 && (status == DPGO_TCG_NEGCURVTURE || status == DPGO_TCG_EXCREGION))
-          Delta = fmin(2.0 * Delta, Delta_max);
-        if (accepted) {
-          cb = 1 - cb; f1 = f2; gn = gn2; zr0 = acc[3];
-          res.f_opt = f2; res.gradnorm_opt = gn2;
-          z0_valid = !exact;
+      phase_eval<R, DH>(kp, cr, 1 - S.cb, false, precond, acc);
+      phase_end(kp, bc, acc, [&](const double *t) {
+        dpgo_opt_result_t &res = S.res;
+        res.spmv_passes++;
+        const double f2 = 0.5 * t[0] + t[1];
+        const double gn2 = sqrt(t[2]);
+        const double denom = S.denom;
+        const double rho = (denom != 0.0) ? (S.f1 - f2) / denom : -1.0;
+        const bool accepted = rho > 0.1;                 // ROPTLIB Acceptence_Rho
+        if (single) {
+          if (accepted) {
+            S.cb = 1 - S.cb; res.f_opt = f2; res.gradnorm_opt = gn2;
+            S.brk = 1;
+          } else {
+            res.rejections++;
+            S.brk = S.total_steps > 10;                  // ref :101-103 return the initial guess
+            if (!S.brk) {
+              S.Delta *= 0.25;                           // ref :104-107
+              S.total_steps++;
+            }
+          }
         } else {
-          res.rejections++;
+          // ROPTLIB SolversTR radius update (Shrinked_tau = 0.25, Magnified_tau = 2)
+          if (rho < 0.25) S.Delta *= 0.25;
+          else if (rho > 0.75 && (S.status == DPGO_TCG_NEGCURVTURE || S.status == DPGO_TCG_EXCREGION))
+            S.Delta = fmin(2.0 * S.Delta, S.Delta_max);
+          if (accepted) {
+            S.cb = 1 - S.cb; S.f1 = f2; S.gn = gn2; S.zr0 = t[3];
+            res.f_opt = f2; res.gradnorm_opt = gn2;
+            S.z0_valid = !exact;
+          } else {
+            res.rejections++;
+          }
+          ++S.iter;
+          S.brk = S.gn < kp.prm.tr_tolerance || S.iter >= kp.prm.tr_iterations;
         }
-        ++iter;
-        if (gn < prm.tr_tolerance || iter >= prm.tr_iterations) break;
-      }
+        if (!S.brk && S.z0_valid) tcg_begin();
+      });
+      tick(0);
+      if (S.brk) break;
     }
-    cur = cb;
+    cur = S.cb;
   }
 
   zero(acc);
   phase_final<R, DH>(kp, cr, cur, acc);
-  phase_end<1>(kp, bc, acc);
+  phase_end<1>(kp, bc, acc, [&](const double *t) {
+    S.res.relative_change = sqrt(t[0] / (double)kp.n);
+    S.res.success = 1;
+  });
   tick(6);
-  res.relative_change = sqrt(acc[0] / (double)kp.n);
-  res.success = 1;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
-    *kp.result = res;
+    *kp.result = S.res;
     *kp.bar_epoch = bc.epoch;
     // the team status reads the relative change from here: the result record is overwritten by every OP_EVAL
-    if (kp.opt_record) { kp.opt_record[0] = res.relative_change; kp.opt_record[1] += 1.0; }
+    if (kp.opt_record) { kp.opt_record[0] = S.res.relative_change; kp.opt_record[1] += 1.0; }
   }
 }
 
@@ -1517,13 +1567,16 @@ __global__ void k_edge_weights(int64_t m, const int *__restrict__ p1, const int 
 // Dynamic shared memory of one launch: the reduction scratch, plus what the launch's preconditioner stages (the dense
 // ring or the sparse plan's tiles, slots and resident panel columns).  Launches without the sparse plan ask for no more
 // than they stage and leave the rest of the SM's 228 KB to L1; the sparse plan's resident columns take what it leaves.
+// (reduction scratch, the solver state and the block-CSR copy: the prefix every launch has)
+constexpr size_t OPT_SMEM_BASE_DOUBLES = (OPT_THREADS / 32) * NRED + 2 * NRED + STATE_DOUBLES + SP_CACHE_INTS / 2;
+
 template <int R, int DH> static size_t nd_staged_doubles(const KNd &nd) {
-  return (OPT_THREADS / 32) * NRED + 2 * NRED + SP_CACHE_INTS / 2 + (size_t)nd.max_ytiles * R * DH +
-         (size_t)(nd.max_slots + 1) * nd::PANEL_ROWS * R + 4 * (size_t)nd.max_gathers + 8;
+  return OPT_SMEM_BASE_DOUBLES + (size_t)nd.max_ytiles * R * DH + (size_t)(nd.max_slots + 1) * nd::PANEL_ROWS * R +
+         4 * (size_t)nd.max_gathers + 8;
 }
 
 template <int R, int DH> static size_t optimize_smem_doubles(const KParams &kp) {
-  const size_t base = (OPT_THREADS / 32) * NRED + 2 * NRED + SP_CACHE_INTS / 2;
+  const size_t base = OPT_SMEM_BASE_DOUBLES;
   const size_t dense = (size_t)DENSE_PER_MAX * R + (size_t)DENSE_RING_DOUBLES + 2 * DENSE_NST + (size_t)SYM_META_DOUBLES;
   if (kp.prm.precond == DPGO_PRECOND_DENSE_EXACT) return base + dense;
   if (kp.prm.precond == DPGO_PRECOND_SPARSE_EXACT) return nd_staged_doubles<R, DH>(kp.nd) + (size_t)kp.nd.resident_doubles;
