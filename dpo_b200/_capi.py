@@ -96,8 +96,6 @@ SIGNATURES = {
     "dpgo_spmv_device": (C.c_int, [_vp, _vp, _vp, C.c_int]),
     "dpgo_spmv_algorithmic_bytes": (C.c_int64, [_vp, C.c_int]),
     "dpgo_precond_algorithmic_bytes": (C.c_int64, [_vp, C.c_int]),
-    "dpgo_sym_plan_sizes": (C.c_int, [C.c_int, _ip, _ip]),
-    "dpgo_sym_plan": (C.c_int, [C.c_int, C.c_int, C.c_double, _ip, _ip, _ip, _ip, C.POINTER(C.c_int64)]),
     "dpgo_nd_info": (C.c_int, [_vp, C.POINTER(C.c_int64)]),
     "dpgo_nd_node_sizes": (C.c_int, [_vp, C.c_int64, _ip, _ip, _ip, C.POINTER(C.c_int64)]),
     "dpgo_nd_debug_emulate": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int64, _ip, _ip, _dp, C.c_double, C.c_int, C.c_int,

@@ -45,6 +45,13 @@ int fail(int code, const std::string &msg) {
     if (_s != DPGO_OK) return _s; \
   } while (0)
 
+// The two exact preconditioners apply the same operator P_X((Q + 0.1 I)^-1 V) with the same block solve: SPARSE_EXACT on
+// the macro levels the cost model picks, DENSE_EXACT on a single one, whose root panels are the dense inverse of every
+// connected component.  A launch reads the factorisation its preconditioner selects (the sparse one unless DENSE_EXACT).
+enum NdSlot { ND_SPARSE = 0, ND_DENSE = 1 };
+int nd_slot(int precond) { return precond == DPGO_PRECOND_DENSE_EXACT ? ND_DENSE : ND_SPARSE; }
+int nd_precond(int slot) { return slot == ND_DENSE ? DPGO_PRECOND_DENSE_EXACT : DPGO_PRECOND_SPARSE_EXACT; }
+
 }  // namespace
 
 struct dpgo_problem {
@@ -72,15 +79,9 @@ struct dpgo_problem {
     std::vector<double> h_bval;
     bool h_stale = false;        // an asynchronous re-weight changed bval on the device only (sync_host_bval)
   } bsr;
-  // the dense exact preconditioner (ensure_dense); dropped whenever Q changes
-  struct Dense {
-    DevBuf<double> pinv, part, t2, ppack;
-    int per = 1;
-    int sym_ok = 0;              // symmetric (upper-triangle) dense preconditioner planned
-    DevBuf<long long> sym_off;
-    DevBuf<int> sym_cut, sym_segptr, sym_cfirst, sym_ccount;
-  } dense;
-  // the sparse exact preconditioner: the nested-dissection factorisation (ensure_nd); dropped whenever Q changes
+  // the exact preconditioners: one nested-dissection block factorisation of Q + 0.1 I per kind (ensure_nd), nd[ND_SPARSE]
+  // on the cost model's macro levels, nd[ND_DENSE] on a single one; dropped by set_Q / a synchronous re-weight, refactorised
+  // in place by an asynchronous one
   struct Nd {
     bool ready = false;
     dpgo::KNd k = {};            // kernel view of the buffers below
@@ -100,7 +101,7 @@ struct dpgo_problem {
     DevBuf<int> rposes, rcmap;
     DevBuf<double> arena, ws;
     DevBuf<dpgo::GjJob> rjobs;
-  } nd;
+  } nd[2];
   // edge records for the device-side Q assembly / robust re-weighting (dpgo_problem_set_edges)
   struct Edges {
     int64_t ne = 0;
@@ -189,17 +190,6 @@ void fill_kparams(const dpgo_problem *p, dpgo::KParams &kp, int op, const dpgo_o
   kp.bcol = p->bsr.bcol.get();
   kp.bval = p->bsr.bval.get();
   kp.dinv = p->bsr.dinv.get();
-  kp.pinv = p->dense.pinv.get();
-  kp.dense_part = p->dense.part.get();
-  kp.dense_per = p->dense.per;
-  kp.sym_ok = p->dense.sym_ok;
-  kp.ppack = p->dense.ppack.get();
-  kp.sym_off = p->dense.sym_off.get();
-  kp.sym_cut = p->dense.sym_cut.get();
-  kp.sym_segptr = p->dense.sym_segptr.get();
-  kp.sym_cfirst = p->dense.sym_cfirst.get();
-  kp.sym_ccount = p->dense.sym_ccount.get();
-  kp.dense_t2 = p->dense.t2.get();
   kp.cta_rows = p->bsr.cta_rows.get();
   kp.G = p->G.get();
   for (int i = 0; i < dpgo::V_COUNT; ++i) kp.v[i] = p->vec[i].get();
@@ -207,8 +197,9 @@ void fill_kparams(const dpgo_problem *p, dpgo::KParams &kp, int op, const dpgo_o
   kp.partials = p->bsr.partials.get();
   kp.bar_counter = p->bar.get();
   kp.bar_epoch = p->bar.get() + 1;
-  kp.nd = p->nd.k;
-  if (!p->nd.ready) kp.nd.nphases = 0;
+  const dpgo_problem::Nd &F = p->nd[nd_slot(prm.precond)];
+  kp.nd = F.k;
+  if (!F.ready) kp.nd.nphases = 0;
   static const int strict = [] { const char *e = std::getenv("DPGO_STRICT_ACQUIRE"); return (e && e[0] == '1') ? 1 : 0; }();
   kp.strict_acquire = strict;
   kp.cluster = p->cluster ? 1 : 0;
@@ -226,122 +217,6 @@ cudaError_t run_spmv(const dpgo_problem *p, const double *X, const double *G, do
     return dpgo::launch_spmv_tma(p->r, p->dh, p->bsr.ngroups, p->bsr.groups.get(), p->bsr.rowptr.get(), p->bsr.bcol.get(),
                                  p->bsr.bval.get(), X, G, out, p->sms, p->stream);
   return dpgo::launch_spmv(p->r, p->dh, p->n, p->bsr.rowptr.get(), p->bsr.bcol.get(), p->bsr.bval.get(), X, G, out, p->stream);
-}
-
-// Work decomposition of the symmetric (upper-triangle) dense apply (phase_dense_sym) -- host only, also exported as
-// dpgo_sym_plan so that CPU tests can check it.  Chunks (segment J of 480 columns, 8-row group g with 8g < end of J) in
-// segment-major order are cut into `grid` contiguous runs of equal cost; per segment the consecutive CTAs that touch it
-// get the partial-panel slots 0..ccount-1; `off` is the chunk-major packed layout (8 rows x (width up to 8, + 4) doubles).
-// Cost model of one chunk in column units: streamed width + a fixed part.  The fixed part dominates (waits, fragment
-// parking, the masked diagonal path cost about the same whatever the width), so the runs get nearly equal chunk COUNTS;
-// DPGO_SYM_CHUNK_COST overrides it for A/B runs.
-constexpr double SYM_CHUNK_COST = 800.0;
-constexpr int SYM_PLAN_SEG = 480;      // = dpgo::SYM_SEG of the kernel (15 consumer warps x 32 columns)
-
-struct SymPlan {
-  int nseg = 0, nchunks = 0;
-  std::vector<int> segptr, cut, cfirst, ccount;
-  std::vector<long long> off;
-};
-
-bool make_sym_plan(int64_t N, int G, double chunk_cost, SymPlan &pl) {
-  if (N % 2 != 0 || N < 2048 || G < 1) return false;       // bulk TMA needs 16-byte aligned rows; small N: plain apply
-  const int SEG = SYM_PLAN_SEG, nseg = (int)((N + SEG - 1) / SEG);
-  pl.nseg = nseg;
-  pl.segptr.assign((size_t)nseg + 1, 0);
-  for (int J = 0; J < nseg; ++J) {
-    const int s1 = (int)std::min<int64_t>(N, (int64_t)(J + 1) * SEG);
-    pl.segptr[(size_t)J + 1] = pl.segptr[(size_t)J] + (s1 + 7) / 8;
-  }
-  const int nchunks = pl.nchunks = pl.segptr[(size_t)nseg];
-  std::vector<double> cum((size_t)nchunks + 1, 0.0);
-  pl.off.assign((size_t)nchunks + 1, 0);
-  {
-    int lin = 0;
-    for (int J = 0; J < nseg; ++J) {
-      const int s0 = J * SEG, s1 = (int)std::min<int64_t>(N, (int64_t)s0 + SEG);
-      for (int g = 0; 8 * g < s1; ++g, ++lin) {
-        const int width = s1 - std::max(s0, 8 * g);
-        cum[(size_t)lin + 1] = cum[(size_t)lin] + (double)width + chunk_cost;
-        pl.off[(size_t)lin + 1] = pl.off[(size_t)lin] + 8LL * (((width + 7) & ~7) + 4);
-      }
-    }
-  }
-  pl.cut.assign((size_t)G + 1, 0);
-  {
-    int lin = 0;
-    for (int b = 1; b < G; ++b) {
-      const double target = cum[(size_t)nchunks] * b / G;
-      while (lin < nchunks && cum[(size_t)lin + 1] <= target) ++lin;
-      pl.cut[(size_t)b] = lin;
-    }
-    pl.cut[(size_t)G] = nchunks;
-  }
-  pl.cfirst.assign((size_t)nseg, 0);
-  pl.ccount.assign((size_t)nseg, 0);
-  int maxslots = 0;
-  for (int J = 0; J < nseg; ++J) {
-    int first = -1, last = -1;
-    for (int b = 0; b < G; ++b)
-      if (pl.cut[(size_t)b] < pl.segptr[(size_t)J + 1] && pl.cut[(size_t)b + 1] > pl.segptr[(size_t)J] &&
-          pl.cut[(size_t)b] < pl.cut[(size_t)b + 1]) {
-        if (first < 0) first = b;
-        last = b;
-      }
-    pl.cfirst[(size_t)J] = std::max(first, 0);
-    pl.ccount[(size_t)J] = (first < 0) ? 0 : last - first + 1;
-    maxslots = std::max(maxslots, pl.ccount[(size_t)J]);
-  }
-  bool runs_ok = (maxslots <= G);   // the panels live in dense_part (grid x r x N)
-  for (int b = 0; b < G; ++b) runs_ok = runs_ok && (pl.cut[(size_t)b] < pl.cut[(size_t)b + 1]);   // slots assume no empty run
-  return runs_ok;
-}
-
-// The dense inverse (Q + 0.1 I)^-1 is built on first use (one-shot: scatter block-CSR into N x N in HBM, blocked
-// Gauss-Jordan in place) -- problems that are only evaluated (e.g. the drivers' centralised problem) never pay for it.
-int ensure_dense(dpgo_problem *p) {
-  if (p->dense.pinv) return DPGO_OK;
-  if (!(p->bsr.precond_mask & (1u << DPGO_PRECOND_DENSE_EXACT)))
-    return fail(DPGO_ERR_STATE, "dense exact preconditioner was not requested in set_Q (precond_mask)");
-  const size_t N = (size_t)p->N;
-  if (N * N * sizeof(double) > (size_t)48 << 30)
-    return fail(DPGO_ERR_UNSUPPORTED, "dense exact preconditioner limited to N^2*8 <= 48 GiB; use block-Jacobi");
-  dpgo_problem::Dense &D = p->dense;
-  D.per = (int)((N + p->grid - 1) / p->grid);
-  if (D.per > dpgo::DENSE_PER_MAX)
-    return fail(DPGO_ERR_UNSUPPORTED, "dense exact preconditioner: N too large for the per-CTA slab; use block-Jacobi");
-  DPGO_CUDA(D.part.alloc((size_t)p->grid * p->r * N));
-  DPGO_CUDA(cudaMemsetAsync(D.part.get(), 0, sizeof(double) * (size_t)p->grid * p->r * N, p->stream));
-  DPGO_CUDA(D.pinv.alloc(N * N));
-  DPGO_CUDA(cudaMemsetAsync(D.pinv.get(), 0, N * N * sizeof(double), p->stream));
-  cudaError_t e = dpgo::launch_bsr_to_dense(p->n, p->dh, p->bsr.nb, p->bsr.rowptr.get(), p->bsr.bcol.get(), p->bsr.bval.get(),
-                                            0.1, D.pinv.get(), p->N, p->stream);
-  if (e == cudaSuccess) e = dpgo::dense_spd_inverse(D.pinv.get(), p->N, p->stream);
-  if (e != cudaSuccess) {
-    D = {};
-    return fail(DPGO_ERR_CUDA, std::string("dense preconditioner setup: ") + cudaGetErrorString(e));
-  }
-  // symmetric (upper-triangle) variant: plan, packed copy, partial buffers (falls back to the full matrix otherwise)
-  static const bool no_sym = [] { const char *e2 = std::getenv("DPGO_DENSE_FULL"); return e2 && e2[0] == '1'; }();
-  static const double chunk_cost = [] { const char *e4 = std::getenv("DPGO_SYM_CHUNK_COST"); return e4 ? std::atof(e4) : SYM_CHUNK_COST; }();
-  D.sym_ok = 0;
-  SymPlan plan;
-  if (!no_sym && make_sym_plan((int64_t)N, p->grid, chunk_cost, plan)) {
-    const int nseg = plan.nseg, nchunks = plan.nchunks;
-    DPGO_CUDA(D.t2.alloc((size_t)nseg * p->r * N));
-    DPGO_CUDA(cudaMemsetAsync(D.t2.get(), 0, sizeof(double) * (size_t)nseg * p->r * N, p->stream));
-    DPGO_CUDA(D.ppack.alloc((size_t)plan.off[(size_t)nchunks]));
-    DPGO_CUDA(D.sym_off.assign(plan.off.data(), plan.off.size(), p->stream));
-    DPGO_CUDA(D.sym_cut.assign(plan.cut.data(), plan.cut.size(), p->stream));
-    DPGO_CUDA(D.sym_segptr.assign(plan.segptr.data(), plan.segptr.size(), p->stream));
-    DPGO_CUDA(D.sym_cfirst.assign(plan.cfirst.data(), plan.cfirst.size(), p->stream));
-    DPGO_CUDA(D.sym_ccount.assign(plan.ccount.data(), plan.ccount.size(), p->stream));
-    DPGO_CUDA(dpgo::launch_pack_sym(D.pinv.get(), (int)N, nchunks, D.sym_segptr.get(), nseg, D.sym_off.get(), D.ppack.get(),
-                                    p->stream));
-    DPGO_CUDA(cudaStreamSynchronize(p->stream));
-    D.sym_ok = 1;
-  }
-  return DPGO_OK;
 }
 
 void nd_fill_info(const dpgo::nd::Hierarchy &H, const dpgo::nd::Plan &P, int64_t *info) {
@@ -383,7 +258,7 @@ dpgo::nd::Options nd_options(int grid, int r, bool cluster = false) {
 
 void free_nd(dpgo_problem *p) {
   ++p->generation;
-  p->nd = {};
+  for (dpgo_problem::Nd &F : p->nd) F = {};
 }
 
 // The host copy of Q's values after an asynchronous re-weight changed them on the device only: downloaded before any
@@ -397,32 +272,96 @@ int sync_host_bval(dpgo_problem *p) {
   return DPGO_OK;
 }
 
-// The nested-dissection block factorisation of Q + 0.1 I is built on first use (host: ordering, symbolic, plan; the
-// dense algebra of large blocks on the device), like the dense inverse.
-int ensure_nd(dpgo_problem *p) {
-  if (p->nd.ready) return DPGO_OK;
-  if (!(p->bsr.precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)))
-    return fail(DPGO_ERR_STATE, "sparse exact preconditioner was not requested in set_Q (precond_mask)");
+// A factorisation's device refactorisation: scatter maps, fronts, sweep jobs of its hierarchy, built once per hierarchy on
+// the host (synchronises).
+int ensure_refactor(dpgo_problem *p, int slot) {
   namespace nd = dpgo::nd;
-  free_nd(p);
-  DPGO_TRY(sync_host_bval(p));
+  dpgo_problem::Nd &F = p->nd[slot];
+  if (F.R) return DPGO_OK;
+  const std::string what = slot == ND_DENSE ? "dense exact preconditioner refactorisation" : "sparse exact preconditioner refactorisation";
+  auto R = std::make_unique<nd::Refactor>();
+  try {
+    nd::build_refactor(*F.H, *R);
+  } catch (const std::exception &e) {
+    return fail(DPGO_ERR_UNSUPPORTED, what + ": " + e.what());
+  }
+  for (size_t st = 0; st + 1 < R->stage0.size(); ++st)
+    if (R->stage0[st + 1] - R->stage0[st] > 65535) return fail(DPGO_ERR_UNSUPPORTED, what + ": more than 65535 nodes in one stage");
+  if (R->child.empty()) R->child.push_back({0, 0});        // one macro level: no children, nothing reads these
+  if (R->cmap.empty()) R->cmap.push_back(-1);
+  DPGO_CUDA(F.rnodes.assign(R->nodes.data(), R->nodes.size(), p->stream));
+  DPGO_CUDA(F.rchild.assign(R->child.data(), R->child.size(), p->stream));
+  DPGO_CUDA(F.rposes.assign(R->poses.data(), R->poses.size(), p->stream));
+  DPGO_CUDA(F.rcmap.assign(R->cmap.data(), R->cmap.size(), p->stream));
+  DPGO_CUDA(F.arena.alloc((size_t)R->arena_doubles));
+  DPGO_CUDA(F.ws.alloc((size_t)R->ws_doubles));
+  std::vector<dpgo::GjJob> jobs(R->nodes.size());
+  constexpr int B = nd::REFACTOR_PIVOT_BLOCK;
+  for (size_t q = 0; q < jobs.size(); ++q) {
+    const nd::RefactorNode &rn = R->nodes[q];
+    const int M = p->dh * (rn.no + rn.nb);
+    double *w = F.ws.get() + rn.ws;
+    jobs[q] = {F.arena.get() + rn.front, w, w + B * B, w + B * B + (size_t)B * M, M, p->dh * rn.no};
+  }
+  DPGO_CUDA(F.rjobs.assign(jobs.data(), jobs.size(), p->stream));
+  DPGO_CUDA(cudaStreamSynchronize(p->stream));
+  F.R = std::move(R);
+  return DPGO_OK;
+}
+
+// The numbers of a factorisation recomputed from Q's values on the device, its panels rewritten in place: ordinary
+// launches on the handle's stream, no host work, no synchronisation.
+int launch_refactor(dpgo_problem *p, int slot) {
+  dpgo_problem::Nd &F = p->nd[slot];
+  dpgo::KRefactor k;
+  k.dh = p->dh;
+  k.shift = 0.1;
+  k.nodes = F.rnodes.get();
+  k.child = F.rchild.get();
+  k.poses = F.rposes.get();
+  k.cmap = F.rcmap.get();
+  k.rowptr = p->bsr.rowptr.get();
+  k.bcol = p->bsr.bcol.get();
+  k.bval = p->bsr.bval.get();
+  k.arena = F.arena.get();
+  k.jobs = F.rjobs.get();
+  k.blob = F.blob.get();
+  k.fail = p->edges.fail.get();
+  DPGO_CUDA(dpgo::launch_nd_refactor(k, *F.R, p->stream));
+  return DPGO_OK;
+}
+
+// An exact preconditioner's block factorisation of Q + 0.1 I is built on first use (host: ordering, symbolic, plan).  The
+// sparse one takes its numbers from the host (build_numeric); the dense one, whose single macro level is the dense inverse
+// of every connected component (an O(N^3) host inverse), from the device refactorisation of Q's values.
+int ensure_nd(dpgo_problem *p, int slot) {
+  dpgo_problem::Nd &F = p->nd[slot];
+  if (F.ready) return DPGO_OK;
+  const bool dense = slot == ND_DENSE;
+  const std::string what = dense ? "dense exact preconditioner" : "sparse exact preconditioner";
+  if (!(p->bsr.precond_mask & (1u << nd_precond(slot))))
+    return fail(DPGO_ERR_STATE, what + " was not requested in set_Q (precond_mask)");
+  namespace nd = dpgo::nd;
+  ++p->generation;
+  F = {};
+  if (!dense) DPGO_TRY(sync_host_bval(p));
   nd::Plan plan;
   std::vector<double> blob;
   auto H = std::make_unique<nd::Hierarchy>();
   try {
-    const nd::Options opt = nd_options(p->grid, p->r, p->cluster);
+    nd::Options opt = nd_options(p->grid, p->r, p->cluster);
+    if (dense) opt.force_ncuts = 0;
     nd::BsrView Q{p->n, p->dh, p->bsr.h_rowptr.data(), p->bsr.h_bcol.data(), p->bsr.h_bval.data()};
     nd::build_hierarchy(Q, opt, *H);
-    nd::build_numeric(Q, opt, *H, blob);
+    if (!dense) nd::build_numeric(Q, opt, *H, blob);
     nd::build_plan(*H, opt, plan);
   } catch (const std::exception &e) {
-    return fail(DPGO_ERR_UNSUPPORTED, std::string("sparse exact preconditioner setup: ") + e.what());
+    return fail(DPGO_ERR_UNSUPPORTED, what + " setup: " + e.what());
   }
   if (plan.max_ytiles > dpgo::ND_YCAP_TILES || plan.max_slots > dpgo::ND_SLOT_CAP)
-    return fail(DPGO_ERR_UNSUPPORTED, "sparse exact preconditioner: plan exceeds the shared-memory capacities");
-  dpgo_problem::Nd &F = p->nd;
+    return fail(DPGO_ERR_UNSUPPORTED, what + ": plan exceeds the shared-memory capacities");
   if ((int)plan.phases.size() > dpgo::nd::MAX_PHASES)
-    return fail(DPGO_ERR_UNSUPPORTED, "sparse exact preconditioner: too many phases");
+    return fail(DPGO_ERR_UNSUPPORTED, what + ": too many phases");
   dpgo::KNd &K = F.k;
   nd_kernel_sizes(plan, K);
   try {
@@ -430,7 +369,7 @@ int ensure_nd(dpgo_problem *p) {
     // sphere2500 / torus3D on one H100 80GB HBM3 at 400 W: 6818-6878 / 7689-7729 rounds/s against 7177-7222 / 7819-7855)
     nd::assign_residency(plan, dpgo::OPT_THREADS / 32, p->cluster ? 0 : dpgo::nd_resident_budget(p->r, p->dh, K));
   } catch (const std::exception &e) {
-    return fail(DPGO_ERR_UNSUPPORTED, std::string("sparse exact preconditioner setup: ") + e.what());
+    return fail(DPGO_ERR_UNSUPPORTED, what + " setup: " + e.what());
   }
   K.resident_doubles = plan.max_resident_doubles;
   nd_fill_info(*H, plan, F.info);
@@ -442,7 +381,13 @@ int ensure_nd(dpgo_problem *p) {
   DPGO_CUDA(F.jobs.assign(plan.jobs.data(), plan.jobs.size(), p->stream));
   DPGO_CUDA(F.epis.assign(plan.epis.data(), plan.epis.size(), p->stream));
   DPGO_CUDA(F.csrc.assign(plan.csrc.data(), plan.csrc.size(), p->stream));
-  DPGO_CUDA(F.blob.assign(blob.data(), blob.size(), p->stream));
+  if (dense) {
+    // the refactorisation writes every panel row a front pose owns; the padding rows keep these zeros
+    DPGO_CUDA(F.blob.alloc((size_t)F.H->blob_doubles));
+    DPGO_CUDA(cudaMemsetAsync(F.blob.get(), 0, sizeof(double) * (size_t)F.H->blob_doubles, p->stream));
+  } else {
+    DPGO_CUDA(F.blob.assign(blob.data(), blob.size(), p->stream));
+  }
   K.cta_phase = F.cta_phase.get(); K.steps = F.steps.get(); K.gathers = F.gathers.get(); K.jobs = F.jobs.get();
   K.epis = F.epis.get(); K.csrc = F.csrc.get(); K.blob = F.blob.get();
   const size_t tile = (size_t)p->ts;
@@ -452,6 +397,10 @@ int ensure_nd(dpgo_problem *p) {
   K.C = F.C.get();
   DPGO_CUDA(cudaMemsetAsync(K.TX, 0, sizeof(double) * tile * (size_t)p->n, p->stream));
   DPGO_CUDA(cudaMemsetAsync(K.C, 0, sizeof(double) * tile * (size_t)F.H->cbuf_tiles, p->stream));
+  if (dense) {
+    DPGO_TRY(ensure_refactor(p, slot));
+    DPGO_TRY(launch_refactor(p, slot));
+  }
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
   K.nphases = (int)plan.phases.size();
   F.ready = true;
@@ -461,10 +410,9 @@ int ensure_nd(dpgo_problem *p) {
 
 int check_precond(dpgo_problem *p, int precond) {
   if (precond < 0 || precond > 3) return fail(DPGO_ERR_INVALID_ARG, "unknown preconditioner id");
-  if (precond == DPGO_PRECOND_SPARSE_EXACT) return ensure_nd(p);
+  if (precond == DPGO_PRECOND_SPARSE_EXACT || precond == DPGO_PRECOND_DENSE_EXACT) return ensure_nd(p, nd_slot(precond));
   if (precond == DPGO_PRECOND_BLOCK_JACOBI && !p->bsr.dinv)
     return fail(DPGO_ERR_STATE, "block-Jacobi preconditioner was not prepared by set_Q (precond_mask)");
-  if (precond == DPGO_PRECOND_DENSE_EXACT) return ensure_dense(p);
   return DPGO_OK;
 }
 
@@ -567,7 +515,7 @@ int build_from_triplets(dpgo_problem *p, std::vector<BlockTriplet> &trip, unsign
   static const int cluster_max_poses = [] { const char *e = std::getenv("DPGO_CLUSTER_MAX_POSES"); return e ? std::atoi(e) : 0; }();
   p->cluster = false;
   const bool want_cluster = p->launch_mode == 1 || (p->launch_mode < 0 && n <= cluster_max_poses);
-  if (p->max_cluster >= 8 && want_cluster && !(precond_mask & (1u << DPGO_PRECOND_DENSE_EXACT))) {
+  if (p->max_cluster >= 8 && want_cluster) {
     // (one CTA per 16 poses is enough: always taking 16 CTAs makes small agents slower)
     grid = std::max(1, std::min(p->max_cluster, (n + rows_per_pass - 1) / rows_per_pass));
     p->cluster = true;
@@ -590,7 +538,6 @@ int build_from_triplets(dpgo_problem *p, std::vector<BlockTriplet> &trip, unsign
   // upload
   cudaSetDevice(p->device);
   p->bsr = {};
-  p->dense = {};
   free_nd(p);
   dpgo_problem::BlockQ &B = p->bsr;
   B.h_rowptr = rowptr;
@@ -1170,49 +1117,21 @@ int64_t dpgo_spmv_algorithmic_bytes(const dpgo_problem_t *p, int add_G) {
   return b;
 }
 
-int dpgo_sym_plan_sizes(int N, int *num_segments, int *num_chunks) {
-  DPGO_REQUIRE(num_segments && num_chunks, DPGO_ERR_INVALID_ARG, "null argument");
-  DPGO_REQUIRE(N >= 1, DPGO_ERR_INVALID_ARG, "bad dimension");
-  const int nseg = (N + SYM_PLAN_SEG - 1) / SYM_PLAN_SEG;
-  int nch = 0;
-  for (int J = 0; J < nseg; ++J) nch += (std::min(N, (J + 1) * SYM_PLAN_SEG) + 7) / 8;
-  *num_segments = nseg;
-  *num_chunks = nch;
-  return DPGO_OK;
-}
-
-int dpgo_sym_plan(int N, int grid, double chunk_cost, int32_t *segptr, int32_t *cut, int32_t *cfirst, int32_t *ccount,
-                  int64_t *chunk_offset) {
-  DPGO_REQUIRE(segptr && cut && cfirst && ccount && chunk_offset, DPGO_ERR_INVALID_ARG, "null argument");
-  SymPlan pl;
-  if (!make_sym_plan((int64_t)N, grid, chunk_cost > 0 ? chunk_cost : SYM_CHUNK_COST, pl))
-    return fail(DPGO_ERR_UNSUPPORTED, "no symmetric plan for this size (odd N, N < 2048, or more CTAs than chunks)");
-  std::copy(pl.segptr.begin(), pl.segptr.end(), segptr);
-  std::copy(pl.cut.begin(), pl.cut.end(), cut);
-  std::copy(pl.cfirst.begin(), pl.cfirst.end(), cfirst);
-  std::copy(pl.ccount.begin(), pl.ccount.end(), ccount);
-  std::copy(pl.off.begin(), pl.off.end(), chunk_offset);
-  return DPGO_OK;
-}
-
 int64_t dpgo_precond_algorithmic_bytes(const dpgo_problem_t *p, int preconditioner) {
   if (!p) return 0;
   const int64_t N = (int64_t)p->dh * p->n, vec = (int64_t)p->r * N * 8;
   if (preconditioner == DPGO_PRECOND_BLOCK_JACOBI) return (int64_t)p->n * 16 * 8 + 2 * vec;
-  if (preconditioner == DPGO_PRECOND_SPARSE_EXACT) return p->nd.ready ? p->nd.info[4] + 2 * vec : 0;
-  if (preconditioner != DPGO_PRECOND_DENSE_EXACT) return 0;
-  // the inverse is symmetric: the unique data is its upper triangle in 8-row groups (what phase_dense_sym reads);
-  // the full-matrix variants read all of it
-  const int64_t mat = p->dense.sym_ok ? (N * N + 8 * N) / 2 * 8 : N * N * 8;
-  return mat + 2 * vec;
+  if (preconditioner != DPGO_PRECOND_SPARSE_EXACT && preconditioner != DPGO_PRECOND_DENSE_EXACT) return 0;
+  const dpgo_problem::Nd &F = p->nd[nd_slot(preconditioner)];
+  return F.ready ? F.info[4] + 2 * vec : 0;
 }
 
 int dpgo_nd_info(dpgo_problem_t *p, int64_t *info16) {
   DPGO_CHECK_HANDLE(p);
   DPGO_REQUIRE(info16, DPGO_ERR_INVALID_ARG, "null argument");
   DPGO_REQUIRE(p->bsr.have, DPGO_ERR_STATE, "set_Q has not been called");
-  DPGO_TRY(ensure_nd(p));
-  std::copy(p->nd.info, p->nd.info + 16, info16);
+  DPGO_TRY(ensure_nd(p, ND_SPARSE));
+  std::copy(p->nd[ND_SPARSE].info, p->nd[ND_SPARSE].info + 16, info16);
   return DPGO_OK;
 }
 
@@ -1324,7 +1243,6 @@ static int reassemble_Q(dpgo_problem *p) {
     DPGO_CUDA(cudaStreamSynchronize(p->stream));
   }
   free_nd(p);                                            // (Q + 0.1 I)^-1 changed: rebuilt on next use
-  p->dense = {};
   return DPGO_OK;
 }
 
@@ -1432,76 +1350,22 @@ int dpgo_problem_robust_reweight(dpgo_problem_t *p, int cost, double mu, double 
 }
 
 // ---- stream-ordered re-weighting: the preconditioners are refactorised on the device --------------------------------
-// The sparse exact preconditioner's device refactorisation: scatter maps, fronts and sweep jobs of its hierarchy, built
-// once per hierarchy on the host (synchronises).
-static int ensure_refactor(dpgo_problem *p) {
-  namespace nd = dpgo::nd;
-  dpgo_problem::Nd &F = p->nd;
-  if (F.R) return DPGO_OK;
-  auto R = std::make_unique<nd::Refactor>();
-  try {
-    nd::build_refactor(*F.H, *R);
-  } catch (const std::exception &e) {
-    return fail(DPGO_ERR_UNSUPPORTED, std::string("sparse exact preconditioner refactorisation: ") + e.what());
-  }
-  for (size_t st = 0; st + 1 < R->stage0.size(); ++st)
-    if (R->stage0[st + 1] - R->stage0[st] > 65535)
-      return fail(DPGO_ERR_UNSUPPORTED, "sparse exact preconditioner refactorisation: more than 65535 nodes in one stage");
-  if (R->child.empty()) R->child.push_back({0, 0});        // one macro level: no children, nothing reads these
-  if (R->cmap.empty()) R->cmap.push_back(-1);
-  DPGO_CUDA(F.rnodes.assign(R->nodes.data(), R->nodes.size(), p->stream));
-  DPGO_CUDA(F.rchild.assign(R->child.data(), R->child.size(), p->stream));
-  DPGO_CUDA(F.rposes.assign(R->poses.data(), R->poses.size(), p->stream));
-  DPGO_CUDA(F.rcmap.assign(R->cmap.data(), R->cmap.size(), p->stream));
-  DPGO_CUDA(F.arena.alloc((size_t)R->arena_doubles));
-  DPGO_CUDA(F.ws.alloc((size_t)R->ws_doubles));
-  std::vector<dpgo::GjJob> jobs(R->nodes.size());
-  constexpr int B = nd::REFACTOR_PIVOT_BLOCK;
-  for (size_t q = 0; q < jobs.size(); ++q) {
-    const nd::RefactorNode &rn = R->nodes[q];
-    const int M = p->dh * (rn.no + rn.nb);
-    double *w = F.ws.get() + rn.ws;
-    jobs[q] = {F.arena.get() + rn.front, w, w + B * B, w + B * B + (size_t)B * M, M, p->dh * rn.no};
-  }
-  DPGO_CUDA(F.rjobs.assign(jobs.data(), jobs.size(), p->stream));
-  DPGO_CUDA(cudaStreamSynchronize(p->stream));
-  F.R = std::move(R);
-  return DPGO_OK;
-}
-
-// After k_assemble_Q on the stream: block-Jacobi and the sparse exact preconditioner refactorised on the device, the dense
-// inverse dropped (rebuilt synchronously on its next use).  Only the first call after the sparse exact structure was
-// dropped (or never built) runs host work and synchronises.
+// After k_assemble_Q on the stream: block-Jacobi and the prepared exact preconditioners refactorised on the device.  Only
+// the first call after the sparse exact structure was dropped (or never built) runs host work and synchronises; an
+// unprepared dense one stays lazy.
 static int refresh_preconditioners_async(dpgo_problem *p) {
   p->bsr.h_stale = true;
-  if (p->dense.pinv) {                                  // its buffers go: a round captured with them must be re-captured
-    p->dense = {};
-    ++p->generation;
-  }
   dpgo_problem::Edges &E = p->edges;
   E.fail_armed = true;
   if (p->bsr.dinv)
     DPGO_CUDA(dpgo::launch_jacobi_blocks(p->n, p->dh, p->bsr.rowptr.get(), p->bsr.bcol.get(), p->bsr.bval.get(), 0.1,
                                          p->bsr.dinv.get(), E.fail.get(), p->stream));
-  if (!(p->bsr.precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT))) return DPGO_OK;
-  DPGO_TRY(ensure_nd(p));
-  DPGO_TRY(ensure_refactor(p));
-  dpgo_problem::Nd &F = p->nd;
-  dpgo::KRefactor k;
-  k.dh = p->dh;
-  k.shift = 0.1;
-  k.nodes = F.rnodes.get();
-  k.child = F.rchild.get();
-  k.poses = F.rposes.get();
-  k.cmap = F.rcmap.get();
-  k.rowptr = p->bsr.rowptr.get();
-  k.bcol = p->bsr.bcol.get();
-  k.bval = p->bsr.bval.get();
-  k.arena = F.arena.get();
-  k.jobs = F.rjobs.get();
-  k.blob = F.blob.get();
-  k.fail = E.fail.get();
-  DPGO_CUDA(dpgo::launch_nd_refactor(k, *F.R, p->stream));
+  if (p->bsr.precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)) DPGO_TRY(ensure_nd(p, ND_SPARSE));
+  for (int slot : {ND_SPARSE, ND_DENSE}) {
+    if (!p->nd[slot].ready) continue;
+    DPGO_TRY(ensure_refactor(p, slot));
+    DPGO_TRY(launch_refactor(p, slot));
+  }
   return DPGO_OK;
 }
 
@@ -1553,8 +1417,8 @@ int dpgo_nd_node_sizes(dpgo_problem_t *p, int64_t cap, int32_t *own, int32_t *bn
   DPGO_CHECK_HANDLE(p);
   DPGO_REQUIRE(count && cap >= 0 && (cap == 0 || (own && bnd && stage)), DPGO_ERR_INVALID_ARG, "null argument");
   DPGO_REQUIRE(p->bsr.have, DPGO_ERR_STATE, "set_Q has not been called");
-  DPGO_TRY(ensure_nd(p));
-  const auto &nodes = p->nd.H->nodes;
+  DPGO_TRY(ensure_nd(p, ND_SPARSE));
+  const auto &nodes = p->nd[ND_SPARSE].H->nodes;
   *count = (int64_t)nodes.size();
   for (size_t q = 0; q < nodes.size() && (int64_t)q < cap; ++q) {
     own[q] = (int32_t)nodes[q].own.size();
@@ -1826,7 +1690,8 @@ int round_preamble(dpgo_problem_t *const *agents, int num_active, const dpgo_opt
     DPGO_TRY(check_params(p, params));
     if (!p->ev_done) DPGO_CUDA(dpgo::create_event(p->ev_done));
     // a cooperative launch does not capture; a pending G clear or an unbuilt factorisation must run eagerly first
-    if (!p->cluster || p->G_dirty || p->phase_ns || ((p->bsr.precond_mask & (1u << DPGO_PRECOND_SPARSE_EXACT)) && !p->nd.ready))
+    const int slot = nd_slot(params->precond);
+    if (!p->cluster || p->G_dirty || p->phase_ns || ((p->bsr.precond_mask & (1u << nd_precond(slot))) && !p->nd[slot].ready))
       graph = false;
   }
   dpgo_problem *lead = agents[0];

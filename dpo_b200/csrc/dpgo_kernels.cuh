@@ -38,9 +38,8 @@ constexpr int ND_YCAP_TILES = 600;  // sparse exact preconditioner: pose tiles o
 constexpr int ND_SLOT_CAP = 240;    // ... and partial-sum slots (8 rows x r doubles) per step
 constexpr int OPT_SMEM_LIMIT = 227 * 1024;  // dynamic shared memory one CTA of an H100 may ask for (checked by optimize_max_grid)
 constexpr int SP_CACHE_INTS = 2048;  // shared-memory copy of a CTA's block-CSR structure (row pointers + block columns), 8 KB
-constexpr int DENSE_PER_MAX = 512;  // max rows of the dense inverse one CTA owns (smem staging of V): N <= 67k at 132 CTAs
 
-// sparse exact preconditioner (nd_precond.h): the static plan and the panel blob in HBM / L2
+// exact preconditioner (nd_precond.h): the static plan and the panel blob in HBM / L2
 struct KNd {
   int nphases;
   int max_ytiles, max_slots;       // shared-memory tiles / partial-sum slots the plan needs per step
@@ -68,17 +67,6 @@ struct KParams {
   const int *bcol;       // nb
   const double *bval;    // nb*16
   const double *dinv;    // n*16   block-Jacobi inverse blocks, may be null
-  const double *pinv;    // N*N    dense inverse of Q+0.1I, may be null
-  double *dense_part;    // grid * r * N  per-CTA partial products of the dense preconditioner
-  int dense_per;         // rows of pinv per CTA
-  int sym_ok;            // symmetric (upper-triangle) variant of the dense preconditioner is planned
-  const double *ppack;   // upper triangle of pinv, chunk-major: chunk = 8 rows x (padded width + 4) doubles, contiguous
-  const long long *sym_off; // nchunks+1: first double of every chunk in ppack
-  const int *sym_cut;    // grid+1: per-CTA range of chunk indices (segment-major order of (segment, 8-row group))
-  const int *sym_segptr; // nseg+1: first chunk index of every column segment
-  const int *sym_cfirst; // nseg: first CTA that touches the segment
-  const int *sym_ccount; // nseg: number of (consecutive) CTAs that touch it = partial panels of its columns
-  double *dense_t2;      // nseg x r x N transposed-product partials, slot = column segment
   const int *cta_rows;   // grid+1 balanced row partition
   const double *G;       // linear term r x N
   double *v[V_COUNT];
@@ -88,7 +76,7 @@ struct KParams {
   unsigned *bar_epoch;
   dpgo_opt_params_t prm;
   dpgo_opt_result_t *result;   // device copy of the result record
-  KNd nd;                // sparse exact preconditioner (nd.nphases == 0: not prepared)
+  KNd nd;                // the exact preconditioner prm.precond selects (nd.nphases == 0: not prepared)
   int cluster;           // 1: the whole grid is ONE thread-block cluster (<= 16 CTAs): phase ends use barrier.cluster
   int strict_acquire;    // 1: the grid barrier polls with ld.acquire (L1 invalidated every phase); 0: relaxed poll (default)
   int smem_doubles;      // dynamic shared memory of this launch, in doubles
@@ -143,13 +131,7 @@ cudaError_t launch_assemble_Q(int64_t nb, const int *cptr, const int2 *contrib, 
 cudaError_t launch_edge_weights(int r, int dh, int64_t m, const int *p1, const int *p2, const double *eT, const double *eom,
                                 const int *fixed, const double *X, int cost, double mu, double param, double *w, double *resid,
                                 unsigned long long *gnc, cudaStream_t stream);
-cudaError_t launch_pack_sym(const double *pinv, int N, int nchunks, const int *segptr, int nseg, const long long *off, double *ppack,
-                            cudaStream_t stream);
-cudaError_t launch_bsr_to_dense(int n, int dh, int64_t nb, const int *rowptr, const int *bcol, const double *bval,
-                                double shift, double *A, int N, cudaStream_t stream);
 
-// dense SPD inverse in place (dense_inverse.cu); A is N x N, ld = N, symmetric positive definite
-cudaError_t dense_spd_inverse(double *A, int N, cudaStream_t stream);
 // One matrix of a batched Gauss-Jordan sweep (dense_inverse.cu): A is M x M column-major (ld = M), swept over its pivots
 // [0, s); piv (32 x 32), Rw (32 x M) and C (M x 32) are its workspace.
 struct GjJob {
@@ -160,7 +142,7 @@ struct GjJob {
 // synchronisation.  A non-positive pivot sets *fail (nullable).
 cudaError_t gj_sweep_batch(const GjJob *jobs_dev, int njobs, int max_M, int max_s, int *fail, cudaStream_t stream);
 
-// ---- numeric refactorisation of the sparse exact preconditioner on the device (nd_refactor.cu) ----
+// ---- numeric refactorisation of the exact preconditioners on the device (nd_refactor.cu) ----
 // Device view of an nd::Refactor plus the buffers it fills; see nd_precond.h.
 struct KRefactor {
   int dh;

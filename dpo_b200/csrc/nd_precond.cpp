@@ -287,7 +287,8 @@ void chol_solve(const double *L, int s, double *B, int m) {
   }
 }
 
-// host version of DenseNodeOps::factor
+// dense algebra of one node.  in: Foo (s x s, row-major, SPD), Fob (s x b), Fbb (b x b);
+// out: W = Foo^-1 (s x s), Fm = W Fob (s x b), Fbb -= Fob^T Fm
 void host_factor(int s, int b, double *Foo, double *Fob, double *Fbb) {
   std::vector<double> L(Foo, Foo + (size_t)s * s);
   if (!chol_lower(L.data(), s)) throw std::runtime_error("nd: Schur complement not positive definite");
@@ -512,8 +513,7 @@ void build_hierarchy(const BsrView &Q, const Options &opt, Hierarchy &H) {
 // =================================================================================================================
 // 2. numeric
 // =================================================================================================================
-void build_numeric(const BsrView &Q, const Options &opt, Hierarchy &H, std::vector<double> &blob, DenseNodeOps *big_node,
-                   int big_threshold) {
+void build_numeric(const BsrView &Q, const Options &opt, Hierarchy &H, std::vector<double> &blob) {
   const int dh = H.dh;
   blob.assign((size_t)H.blob_doubles, 0.0);
   const size_t nn = H.nodes.size();
@@ -576,9 +576,7 @@ void build_numeric(const BsrView &Q, const Options &opt, Hierarchy &H, std::vect
       U[(size_t)c].clear();
       U[(size_t)c].shrink_to_fit();
     }
-    bool done = false;
-    if (big_node && s >= big_threshold) done = big_node->factor(s, b, Foo.data(), Fob.data(), Fbb.data());
-    if (!done) host_factor(s, b, Foo.data(), Fob.data(), Fbb.data());
+    host_factor(s, b, Foo.data(), Fob.data(), Fbb.data());
     if (b > 0) {
       U[(size_t)m].assign(Fbb.begin(), Fbb.begin() + (size_t)b * b);
     }

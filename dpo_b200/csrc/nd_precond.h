@@ -108,15 +108,8 @@ struct BsrView { int n; int dh; const int *rowptr; const int *bcol; const double
 
 // 1. ordering + macro levels (symbolic).  Throws std::runtime_error on impossible input.
 void build_hierarchy(const BsrView &Q, const Options &opt, Hierarchy &H);
-// 2. numeric: fills the panel blob (host, OpenMP over columns).  big_node (optional) may take over the dense algebra
-//    of one node (device offload); return false to let the host do it.
-struct DenseNodeOps {
-  // in: Foo (s x s, row-major, SPD), Fob (s x b), Fbb (b x b);  out: W = Foo^-1 (s x s), Fm = W Fob (s x b), Fbb -= Fob^T Fm
-  virtual bool factor(int s, int b, double *Foo, double *Fob, double *Fbb) = 0;
-  virtual ~DenseNodeOps() {}
-};
-void build_numeric(const BsrView &Q, const Options &opt, Hierarchy &H, std::vector<double> &blob, DenseNodeOps *big_node = nullptr,
-                   int big_threshold = 1 << 30);
+// 2. numeric: fills the panel blob (host, OpenMP over columns)
+void build_numeric(const BsrView &Q, const Options &opt, Hierarchy &H, std::vector<double> &blob);
 // 3. static work plan of every phase
 void build_plan(const Hierarchy &H, const Options &opt, Plan &P);
 // 4. residency: annotates the jobs (soff, nres) so that every CTA keeps at most budget_bytes of its panels in shared

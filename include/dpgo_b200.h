@@ -46,8 +46,8 @@ enum {
   DPGO_ERR_NO_DEVICE = 2,   /* no CUDA device / device index out of range */
   DPGO_ERR_CUDA = 3,        /* a CUDA runtime call or kernel failed */
   DPGO_ERR_STATE = 4,       /* call order violation (e.g. optimise before set_Q) */
-  DPGO_ERR_UNSUPPORTED = 5, /* d not in {2,3}; r outside the compiled set (d=3: 3..5, d=2: 2,3,5); N too large for
-                               the dense preconditioner */
+  DPGO_ERR_UNSUPPORTED = 5, /* d not in {2,3}; r outside the compiled set (d=3: 3..5, d=2: 2,3,5); an exact
+                               preconditioner whose blocks would exceed 24 GB (DENSE_EXACT: N above about 54k) */
   DPGO_ERR_ALLOC = 6
 };
 
@@ -57,12 +57,12 @@ enum { DPGO_ALG_RTR = 0, DPGO_ALG_RGD = 1 };
 
 /* Preconditioner used inside truncated CG.
  * ref: src/QuadraticProblem.cpp:31-42,75-87: exact solve with Q + 0.1 I (CHOLMOD) followed by
- * tangent projection.  DENSE_EXACT applies the same operator through a dense inverse resident
- * in HBM (per-iteration trace parity with the reference); BLOCK_JACOBI is the SpMV-only
- * throughput mode (same fixed points, different inner iterates); NONE is projection only.
- * SPARSE_EXACT applies the same operator as DENSE_EXACT through a nested-dissection block factorisation (dense
+ * tangent projection.  SPARSE_EXACT applies it through a nested-dissection block factorisation (dense
  * Schur-complement blocks on 2-4 macro levels, L2-resident for sphere2500-sized agents; O(n log n)-ish memory instead
- * of O(n^2)): the default, and what "exact" means everywhere below. */
+ * of O(n^2)): the default, and what "exact" means everywhere below.  DENSE_EXACT applies the same operator with the
+ * same block solve on a single macro level: the dense inverse of every connected component, 8 N^2 bytes in HBM
+ * streamed per application (an A/B reference for the default).  BLOCK_JACOBI is the SpMV-only throughput mode (same
+ * fixed points, different inner iterates); NONE is projection only. */
 enum { DPGO_PRECOND_NONE = 0, DPGO_PRECOND_BLOCK_JACOBI = 1, DPGO_PRECOND_DENSE_EXACT = 2, DPGO_PRECOND_SPARSE_EXACT = 3 };
 
 /* ref: ROPTLIB tCGstatusSet as recorded by src/QuadraticOptimizer.cpp:115 */
@@ -159,13 +159,12 @@ DPGO_API int dpgo_problem_set_edge_weights(dpgo_problem_t *p, const double *weig
  * robustOptInnerIters iterations (PGOAgent::iterate / updateLoopClosuresWeights / constructQMatrix + setQ,
  * src/PGOAgent.cpp:653-667, 1109-1112, 1174-1289).  These calls do it without a host copy or a synchronisation, on the
  * handle's stream: the same weights and the same k_assemble_Q as the synchronous calls above, then every prepared
- * preconditioner is refactorised ON THE DEVICE -- block-Jacobi (one 4x4 SPD inverse per pose) and the sparse exact one
- * (the multifrontal factorisation of its hierarchy, written into its panels in place).  Device buffers keep their
- * addresses and the handle's generation is not bumped, so a round graph captured before stays valid, and the calls can
- * themselves be captured into a CUDA graph, with two exceptions that synchronise (and so cannot be captured):
- *  - the first call after the sparse exact preconditioner's structure was dropped (set_edges, a synchronous re-weight) or
- *    never built builds its hierarchy and plan on the host, as its first use does;
- *  - a prepared dense exact preconditioner (the A/B switch) is dropped and rebuilt synchronously on its next use.
+ * preconditioner is refactorised ON THE DEVICE -- block-Jacobi (one 4x4 SPD inverse per pose) and the exact ones (the
+ * multifrontal factorisation of each hierarchy, written into its panels in place; a dense exact one not prepared yet is
+ * built on its first use).  Device buffers keep their addresses and the handle's generation is not bumped, so a round
+ * graph captured before stays valid, and the calls can themselves be captured into a CUDA graph, with one exception that
+ * synchronises (and so cannot be captured): the first call after the sparse exact preconditioner's structure was dropped
+ * (set_edges, a synchronous re-weight) or never built builds its hierarchy and plan on the host, as its first use does.
  * A front that is not positive definite (impossible for weights >= 0) sets a device flag that the next synchronising call
  * (dpgo_problem_sync, dpgo_optimize_result, dpgo_problem_gnc_counts, ...) reports as DPGO_ERR_CUDA.
  * weights_dev: m doubles in device memory on the handle's device, read in stream order. */
@@ -238,18 +237,9 @@ DPGO_API int dpgo_optimize_result(dpgo_problem_t *p, dpgo_opt_result_t *result);
 DPGO_API int dpgo_spmv_device(dpgo_problem_t *p, const double *X_dev, double *out_dev, int add_G);
 DPGO_API int64_t dpgo_spmv_algorithmic_bytes(const dpgo_problem_t *p, int add_G);
 /* bytes one application of the preconditioner (ref: QuadraticProblem::PreConditioner, src/QuadraticProblem.cpp:75-87)
- * has to move: the operator's unique data (upper triangle of the symmetric dense inverse when the symmetric
- * kernel is planned, i.e. after the first exact-mode optimise; the full matrix otherwise) + input and output vector */
+ * has to move: the operator's blocks + input and output vector.  An exact preconditioner reports 0 until it has been
+ * prepared (its first use); DENSE_EXACT then streams 8 N^2 bytes of blocks for a connected graph with an even n. */
 DPGO_API int64_t dpgo_precond_algorithmic_bytes(const dpgo_problem_t *p, int preconditioner);
-/* host only (no device needed): the work decomposition the symmetric dense apply uses for an N x N operator on `grid`
- * CTAs -- column segments of 480, 8-row groups, chunks in segment-major order.  segptr[nseg+1] = first chunk of every
- * segment, cut[grid+1] = chunk range of every CTA, cfirst/ccount[nseg] = the consecutive CTAs that touch a segment
- * (= partial-panel slots of its columns), chunk_offset[nchunks+1] = first double of every chunk in the packed upper
- * triangle.  chunk_cost <= 0 selects the built-in cost model.  DPGO_ERR_UNSUPPORTED when no plan exists for this size
- * (odd N, N < 2048, fewer chunks than CTAs); the library then streams the full matrix. */
-DPGO_API int dpgo_sym_plan_sizes(int N, int *num_segments, int *num_chunks);
-DPGO_API int dpgo_sym_plan(int N, int grid, double chunk_cost, int32_t *segptr, int32_t *cut, int32_t *cfirst,
-                           int32_t *ccount, int64_t *chunk_offset);
 /* ---- sparse exact preconditioner: diagnostics ------------------------------------------------------------------ */
 /* info[16] of the prepared hierarchy (prepares it if needed): 0 macro levels, 1 macro nodes, 2 phases per application,
  * 3 bytes of all blocks, 4 matrix bytes streamed per application, 5 largest own block (scalars), 6 largest boundary
@@ -269,12 +259,11 @@ DPGO_API int dpgo_nd_debug_emulate(int n, int d, int r, int64_t nb, const int32_
 DPGO_API int dpgo_debug_phase_latency(dpgo_problem_t *p, int phases, double *us_per_phase, double *us_launch);
 /* diagnostic: phase clock of the persistent kernel.  enable != 0 switches it on (subsequent optimise calls
  * accumulate, per phase kind, the nanoseconds CTA 0 spent up to the closing grid barrier); every call returns the
- * accumulated milliseconds in ms_by_kind[8] (0 eval pass, 1 dense preconditioner apply, 2 partial sums + projection,
- * 3 Hessian product, 4 tCG update, 5 retraction, 6 final, 7 unused) and resets them; enable == 0 switches it off. */
+ * accumulated milliseconds in ms_by_kind[8] (0 eval pass, 3 Hessian product, 4 tCG update, 5 retraction, 6 final;
+ * 1, 2 and 7 unused) and resets them; enable == 0 switches it off. */
 DPGO_API int dpgo_debug_phase_times(dpgo_problem_t *p, int enable, double *ms_by_kind);
-/* same with 32 slots: 0..7 as above (1 = the whole exact-preconditioner application when the dense inverse is used),
- * 8 + k = phase k of the sparse exact preconditioner's application (k < 16), 24 / 25 / 26 = gathers / panel jobs /
- * epilogues of those phases as seen by CTA 0, others unused */
+/* same with 32 slots: 0..7 as above, 8 + k = phase k of an exact preconditioner's application (k < 16; DENSE_EXACT
+ * has phase 0 only), 24 / 25 / 26 = gathers / panel jobs / epilogues of those phases as seen by CTA 0, others unused */
 DPGO_API int dpgo_debug_phase_times32(dpgo_problem_t *p, int enable, double *ms_by_kind);
 /* same with 64 slots: 32 + 3 k + {0, 1, 2} = gathers / panel jobs / epilogues of phase k (k < 10) as seen by CTA 0 */
 DPGO_API int dpgo_debug_phase_times64(dpgo_problem_t *p, int enable, double *ms_by_kind);

@@ -15,7 +15,7 @@ import torch
 import dpo_b200 as dp
 from dpo_b200 import posegraph as pg, _capi
 
-KINDS = ["eval", "dense_apply", "partial_sums_project", "hessian", "tcg_update", "retract", "final"]
+KINDS = ["eval", None, None, "hessian", "tcg_update", "retract", "final"]     # slots 1, 2: unused
 
 
 def main():
@@ -72,17 +72,19 @@ def main():
     _capi.check(prob._lib.dpgo_debug_phase_times64(prob._h, 0, ms))
     out = {"workload": f"{args.dataset} agent 0 of {args.agents} ({n} poses) r={args.rank} {args.precond}", "steps": args.steps,
            "ms_per_step_events": e0.elapsed_time(e1) / args.steps, "precond_applies": applies, "q_passes": passes,
-           "ms_per_step_by_kind": {k: ms[i] / args.steps for i, k in enumerate(KINDS) if ms[i] > 0},
-           "us_per_dense_apply": 1e3 * ms[1] / max(applies, 1), "us_per_partial_sum": 1e3 * ms[2] / max(applies, 1),
+           "ms_per_step_by_kind": {k: ms[i] / args.steps for i, k in enumerate(KINDS) if k and ms[i] > 0},
            "us_per_hessian": 1e3 * ms[3] / max(passes - 2 * args.steps, 1)}
     out["hessian_cta0_us"] = {"first_gather": 1e3 * ms[27] / max(passes - 2 * args.steps, 1), "whole_loop": 1e3 * ms[28] / max(passes - 2 * args.steps, 1)}
-    if args.precond == "exact":
-        out["nd"] = prob.nd_info()
-        out["us_per_apply_by_nd_phase"] = [1e3 * ms[8 + k] / max(applies, 1) for k in range(out["nd"]["phases"])]
+    if args.precond in ("exact", "dense"):
+        nphases = 1                                   # dense: the block solve's single macro level, one phase
+        if args.precond == "exact":
+            out["nd"] = prob.nd_info()
+            nphases = out["nd"]["phases"]
+        out["us_per_apply_by_nd_phase"] = [1e3 * ms[8 + k] / max(applies, 1) for k in range(nphases)]
         out["us_per_apply_cta0"] = {"gathers": 1e3 * ms[24] / max(applies, 1), "jobs": 1e3 * ms[25] / max(applies, 1),
                                     "epilogues": 1e3 * ms[26] / max(applies, 1)}
         out["us_per_apply_cta0_by_phase"] = [[round(1e3 * ms[32 + 3 * k + q] / max(applies, 1), 3) for q in range(3)]
-                                             for k in range(out["nd"]["phases"])]
+                                             for k in range(nphases)]
     print(json.dumps(out))
 
 

@@ -23,7 +23,7 @@ from dpo_b200 import posegraph as pg
 SPMV_GROUP_BLOCKS = 192      # blocks per row group of the TMA-fed Q.X product; a longer row sends it to the gather kernel
 SP_CACHE_INTS = 2048         # a CTA's block-CSR slice (rows + 1 + blocks) beyond this is read from global memory
 ND_YCAP_TILES = 600          # shared-memory tile capacity of one nested-dissection step (larger leaves: column chunks)
-DENSE_MAX_N = 12000          # the dense-inverse preconditioner is exercised up to this N ((d+1) n)
+DENSE_MAX_N = 12000          # the dense exact preconditioner (one macro level) is exercised up to this N ((d+1) n)
 U = 2.0 ** -53               # unit roundoff of float64
 
 RANKS = {3: (3, 4, 5), 2: (2, 3, 5)}   # every compiled relaxation rank per d
@@ -163,7 +163,7 @@ def make_case(name: str, d: int, seed: int = 0) -> Case:
     elif name == "clique700":
         n = 700 if d == 3 else 701
         pairs = _clique(n)
-        target = "ND leaf > ND_YCAP_TILES; dense N = 2800 (symmetric plan) / 2103 (odd: non-TMA dense apply)"
+        target = "ND leaf > ND_YCAP_TILES; n even (N = 2800) and odd (N = 2103: the last panel half used)"
     elif name == "multi_edges":
         (n, pairs), target = _multi_edges(rng), "duplicated and reversed edges, both directions, random sparse part"
     elif name == "long_chain":
@@ -201,11 +201,6 @@ def tma_groups(row_blocks, bt=SPMV_GROUP_BLOCKS):
 def zero_byte_index_groups(groups):
     """Groups without blocks whose first block index is a multiple of 4: their index window is empty."""
     return [g for g in (groups or []) if g[2] == g[3] and g[2] % 4 == 0]
-
-
-def dense_variant(N):
-    """Which dense apply the persistent kernel takes for DENSE_EXACT (dpgo_kernels.cu: TMA only for even N >= 2048)."""
-    return "tma" if (N % 2 == 0 and N >= 2048) else "plain"
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -73,8 +73,6 @@ def test_manifold_ops(ds, r, data_dir):
     assert relerr(gp.project(M), orc.manifold_project(M, d)) <= 1e-12
 
 
-# sphere2500 (N = 10000) and parking-garage (N = 6644 = 4 mod 8: ragged last row group and last segment) take the
-# symmetric packed-upper-triangle apply, the others the plain dense apply
 @pytest.mark.parametrize("ds,r", [("tinyGrid3D", 3), ("smallGrid3D", 5), ("sphere2500", 5), ("CSAIL", 5),
                                   ("parking-garage", 3), ("sphere2500", 4)])
 def test_preconditioners(ds, r, data_dir):
@@ -83,36 +81,37 @@ def test_preconditioners(ds, r, data_dir):
     V = rng.standard_normal(X.shape)
     exact = op.precondition(X, V)
     assert relerr(gp.PreConditioner(X, V, dp.PRECOND_SPARSE_EXACT), exact) <= 1e-11      # nested-dissection block solve (default)
-    assert relerr(gp.PreConditioner(X, V, dp.PRECOND_DENSE_EXACT), exact) <= 1e-9        # dense inverse (A/B)
+    assert relerr(gp.PreConditioner(X, V, dp.PRECOND_DENSE_EXACT), exact) <= 1e-9        # one macro level (A/B)
     oo = orc.QuadraticOptimizer(op, precond="jacobi")
     assert relerr(gp.PreConditioner(X, V, dp.PRECOND_BLOCK_JACOBI), oo._apply_precond(X, V)) <= 1e-12
     assert relerr(gp.PreConditioner(X, V, dp.PRECOND_NONE), orc.tangent_project(X, V, op.d)) <= 1e-13
 
 
-def test_precond_bytes_and_phase_clock(data_dir):
-    """dpgo_precond_algorithmic_bytes reports the unique bytes of the operator (upper triangle once the symmetric
-    apply is planned); dpgo_debug_phase_times accumulates per-phase time of the persistent kernel."""
+def test_dense_exact_bytes_and_phase_clock(data_dir):
+    """dpgo_precond_algorithmic_bytes reports the bytes of the operator's blocks once it is prepared (the dense inverse
+    of the connected sphere2500 graph); dpgo_debug_phase_times32 accumulates per-phase time of the persistent kernel."""
     import ctypes as C
     import dpo_b200 as dp
     from dpo_b200 import _capi
     op, gp, X, rng = make_problem("sphere2500", 5, data_dir, with_G=False)
     n, N, vec = op.n, X.shape[1], X.size * 8
     assert gp.precond_algorithmic_bytes(dp.PRECOND_BLOCK_JACOBI) == n * 128 + 2 * vec
-    assert gp.precond_algorithmic_bytes(dp.PRECOND_DENSE_EXACT) == 8 * N * N + 2 * vec       # nothing planned yet
+    assert gp.precond_algorithmic_bytes(dp.PRECOND_DENSE_EXACT) == 0                         # nothing prepared yet
     gp.PreConditioner(X, rng.standard_normal(X.shape), dp.PRECOND_DENSE_EXACT)
-    assert gp.precond_algorithmic_bytes(dp.PRECOND_DENSE_EXACT) == 4 * N * (N + 8) + 2 * vec
-    ms = (C.c_double * 8)()
-    _capi.check(gp._lib.dpgo_debug_phase_times(gp._h, 1, ms))
+    assert gp.precond_algorithmic_bytes(dp.PRECOND_DENSE_EXACT) == 8 * N * N + 2 * vec
+    ms = (C.c_double * 32)()
+    _capi.check(gp._lib.dpgo_debug_phase_times32(gp._h, 1, ms))
     opt = dp.QuadraticOptimizer(gp)
     opt.setTrustRegionIterations(1)
     opt.setTrustRegionMaxInnerIterations(5)
     opt.setPreconditioner(dp.PRECOND_DENSE_EXACT)
     opt.optimize(X)
     res = opt.getOptResult()
-    _capi.check(gp._lib.dpgo_debug_phase_times(gp._h, 0, ms))
-    assert ms[0] > 0 and ms[1] > 0 and ms[2] > 0 and ms[3] > 0                                # eval, dense, sums, Hessian
-    assert sum(ms[:7]) <= res.elapsed_ms * 1.5 + 1.0
-    _capi.check(gp._lib.dpgo_debug_phase_times(gp._h, 0, ms))                                 # switched off: zeros
+    _capi.check(gp._lib.dpgo_debug_phase_times32(gp._h, 0, ms))
+    assert ms[0] > 0 and ms[8] > 0 and ms[3] > 0                                              # eval, dense apply, Hessian
+    assert ms[1] == 0 and ms[2] == 0 and ms[9] == 0                                           # one phase per application
+    assert sum(ms[:24]) <= res.elapsed_ms * 1.5 + 1.0
+    _capi.check(gp._lib.dpgo_debug_phase_times32(gp._h, 0, ms))                               # switched off: zeros
     assert all(v == 0.0 for v in ms)
 
 

@@ -313,7 +313,7 @@ def test_no_stale_host_copy_after_async(data_dir):
     w = seeded_weights(len(edges), 4)
     gp.setEdgeWeightsAsync(torch.tensor(w, dtype=torch.float64, device="cuda"))
     ref = lu_precondition(gp, meas, w, n, X, V)
-    assert relerr(gp.PreConditioner(X, V, PRECOND_DENSE_EXACT), ref) <= 1e-10   # rebuilt from the new Q
+    assert relerr(gp.PreConditioner(X, V, PRECOND_DENSE_EXACT), ref) <= 1e-10   # refactorised from the new Q
     assert relerr(gp.PreConditioner(X, V), ref) <= 1e-10
     # a later synchronous re-weight behaves as on a handle that never saw the asynchronous path
     w2 = seeded_weights(len(edges), 6)
@@ -323,3 +323,39 @@ def test_no_stale_host_copy_after_async(data_dir):
     assert np.array_equal(gp.EucGrad(X), fresh.EucGrad(X))
     for p in pc:
         assert np.array_equal(gp.PreConditioner(X, V, p), fresh.PreConditioner(X, V, p)), p
+
+
+@pytest.mark.gpu
+def test_dense_exact_refactorised_by_a_captured_reweight(data_dir):
+    """A prepared dense exact preconditioner is refactorised in place by the asynchronous re-weight, like the sparse one:
+    after one eager call the call captures into a CUDA graph, and after a replay with new weights DENSE_EXACT applies the
+    re-weighted operator with no further setup."""
+    import torch
+    from dpo_b200._capi import PRECOND_BLOCK_JACOBI, PRECOND_DENSE_EXACT, PRECOND_SPARSE_EXACT
+    edges, meas, n = load("smallGrid3D", data_dir)
+    fixed = odometry_flags(edges)
+    rng = np.random.default_rng(17)
+    X = orc.manifold_project(rng.standard_normal((5, 4 * n)), 3)
+    V = rng.standard_normal(X.shape)
+    gp = make_problem(edges, n, fixed, precond=(PRECOND_BLOCK_JACOBI, PRECOND_DENSE_EXACT, PRECOND_SPARSE_EXACT))
+    gp.PreConditioner(X, V, PRECOND_DENSE_EXACT)                 # the dense exact preconditioner prepared
+    prepared = gp.precond_algorithmic_bytes(PRECOND_DENSE_EXACT)
+    assert prepared > 0
+    w = torch.tensor(seeded_weights(len(edges), 8), dtype=torch.float64, device="cuda")
+    gp.setEdgeWeightsAsync(w)                                     # eager: builds the sparse exact structure
+    gp.sync()
+    s = torch.cuda.Stream()
+    gp.set_stream(s.cuda_stream)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g, stream=s):
+        gp.setEdgeWeightsAsync(w)
+    w2 = seeded_weights(len(edges), 9)
+    w.copy_(torch.tensor(w2, dtype=torch.float64, device="cuda"))
+    g.replay()
+    torch.cuda.synchronize()
+    gp.set_stream(None)
+    gp.sync()
+    assert gp.precond_algorithmic_bytes(PRECOND_DENSE_EXACT) == prepared        # still prepared: nothing to rebuild
+    ref = lu_precondition(gp, meas, w2, n, X, V)
+    assert relerr(gp.PreConditioner(X, V, PRECOND_DENSE_EXACT), ref) <= 1e-10
+    assert relerr(gp.PreConditioner(X, V), ref) <= 1e-10

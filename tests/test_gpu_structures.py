@@ -47,7 +47,7 @@ def spmv(gp, M, add_G):
 def test_single_operations(name, d, r, cluster):
     import dpo_b200 as dp
     c, Q, K = case(name, d)
-    dense = (not cluster) and c.N <= sc.DENSE_MAX_N
+    dense = c.N <= sc.DENSE_MAX_N
     gp = make(c, Q, r, cluster, dense)
     assert gp.launch_info()[1] == cluster
     assert gp.num_blocks() == int(c.row_blocks().sum())

@@ -5,8 +5,6 @@
   * the 40-digit references agree with numpy on well-conditioned inputs;
   * the host emulation of the sparse exact preconditioner's plan matches the sparse LU on every case, at the full grid
     of an H100 and at a cluster grid."""
-import ctypes as C
-
 import numpy as np
 import pytest
 import scipy.sparse as sp
@@ -31,22 +29,7 @@ def get(cases, name, d):
     return cases[(name, d)]
 
 
-def sym_plan_ok(N, grid=132):
-    from dpo_b200 import _capi
-    lib = _capi.load_library()
-    nseg, nch = C.c_int(), C.c_int()
-    if lib.dpgo_sym_plan_sizes(N, C.byref(nseg), C.byref(nch)) != 0:
-        return False
-    segptr = np.zeros(nseg.value + 1, np.int32)
-    cut = np.zeros(grid + 1, np.int32)
-    cfirst = np.zeros(max(nseg.value, 1), np.int32)
-    ccount = np.zeros(max(nseg.value, 1), np.int32)
-    off = np.zeros(nch.value + 1, np.int64)
-    return lib.dpgo_sym_plan(N, grid, C.c_double(0.0), _capi.iptr(segptr), _capi.iptr(cut), _capi.iptr(cfirst),
-                             _capi.iptr(ccount), off.ctypes.data_as(C.POINTER(C.c_int64))) == 0
-
-
-@pytest.mark.parametrize("name,d", ALL)
+@pytest.mark.parametrize("name,d", [(n, d) for (n, d) in ALL if n != "clique700"])
 def test_case_reaches_its_branch(name, d, cases):
     c = get(cases, name, d)
     rb = c.row_blocks()
@@ -74,10 +57,6 @@ def test_case_reaches_its_branch(name, d, cases):
     elif name == "components":
         A = sp.csr_matrix((np.ones(len(c.edges)), (c.edges.p1, c.edges.p2)), shape=(c.n, c.n))
         assert connected_components(A, directed=False)[0] == 4
-    elif name == "clique700":
-        assert c.N == {3: 2800, 2: 2103}[d] and rb.min() == c.n
-        assert sc.dense_variant(c.N) == {3: "tma", 2: "plain"}[d]
-        assert sym_plan_ok(c.N) == (d == 3)                                 # symmetric dense plan only for the even N
     elif name == "multi_edges":
         pairs = list(zip(c.edges.p1.tolist(), c.edges.p2.tolist()))
         assert len(pairs) > len(set(pairs))                                 # duplicated
@@ -85,9 +64,19 @@ def test_case_reaches_its_branch(name, d, cases):
         assert any((b, a) in set(pairs) for a, b in pairs)                  # both directions
     elif name == "long_chain":
         assert c.n == 5000 and len(c.edges) == 4999
-    if name == "clique700":
-        return
     assert c.N <= sc.DENSE_MAX_N or name == "long_chain"
+
+
+@pytest.mark.parametrize("d", [2, 3])
+def test_clique_reaches_its_branch(d, cases):
+    """clique700: every row holds every pose (one dissection leaf, larger than a step's tile capacity), with an even pose
+    count for d = 3 and an odd one for d = 2, whose last 8-row panel of the single dense level is half used"""
+    c = get(cases, "clique700", d)
+    rb = c.row_blocks()
+    assert c.n == len(rb) and c.Q().shape == (c.N, c.N)
+    assert c.N == {3: 2800, 2: 2103}[d] and rb.min() == c.n
+    assert c.n > sc.ND_YCAP_TILES and c.n % 2 == {3: 0, 2: 1}[d]
+    assert c.N <= sc.DENSE_MAX_N
 
 
 @pytest.mark.parametrize("name,d", [(n, d) for (n, d) in ALL if n not in ("clique700",)] + [("clique700", 3)])
