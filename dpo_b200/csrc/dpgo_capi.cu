@@ -1620,6 +1620,14 @@ int dpgo_optimize_resident_from_aux_async(dpgo_problem_t *p, const dpgo_opt_para
 
 namespace {
 
+// The batched calls keep per-agent device state (ticket counters, partial sums, momentum records) that one launch must not
+// touch twice: an agent listed twice would share its ticket between two jobs and could leave it non-zero for good.
+bool handles_distinct(dpgo_problem_t *const *agents, int count) {
+  std::vector<const dpgo_problem_t *> h(agents, agents + count);
+  std::sort(h.begin(), h.end());
+  return std::adjacent_find(h.begin(), h.end()) == h.end();
+}
+
 struct StreamSwap {                        // the handle's work goes to another stream for the duration of a call
   dpgo_problem *p; cudaStream_t saved;
   StreamSwap(dpgo_problem *q, cudaStream_t to) : p(q), saved(q->stream) { q->stream = to; }
@@ -1760,6 +1768,7 @@ int dpgo_agents_round_async(dpgo_problem_t *const *agents, int num_active, const
                             int pack_after_join) {
   DPGO_REQUIRE(num_active >= 0 && (num_active == 0 || (agents && send_dev)) && params, DPGO_ERR_INVALID_ARG, "bad arguments");
   if (num_active == 0) return DPGO_OK;
+  DPGO_REQUIRE(handles_distinct(agents, num_active), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
   cudaStream_t main = nullptr;
   bool graph = false;
   DPGO_TRY(round_preamble(agents, num_active, params, main_stream, main, graph));
@@ -2063,6 +2072,7 @@ int dpgo_agents_status_async(dpgo_problem_t *const *agents, int count, const int
   std::sort(sorted.begin(), sorted.end());
   DPGO_REQUIRE(sorted[0] >= 0, DPGO_ERR_INVALID_ARG, "negative status slot");
   DPGO_REQUIRE(std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end(), DPGO_ERR_INVALID_ARG, "duplicate status slot");
+  DPGO_REQUIRE(handles_distinct(agents, count), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
   std::vector<uint64_t> key;
   key.reserve(3 * (size_t)count + 1);
   for (int i = 0; i < count; ++i) {
@@ -2143,6 +2153,7 @@ int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, cons
                "momentum_N must be >= 1 and restart_interval >= 1");
   dpgo_problem *lead = agents[0];
   DPGO_REQUIRE(lead, DPGO_ERR_INVALID_ARG, "null problem handle");
+  DPGO_REQUIRE(handles_distinct(agents, count), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
   std::vector<uint64_t> key;
   key.reserve(5 * (size_t)count);
   for (int i = 0; i < count; ++i) {
@@ -2225,6 +2236,7 @@ int dpgo_agents_accel_round_async(dpgo_problem_t *const *agents, int num_active,
   DPGO_TRY(require_device());
   DPGO_REQUIRE(num_active >= 0 && (num_active == 0 || agents) && params, DPGO_ERR_INVALID_ARG, "bad arguments");
   if (num_active == 0) return DPGO_OK;
+  DPGO_REQUIRE(handles_distinct(agents, num_active), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
   for (int i = 0; i < num_active; ++i) {
     DPGO_CHECK_HANDLE(agents[i]);
     DPGO_ACC_READY(agents[i]);
@@ -2294,6 +2306,7 @@ int dpgo_agents_select_round_async(dpgo_problem_t *const *agents, int count, con
   DPGO_REQUIRE(count > 0 && agents && agent_index && params && records_dev && send_dev, DPGO_ERR_INVALID_ARG, "bad arguments");
   dpgo_problem *lead = agents[0];
   DPGO_CHECK_HANDLE(lead);
+  DPGO_REQUIRE(handles_distinct(agents, count), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
   DPGO_REQUIRE(lead->sel.k > 0, DPGO_ERR_STATE, "dpgo_agents_set_agent_graph has not been called for the first agent");
   std::vector<char> seen((size_t)lead->sel.k, 0);
   for (int i = 0; i < count; ++i) {

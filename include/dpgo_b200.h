@@ -324,7 +324,8 @@ DPGO_API int dpgo_optimize_resident_from_aux_async(dpgo_problem_t *p, const dpgo
  * main_stream NULL = the stream the first handle is set to.  pack_after_join != 0 issues the packs in a second pass,
  * after every agent's step (needed when neighbouring agents are active in the same round and send_dev aliases
  * gathered_dev).  A repeated round of cluster agents is replayed as a CUDA graph; a round with a full-grid agent is issued
- * eagerly (a cooperative launch does not capture).  DPGO_ROUND_GRAPH=0 keeps the eager launches. */
+ * eagerly (a cooperative launch does not capture).  DPGO_ROUND_GRAPH=0 keeps the eager launches.  A handle listed twice
+ * is refused with DPGO_ERR_INVALID_ARG. */
 DPGO_API int dpgo_agents_round_async(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
                             const double *gathered_dev, int64_t num_slots, double *const *send_dev, void *main_stream,
                             int pack_after_join);
@@ -342,8 +343,8 @@ DPGO_API int dpgo_agents_host_io_async(dpgo_problem_t *const *agents, int count,
  * finishes its iterate(false): X = Y, V = proj(V + gamma (X - Y)), and on a restart round ((iterations + 1) %
  * restart_interval == 0) X = XPrev, V = Y = X, gamma = alpha = 0.  Then every agent's public tiles of X and Y go to
  * send_dev[i] and send_aux_dev[i].  One launch on `stream` (NULL: the first agent's).  Calls that share an agent must be
- * ordered (one ticket counter per agent).  Job tables are kept per agent list and active set, as for
- * dpgo_agents_status_async. */
+ * ordered (one ticket counter per agent), and a handle listed twice in one call is refused with DPGO_ERR_INVALID_ARG.
+ * Job tables are kept per agent list and active set, as for dpgo_agents_status_async. */
 DPGO_API int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, const int32_t *active_flags,
                                            double momentum_N, int restart_interval, double *const *send_dev,
                                            double *const *send_aux_dev, void *stream);
@@ -355,7 +356,7 @@ DPGO_API int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int co
  * its status record (dpgo_agents_status_async) gets [3] = sqrt(|X - XPrev|^2 / n), X the iterate after the V update and
  * any restart, XPrev the iterate at the round's begin, and [4] = the count at the begin + 1, on plain and restart rounds
  * alike.  Agents idle in the round keep their fields [3] and [4].  Nothing is packed.  A repeated round is replayed as a CUDA graph (two variants per active set: plain and restart);
- * DPGO_ROUND_GRAPH=0 keeps the eager launches. */
+ * DPGO_ROUND_GRAPH=0 keeps the eager launches.  A handle listed twice is refused with DPGO_ERR_INVALID_ARG. */
 DPGO_API int dpgo_agents_accel_round_async(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
                                            const double *gathered_dev, const double *gathered_aux_dev, int64_t num_slots,
                                            void *main_stream);
@@ -406,7 +407,8 @@ DPGO_API int dpgo_robust_single_rotation_averaging(int device, int d, int m, con
  * status_dev + slot[i] * DPGO_STATUS_DOUBLES (device memory; slots distinct).  An agent's record depends only on that
  * agent (fixed work split and reduction order), bit for bit.  Asynchronous on `stream` (NULL: the first agent's).
  * Each agent has one partial-sum buffer and one ticket counter: two status calls that include the same agent must be
- * ordered (one stream, or an event between them), as the round calls of one agent must be.
+ * ordered (one stream, or an event between them), as the round calls of one agent must be.  For the same reason a handle
+ * listed twice in one call (under two slots) is refused with DPGO_ERR_INVALID_ARG: its two jobs would share the ticket.
  * The first call with a given agent list (and status_dev) uploads its job table and keeps it with the first agent; a
  * repeated call is a single kernel launch, which a CUDA graph can capture.  A first call cannot be captured.  Up to 32
  * tables are kept per first agent; a 33rd list synchronises the device and frees the oldest table, so a graph that
@@ -434,12 +436,15 @@ DPGO_API int dpgo_agents_set_agent_graph(dpgo_problem_t *lead, int num_agents, c
  * dpgo_agents_status_async writes them): agents in decreasing |rgrad|^2 (field 2), ties to the lower id, each taken unless a
  * neighbour already is.  The k-byte mask is appended to lead's selection log.  Then, as dpgo_agents_round_async with
  * pack_after_join = 0, every listed agent's G rebuild -> step -> pack into send_dev[i]; the kernels of an agent left out
- * return at entry and touch nothing (iterate, G, tiles, result record, status fields 3 and 4).
+ * return at entry and touch nothing (iterate, G, tiles, result record, status fields 3 and 4).  The exception is a G clear
+ * still pending from dpgo_problem_set_G_*, dpgo_agent_set_shared_edges or dpgo_problem_device_G: it is issued from the
+ * host, before the mask exists, so it runs for a left-out agent too.
  * Ordering: the records must be complete on `stream` before the call (e.g. the status launch, or the all-gather of the
  * records, issued earlier on the same stream); the calls that share a lead must be ordered.  A repeated call of cluster
  * agents with the same buffers is replayed as a CUDA graph (the selection is device data, so one graph serves every set;
  * the log's doubling starts a new one); a call with a full-grid agent is issued eagerly, and a left-out full-grid agent
- * still costs its launches.  This call is itself never captured by the caller's graph: the log can grow on the host. */
+ * still costs its launches.  This call is itself never captured by the caller's graph: the log can grow on the host.
+ * Agent indices must be distinct, and so must the handles: either repeated is refused with DPGO_ERR_INVALID_ARG. */
 DPGO_API int dpgo_agents_select_round_async(dpgo_problem_t *const *agents, int count, const int32_t *agent_index,
                                             const dpgo_opt_params_t *params, const double *records_dev,
                                             const double *gathered_dev, int64_t num_slots, double *const *send_dev,
