@@ -123,7 +123,6 @@ SIGNATURES = {
     "dpgo_agent_accel_restart_begin": (C.c_int, [_vp]),
     "dpgo_agent_accel_restart_end": (C.c_int, [_vp]),
     "dpgo_agent_pack_public_aux": (C.c_int, [_vp, _vp]),
-    "dpgo_optimize_resident_from_aux_async": (C.c_int, [_vp, C.POINTER(OptParams)]),
     "dpgo_agents_round_async": (C.c_int, [C.POINTER(_vp), C.c_int, C.POINTER(OptParams), _vp, C.c_int64, C.POINTER(_vp), _vp,
                                           C.c_int]),
     "dpgo_agents_accel_begin_async": (C.c_int, [C.POINTER(_vp), C.c_int, _ip, C.c_double, C.c_int, C.POINTER(_vp),

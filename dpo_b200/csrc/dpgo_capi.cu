@@ -60,7 +60,7 @@ struct dpgo_problem {
   int device = 0, sms = 0, grid = 0, max_grid = 0, max_cluster = 0;
   bool cluster = false;          // the persistent kernel runs as ONE thread-block cluster (small agents)
   cudaStream_t stream = nullptr;
-  dpgo::Event ev_done, ev_fork;  // fork / join of dpgo_agents_round_async
+  dpgo::Event ev_done, ev_fork;  // fork / join of the batched calls (fan_out)
   uint64_t generation = 0;       // bumped whenever device buffers a captured round refers to may have been replaced
   struct RoundGraph { std::vector<uint64_t> key; dpgo::GraphExec exec; int uses = 0; bool failed = false; };
   std::vector<RoundGraph> round_graphs;      // CUDA graphs of the batched round / host I/O calls, kept by the call's first agent
@@ -141,9 +141,9 @@ struct dpgo_problem {
   } align;
   DevBuf<double> T_align;
   DevBuf<int> align_info;
-  DevBuf<dpgo::AlignJob> align_jobs;       // per-call tables of dpgo_agents_align_async (kept by the call's first agent)
+  std::vector<JobTable<dpgo::AlignJob>> align_tables;   // job tables of dpgo_agents_align_async, kept by the call's first agent
   DevBuf<int> ready;
-  int jobs_cap = 0, ready_cap = 0;
+  int ready_cap = 0;
   dpgo::Event ev_align;                    // recorded on the stream of the last dpgo_agents_align_async that aligned this agent
   // team status (dpgo_status.cu): last optimising call's relative change + count, per-CTA partials, ticket of the last CTA
   struct Status {
@@ -1609,23 +1609,58 @@ int dpgo_agent_pack_public_aux(dpgo_problem_t *p, double *send_dev) {
   DPGO_CUDA(dpgo::launch_pack_tiles(p->ts, p->pub.num, p->pub.pose.get(), p->acc.vec[0].get(), send_dev, p->stream));
   return DPGO_OK;
 }
-int dpgo_optimize_resident_from_aux_async(dpgo_problem_t *p, const dpgo_opt_params_t *params) {
-  DPGO_CHECK_HANDLE(p);
-  DPGO_ACC_READY(p);
-  DPGO_CUDA(cudaMemcpyAsync(p->vec[dpgo::V_X0].get(), p->acc.vec[0].get(), p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
-  return dpgo_optimize_resident_async(p, params);
-}
 
 }  // extern "C"
 
 namespace {
 
-// The batched calls keep per-agent device state (ticket counters, partial sums, momentum records) that one launch must not
-// touch twice: an agent listed twice would share its ticket between two jobs and could leave it non-zero for good.
-bool handles_distinct(dpgo_problem_t *const *agents, int count) {
+int require_device() {
+  int count = 0;
+  if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
+    cudaGetLastError();
+    return fail(DPGO_ERR_NO_DEVICE, "no CUDA device available: the GPU path has no CPU fallback");
+  }
+  return DPGO_OK;
+}
+
+// The agent list of a batched call: at least one handle, none null, all on the first one's device (made current) and, for
+// the calls that serve every agent with one launch (same_shape), all with its d and r.  The handles must be distinct: the
+// batched calls keep per-agent device state (ticket counters, partial sums, momentum records, alignment buffers) that one
+// call must not touch twice; an agent listed twice would share its ticket between two jobs and could leave it non-zero
+// for good.
+int check_agents(dpgo_problem_t *const *agents, int count, bool same_shape) {
+  DPGO_TRY(require_device());
+  DPGO_REQUIRE(agents && count >= 1, DPGO_ERR_INVALID_ARG, "no agents");
+  const dpgo_problem *lead = agents[0];
+  for (int i = 0; i < count; ++i) {
+    const dpgo_problem *p = agents[i];
+    DPGO_REQUIRE(p, DPGO_ERR_INVALID_ARG, "null problem handle");
+    DPGO_REQUIRE(p->device == lead->device, DPGO_ERR_INVALID_ARG, "the agents of one call must live on one device");
+    DPGO_REQUIRE(!same_shape || (p->d == lead->d && p->r == lead->r), DPGO_ERR_INVALID_ARG,
+                 "the agents of one call must share d and r");
+  }
   std::vector<const dpgo_problem_t *> h(agents, agents + count);
   std::sort(h.begin(), h.end());
-  return std::adjacent_find(h.begin(), h.end()) == h.end();
+  DPGO_REQUIRE(std::adjacent_find(h.begin(), h.end()) == h.end(), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
+  DPGO_CUDA(cudaSetDevice(lead->device));
+  return DPGO_OK;
+}
+
+// The stream a batched call works on: `stream`, or for NULL the stream the first agent is set to.
+cudaStream_t call_stream(const dpgo_problem *lead, void *stream) { return stream ? (cudaStream_t)stream : lead->stream; }
+
+// What a call that fans out over its agents (fan_out) needs: its stream, the first agent's fork event and every agent's
+// join event; and whether the call may be replayed as a CUDA graph: not on the legacy default stream, which cannot be
+// captured, nor with DPGO_ROUND_GRAPH=0.
+int fan_out_stream(dpgo_problem_t *const *agents, int count, void *stream, cudaStream_t &main, bool &graph) {
+  static const bool enabled = [] { const char *e = std::getenv("DPGO_ROUND_GRAPH"); return !e || std::atoi(e) != 0; }();
+  dpgo_problem *lead = agents[0];
+  main = call_stream(lead, stream);
+  graph = enabled && main != cudaStreamLegacy && main != nullptr;
+  if (!lead->ev_fork) DPGO_CUDA(dpgo::create_event(lead->ev_fork));
+  for (int i = 0; i < count; ++i)
+    if (!agents[i]->ev_done) DPGO_CUDA(dpgo::create_event(agents[i]->ev_done));
+  return DPGO_OK;
 }
 
 struct StreamSwap {                        // the handle's work goes to another stream for the duration of a call
@@ -1633,6 +1668,25 @@ struct StreamSwap {                        // the handle's work goes to another 
   StreamSwap(dpgo_problem *q, cudaStream_t to) : p(q), saved(q->stream) { q->stream = to; }
   ~StreamSwap() { p->stream = saved; }
 };
+
+// Issues body(i, agents[i]) for every agent with the handle set to stream_of(agent): an agent on a stream of its own works
+// between a fork from `main` and a join into it, side by side with the others; an agent on `main` works in list order.
+template <class StreamOf, class Body>
+int fan_out(dpgo_problem_t *const *agents, int count, cudaStream_t main, StreamOf stream_of, Body body) {
+  dpgo_problem *lead = agents[0];
+  DPGO_CUDA(cudaEventRecord(lead->ev_fork.get(), main));
+  for (int i = 0; i < count; ++i) {
+    dpgo_problem *p = agents[i];
+    StreamSwap swap(p, stream_of(p));
+    if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork.get(), 0));
+    DPGO_TRY(body(i, p));
+    if (p->stream != main) {
+      DPGO_CUDA(cudaEventRecord(p->ev_done.get(), p->stream));
+      DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done.get(), 0));
+    }
+  }
+  return DPGO_OK;
+}
 
 // Replay a repeated multi-launch sequence as a CUDA graph.  The graphs live with `lead` (the first agent of the call),
 // keyed by everything the captured launches depend on.  First use: eager (warms every lazily created resource);
@@ -1679,50 +1733,75 @@ template <class Issue> int replay_or_issue(dpgo_problem *lead, const std::vector
   return DPGO_OK;
 }
 
-// DPGO_ROUND_GRAPH=0 keeps the eager launches of every call that would otherwise replay a CUDA graph
-bool round_graphs_enabled() {
-  static const bool on = [] { const char *e = std::getenv("DPGO_ROUND_GRAPH"); return !e || std::atoi(e) != 0; }();
-  return on;
-}
+constexpr size_t JOB_TABLES_MAX = 32;
 
-// What the round calls check and prepare alike: every handle on the first one's device, with valid parameters and a join
-// event; the first handle's fork event; the stream the round forks from and joins into (main_stream, NULL: the stream the
-// first handle is set to); whether the round may be replayed as a CUDA graph.
-int round_preamble(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params, void *main_stream,
-                   cudaStream_t &main, bool &graph) {
-  graph = round_graphs_enabled();
-  for (int i = 0; i < num_active; ++i) {
-    dpgo_problem *p = agents[i];
-    DPGO_CHECK_HANDLE(p);
-    DPGO_REQUIRE(p->device == agents[0]->device, DPGO_ERR_INVALID_ARG, "the agents of a round must live on one device");
-    DPGO_TRY(check_params(p, params));
-    if (!p->ev_done) DPGO_CUDA(dpgo::create_event(p->ev_done));
-    // a cooperative launch does not capture; a pending G clear or an unbuilt factorisation must run eagerly first
-    const int slot = nd_slot(params->precond);
-    if (!p->cluster || p->G_dirty || p->phase_ns || ((p->bsr.precond_mask & (1u << nd_precond(slot))) && !p->nd[slot].ready))
-      graph = false;
+// The job table of an agent list is filled (fill(jobs) returns the CTA count) and uploaded once, stream-ordered, and kept in
+// `tables` under `key`; a repeated call finds it, so the call is its kernel launches and nothing else and can be captured
+// into a CUDA graph.  Past JOB_TABLES_MAX tables the oldest is freed.
+template <class Job, class Fill>
+int job_table(std::vector<dpgo_problem::JobTable<Job>> &tables, std::vector<uint64_t> &key, int count, cudaStream_t st,
+              Fill fill, const dpgo_problem::JobTable<Job> *&tab) {
+  for (const auto &t : tables)
+    if (t.key == key) { tab = &t; return DPGO_OK; }
+  if (tables.size() >= JOB_TABLES_MAX) {                   // a table may still be read by a launch in flight
+    DPGO_CUDA(cudaDeviceSynchronize());
+    tables.erase(tables.begin());
   }
-  dpgo_problem *lead = agents[0];
-  main = main_stream ? (cudaStream_t)main_stream : lead->stream;
-  DPGO_CUDA(cudaSetDevice(lead->device));
-  if (!lead->ev_fork) DPGO_CUDA(dpgo::create_event(lead->ev_fork));
-  if (main == cudaStreamLegacy || main == nullptr) graph = false;   // the legacy default stream cannot be captured
+  std::vector<Job> jobs((size_t)count);
+  const int ctas = fill(jobs);
+  DevBuf<Job> d_jobs;
+  DPGO_CUDA(d_jobs.assign(jobs.data(), jobs.size(), st));
+  tables.push_back({std::move(key), std::move(d_jobs), ctas});
+  tab = &tables.back();
   return DPGO_OK;
 }
 
-// The start of a round graph's key: a tag that keeps the keys of different calls apart, the stream, the slot count, the
-// parameters, every agent's handle and generation.  The caller appends the buffers its launches capture.
-std::vector<uint64_t> round_key(uint64_t tag, dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
-                                cudaStream_t main, int64_t num_slots) {
-  uint64_t w[(sizeof(*params) + 7) / 8] = {};
-  std::memcpy(w, params, sizeof(*params));
-  std::vector<uint64_t> key{tag, (uint64_t)(uintptr_t)main, (uint64_t)num_slots};
-  key.insert(key.end(), w, w + sizeof(w) / 8);
+// What the round calls prepare alike after check_agents: valid parameters for every agent, the call's stream and events,
+// and whether the round may be replayed as a CUDA graph.
+int round_preamble(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params, void *main_stream,
+                   cudaStream_t &main, bool &graph) {
+  bool capturable = true;
   for (int i = 0; i < num_active; ++i) {
+    dpgo_problem *p = agents[i];
+    DPGO_TRY(check_params(p, params));
+    // a cooperative launch does not capture; a pending G clear or an unbuilt factorisation must run eagerly first
+    const int slot = nd_slot(params->precond);
+    if (!p->cluster || p->G_dirty || p->phase_ns || ((p->bsr.precond_mask & (1u << nd_precond(slot))) && !p->nd[slot].ready))
+      capturable = false;
+  }
+  DPGO_TRY(fan_out_stream(agents, num_active, main_stream, main, graph));
+  graph = graph && capturable;
+  return DPGO_OK;
+}
+
+// The start of every key a batched call keeps a CUDA graph or a job table under: a tag that keeps the keys of different
+// calls apart, then every agent's handle and generation.  The caller appends whatever else its cached work depends on.
+std::vector<uint64_t> call_key(uint64_t tag, dpgo_problem_t *const *agents, int count) {
+  std::vector<uint64_t> key{tag};
+  for (int i = 0; i < count; ++i) {
     key.push_back((uint64_t)(uintptr_t)agents[i]);
     key.push_back(agents[i]->generation);
   }
   return key;
+}
+
+// The start of a round graph's key: call_key, the stream, the slot count and the parameters.  The caller appends the
+// buffers its launches capture.
+std::vector<uint64_t> round_key(uint64_t tag, dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
+                                cudaStream_t main, int64_t num_slots) {
+  uint64_t w[(sizeof(*params) + 7) / 8] = {};
+  std::memcpy(w, params, sizeof(*params));
+  std::vector<uint64_t> key = call_key(tag, agents, num_active);
+  key.push_back((uint64_t)(uintptr_t)main);
+  key.push_back((uint64_t)num_slots);
+  key.insert(key.end(), w, w + sizeof(w) / 8);
+  return key;
+}
+
+// The stream_of of the round calls' fan_out: cluster agents step side by side on their own streams, full-grid agents in
+// order on main.
+auto round_streams(cudaStream_t main) {
+  return [main](const dpgo_problem *p) { return p->cluster ? p->own_stream.get() : main; };
 }
 
 }  // namespace
@@ -1732,24 +1811,15 @@ extern "C" {
 static int issue_round(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
                        const double *gathered_dev, int64_t num_slots, double *const *send_dev, cudaStream_t main,
                        int pack_after_join) {
-  dpgo_problem *lead = agents[0];
   const int passes = pack_after_join ? 2 : 1;
   for (int pass = 0; pass < passes; ++pass) {
-    DPGO_CUDA(cudaEventRecord(lead->ev_fork.get(), main));
-    for (int i = 0; i < num_active; ++i) {
-      dpgo_problem *p = agents[i];
-      StreamSwap swap(p, p->cluster ? p->own_stream.get() : main);   // cluster steps side by side, full-grid steps in order
-      if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork.get(), 0));
+    DPGO_TRY(fan_out(agents, num_active, main, round_streams(main), [&](int i, dpgo_problem *p) -> int {
       if (pass == 0) {
         DPGO_TRY(dpgo_agent_build_G(p, gathered_dev, num_slots));
         DPGO_TRY(dpgo_optimize_resident_async(p, params));
       }
-      if (pass == passes - 1) DPGO_TRY(dpgo_agent_pack_public(p, send_dev[i]));
-      if (p->stream != main) {
-        DPGO_CUDA(cudaEventRecord(p->ev_done.get(), p->stream));
-        DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done.get(), 0));
-      }
-    }
+      return pass == passes - 1 ? dpgo_agent_pack_public(p, send_dev[i]) : DPGO_OK;
+    }));
   }
   return DPGO_OK;
 }
@@ -1766,9 +1836,9 @@ static int issue_round(dpgo_problem_t *const *agents, int num_active, const dpgo
 int dpgo_agents_round_async(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
                             const double *gathered_dev, int64_t num_slots, double *const *send_dev, void *main_stream,
                             int pack_after_join) {
-  DPGO_REQUIRE(num_active >= 0 && (num_active == 0 || (agents && send_dev)) && params, DPGO_ERR_INVALID_ARG, "bad arguments");
+  DPGO_REQUIRE(num_active >= 0 && (num_active == 0 || send_dev) && params, DPGO_ERR_INVALID_ARG, "bad arguments");
   if (num_active == 0) return DPGO_OK;
-  DPGO_REQUIRE(handles_distinct(agents, num_active), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
+  DPGO_TRY(check_agents(agents, num_active, false));
   cudaStream_t main = nullptr;
   bool graph = false;
   DPGO_TRY(round_preamble(agents, num_active, params, main_stream, main, graph));
@@ -1787,53 +1857,30 @@ int dpgo_agents_round_async(dpgo_problem_t *const *agents, int num_active, const
 // all on `stream`; a repeated call (same agents, buffers, stream) is replayed as a CUDA graph of memcpy / kernel nodes.
 int dpgo_agents_host_io_async(dpgo_problem_t *const *agents, int count, double *const *X_host, double *const *send_dev,
                               int direction, void *stream) {
-  DPGO_REQUIRE(count >= 0 && (count == 0 || (agents && X_host)) && (direction == 0 || direction == 1), DPGO_ERR_INVALID_ARG,
+  DPGO_REQUIRE(count >= 0 && (count == 0 || X_host) && (direction == 0 || direction == 1), DPGO_ERR_INVALID_ARG,
                "bad arguments");
   if (count == 0) return DPGO_OK;
-  for (int i = 0; i < count; ++i) {
-    DPGO_CHECK_HANDLE(agents[i]);
-    DPGO_REQUIRE(X_host[i], DPGO_ERR_INVALID_ARG, "null host buffer");
-    DPGO_REQUIRE(agents[i]->device == agents[0]->device, DPGO_ERR_INVALID_ARG, "the agents of a call must live on one device");
-  }
-  dpgo_problem *lead = agents[0];
-  cudaStream_t main = stream ? (cudaStream_t)stream : lead->stream;
-  DPGO_CUDA(cudaSetDevice(lead->device));
-  if (!lead->ev_fork) DPGO_CUDA(dpgo::create_event(lead->ev_fork));
-  for (int i = 0; i < count; ++i)
-    if (!agents[i]->ev_done) DPGO_CUDA(dpgo::create_event(agents[i]->ev_done));
-  auto issue = [&]() -> int {
-    // every agent's copy (+ pack) on its own stream between a fork from and a join into `main`: the copies of different
-    // agents overlap each other and the packs
-    DPGO_CUDA(cudaEventRecord(lead->ev_fork.get(), main));
-    for (int i = 0; i < count; ++i) {
-      dpgo_problem *p = agents[i];
-      StreamSwap swap(p, p->own_stream.get());
-      if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork.get(), 0));
-      if (direction == 0) {
-        DPGO_TRY(upload_vec(p, dpgo::V_X0, X_host[i]));
-        if (send_dev && send_dev[i]) DPGO_TRY(dpgo_agent_pack_public(p, send_dev[i]));
-      } else {
-        DPGO_TRY(download_vec(p, dpgo::V_X0, X_host[i]));
-      }
-      if (p->stream != main) {
-        DPGO_CUDA(cudaEventRecord(p->ev_done.get(), p->stream));
-        DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done.get(), 0));
-      }
-    }
-    return DPGO_OK;
+  DPGO_TRY(check_agents(agents, count, false));
+  for (int i = 0; i < count; ++i) DPGO_REQUIRE(X_host[i], DPGO_ERR_INVALID_ARG, "null host buffer");
+  cudaStream_t main = nullptr;
+  bool graph = false;
+  DPGO_TRY(fan_out_stream(agents, count, stream, main, graph));
+  // every agent's copy (+ pack) on its own stream: the copies of different agents overlap each other and the packs
+  auto issue = [&]() {
+    return fan_out(agents, count, main, [](dpgo_problem *p) { return p->own_stream.get(); }, [&](int i, dpgo_problem *p) -> int {
+      if (direction == 1) return download_vec(p, dpgo::V_X0, X_host[i]);
+      DPGO_TRY(upload_vec(p, dpgo::V_X0, X_host[i]));
+      return send_dev && send_dev[i] ? dpgo_agent_pack_public(p, send_dev[i]) : DPGO_OK;
+    });
   };
-  if (!round_graphs_enabled() || main == cudaStreamLegacy || main == nullptr) return issue();
-  std::vector<uint64_t> key;
-  key.reserve(3 * (size_t)count + 4);
-  key.push_back(0x696f0000ull + (uint64_t)direction);       // "io": never equal to a round key (those start with another tag)
+  if (!graph) return issue();
+  std::vector<uint64_t> key = call_key(0x696f0000ull + (uint64_t)direction, agents, count);   // "io"
   for (int i = 0; i < count; ++i) {
-    key.push_back((uint64_t)(uintptr_t)agents[i]);
-    key.push_back(agents[i]->generation);
     key.push_back((uint64_t)(uintptr_t)X_host[i]);
     key.push_back((uint64_t)(uintptr_t)((send_dev && direction == 0) ? send_dev[i] : nullptr));
   }
   key.push_back((uint64_t)(uintptr_t)main);
-  return replay_or_issue(lead, key, main, issue);
+  return replay_or_issue(agents[0], key, main, issue);
 }
 
 int dpgo_agent_f_rgradnorm_resident(dpgo_problem_t *p, double *f_out, double *norm_out) {
@@ -1851,18 +1898,8 @@ int dpgo_agent_f_rgradnorm_resident(dpgo_problem_t *p, double *f_out, double *no
 
 // ---- distributed initialisation: frame alignment -------------------------------------------------------
 namespace {
-int ensure_jobs(dpgo_problem *p, int jobs, int ready) {
-  if (jobs > p->jobs_cap) {
-    DPGO_CUDA(p->align_jobs.alloc((size_t)jobs));
-    p->jobs_cap = jobs;
-  }
-  if (ready > p->ready_cap) {
-    DPGO_CUDA(p->ready.alloc((size_t)ready));
-    p->ready_cap = ready;
-  }
-  return DPGO_OK;
-}
-
+// Every buffer an AlignJob points to is allocated once, except the candidate table's: dpgo_agent_set_align_candidates
+// replaces those and bumps the handle's generation, so a kept job table never points to freed memory.
 dpgo::AlignJob align_job(const dpgo_problem *p) {
   const dpgo_problem::Align &A = p->align;
   dpgo::AlignJob J = {};
@@ -1886,12 +1923,12 @@ int dpgo_agent_set_local_trajectory(dpgo_problem_t *p, const double *T_host, con
   if (!p->ylift) DPGO_CUDA(p->ylift.alloc(yn));
   DPGO_CUDA(p->Tloc.upload(T_host, tn, p->stream));
   DPGO_CUDA(p->ylift.upload(YLift_host, yn, p->stream));
-  DPGO_TRY(ensure_jobs(p, 1, 0));
   dpgo::AlignJob J = align_job(p);
   J.T_align = nullptr;                     // identity: X = YLift T
   J.info = nullptr;
-  DPGO_CUDA(p->align_jobs.upload(&J, 1, p->stream));
-  DPGO_CUDA(dpgo::launch_frame_lift(p->d, p->r, 1, p->n, p->align_jobs.get(), p->stream));
+  DevBuf<dpgo::AlignJob> job;
+  DPGO_CUDA(job.assign(&J, 1, p->stream));
+  DPGO_CUDA(dpgo::launch_frame_lift(p->d, p->r, 1, p->n, job.get(), p->stream));
   DPGO_CUDA(cudaStreamSynchronize(p->stream));
   return DPGO_OK;
 }
@@ -1914,6 +1951,7 @@ int dpgo_agent_set_align_candidates(dpgo_problem_t *p, int num_groups, const int
                  "candidate index out of range");
     max_slot = std::max(max_slot, (int)nbr_slot[q]);
   }
+  ++p->generation;                         // the job tables of dpgo_agents_align_async point into the old candidate table
   p->align = {};
   p->align.groups = num_groups;
   p->align.cands = m;
@@ -1940,34 +1978,37 @@ int dpgo_agent_set_align_candidates(dpgo_problem_t *p, int num_groups, const int
 
 int dpgo_agents_align_async(dpgo_problem_t *const *agents, int count, const double *gathered_dev, int64_t num_slots,
                             const int32_t *ready_host, int num_agents, void *stream) {
-  DPGO_REQUIRE(agents && count >= 1 && agents[0], DPGO_ERR_INVALID_ARG, "no agents to align");
+  DPGO_TRY(check_agents(agents, count, true));
   DPGO_REQUIRE(ready_host && num_agents >= 1, DPGO_ERR_INVALID_ARG, "null ready flags");
   dpgo_problem *lead = agents[0];
-  DPGO_CHECK_HANDLE(lead);
-  std::vector<dpgo::AlignJob> jobs((size_t)count);
   int max_cands = 0, max_poses = 0;
   for (int i = 0; i < count; ++i) {
     dpgo_problem *p = agents[i];
-    DPGO_REQUIRE(p && p->device == lead->device && p->d == lead->d && p->r == lead->r, DPGO_ERR_INVALID_ARG,
-                 "the agents of one align call must share the device, d and r");
     DPGO_REQUIRE(p->Tloc && p->T_align, DPGO_ERR_STATE,
                  "dpgo_agent_set_local_trajectory and dpgo_agent_set_align_candidates must be called first");
     DPGO_REQUIRE(p->align.cands == 0 || (gathered_dev && p->align.max_slot < num_slots), DPGO_ERR_INVALID_ARG,
                  "a candidate refers to a slot beyond the gathered buffer");
     DPGO_REQUIRE(p->align.max_nbr < num_agents, DPGO_ERR_INVALID_ARG, "a candidate group names an agent beyond the ready flags");
     if (!p->ev_align) DPGO_CUDA(dpgo::create_event(p->ev_align));
-    jobs[(size_t)i] = align_job(p);
     max_cands = std::max(max_cands, p->align.cands);
     max_poses = std::max(max_poses, p->n);
   }
-  cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
-  DPGO_TRY(ensure_jobs(lead, count, num_agents));
-  DPGO_CUDA(lead->align_jobs.upload(jobs.data(), jobs.size(), st));
-  DPGO_CUDA(lead->ready.upload(ready_host, (size_t)num_agents, st));
-  DPGO_CUDA(dpgo::launch_align_candidates(lead->d, lead->r, count, max_cands, lead->align_jobs.get(), gathered_dev, st));
-  DPGO_CUDA(dpgo::launch_robust_rotation_average(lead->d, count, lead->align_jobs.get(), lead->ready.get(),
+  const cudaStream_t st = call_stream(lead, stream);
+  std::vector<uint64_t> key = call_key(0x616c6e0000ull, agents, count);   // "aln"
+  const dpgo_problem::JobTable<dpgo::AlignJob> *tab = nullptr;
+  DPGO_TRY(job_table(lead->align_tables, key, count, st, [&](std::vector<dpgo::AlignJob> &jobs) {
+    for (int i = 0; i < count; ++i) jobs[(size_t)i] = align_job(agents[i]);
+    return 0;                              // the align launches size their grids by count, max_cands and max_poses
+  }, tab));
+  if (num_agents > lead->ready_cap) {
+    DPGO_CUDA(lead->ready.alloc((size_t)num_agents));
+    lead->ready_cap = num_agents;
+  }
+  DPGO_CUDA(lead->ready.upload(ready_host, (size_t)num_agents, st));   // the flags change every wave
+  DPGO_CUDA(dpgo::launch_align_candidates(lead->d, lead->r, count, max_cands, tab->jobs.get(), gathered_dev, st));
+  DPGO_CUDA(dpgo::launch_robust_rotation_average(lead->d, count, tab->jobs.get(), lead->ready.get(),
                                                  2.0 * std::sqrt(2.0) * std::sin(0.25), st));
-  DPGO_CUDA(dpgo::launch_frame_lift(lead->d, lead->r, count, max_poses, lead->align_jobs.get(), st));
+  DPGO_CUDA(dpgo::launch_frame_lift(lead->d, lead->r, count, max_poses, tab->jobs.get(), st));
   for (int i = 0; i < count; ++i) DPGO_CUDA(cudaEventRecord(agents[i]->ev_align.get(), st));   // dpgo_agent_align_result waits on it
   return DPGO_OK;
 }
@@ -2027,66 +2068,20 @@ int dpgo_robust_single_rotation_averaging(int device, int d, int m, const double
 }  // extern "C"
 
 // ---- team status and rounding (dpgo_status.cu) ---------------------------------------------------------------------------
-namespace {
-int require_device() {
-  int count = 0;
-  if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
-    cudaGetLastError();
-    return fail(DPGO_ERR_NO_DEVICE, "no CUDA device available: the GPU path has no CPU fallback");
-  }
-  return DPGO_OK;
-}
-constexpr size_t STATUS_TABLES_MAX = 32;
-
-// The job table of an agent list is filled (fill(jobs) returns the CTA count) and uploaded once, stream-ordered, and kept in
-// `tables` under `key`; a repeated call finds it, so the call is one kernel launch and nothing else and can be captured into
-// a CUDA graph.  Past STATUS_TABLES_MAX tables the oldest is freed.
-template <class Job, class Fill>
-int job_table(std::vector<dpgo_problem::JobTable<Job>> &tables, std::vector<uint64_t> &key, int count, cudaStream_t st,
-              Fill fill, const dpgo_problem::JobTable<Job> *&tab) {
-  for (const auto &t : tables)
-    if (t.key == key) { tab = &t; return DPGO_OK; }
-  if (tables.size() >= STATUS_TABLES_MAX) {                // a table may still be read by a launch in flight
-    DPGO_CUDA(cudaDeviceSynchronize());
-    tables.erase(tables.begin());
-  }
-  std::vector<Job> jobs((size_t)count);
-  const int ctas = fill(jobs);
-  DevBuf<Job> d_jobs;
-  DPGO_CUDA(d_jobs.assign(jobs.data(), jobs.size(), st));
-  tables.push_back({std::move(key), std::move(d_jobs), ctas});
-  tab = &tables.back();
-  return DPGO_OK;
-}
-}  // namespace
-
 extern "C" {
 
 int dpgo_agents_status_async(dpgo_problem_t *const *agents, int count, const int32_t *slot, double *status_dev, void *stream) {
-  DPGO_TRY(require_device());
-  DPGO_REQUIRE(agents && slot && status_dev, DPGO_ERR_INVALID_ARG, "null agents, slots or status buffer");
-  DPGO_REQUIRE(count > 0, DPGO_ERR_INVALID_ARG, "count must be positive");
+  DPGO_TRY(check_agents(agents, count, true));
+  DPGO_REQUIRE(slot && status_dev, DPGO_ERR_INVALID_ARG, "null slots or status buffer");
   dpgo_problem *lead = agents[0];
-  DPGO_REQUIRE(lead, DPGO_ERR_INVALID_ARG, "null problem handle");
   std::vector<int32_t> sorted(slot, slot + count);
   std::sort(sorted.begin(), sorted.end());
   DPGO_REQUIRE(sorted[0] >= 0, DPGO_ERR_INVALID_ARG, "negative status slot");
   DPGO_REQUIRE(std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end(), DPGO_ERR_INVALID_ARG, "duplicate status slot");
-  DPGO_REQUIRE(handles_distinct(agents, count), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
-  std::vector<uint64_t> key;
-  key.reserve(3 * (size_t)count + 1);
-  for (int i = 0; i < count; ++i) {
-    const dpgo_problem *p = agents[i];
-    DPGO_REQUIRE(p, DPGO_ERR_INVALID_ARG, "null problem handle");
-    DPGO_REQUIRE(p->device == lead->device && p->d == lead->d && p->r == lead->r, DPGO_ERR_INVALID_ARG,
-                 "the agents of one status call must share the device, d and r");
-    key.push_back((uint64_t)(uintptr_t)p);
-    key.push_back(p->generation);
-    key.push_back((uint64_t)slot[i]);
-  }
+  std::vector<uint64_t> key = call_key(0x7374730000ull, agents, count);   // "sts"
+  key.insert(key.end(), slot, slot + count);
   key.push_back((uint64_t)(uintptr_t)status_dev);
-  DPGO_CUDA(cudaSetDevice(lead->device));
-  cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
+  const cudaStream_t st = call_stream(lead, stream);
   const dpgo_problem::JobTable<dpgo::StatusJob> *tab = nullptr;
   DPGO_TRY(job_table(lead->status.tables, key, count, st, [&](std::vector<dpgo::StatusJob> &jobs) {
     int ctas = 0;
@@ -2145,34 +2140,23 @@ int dpgo_copy_to_host_async(int device, void *dst_host, const void *src_dev, siz
 // ---- accelerated rounds (dpgo_accel.cu) ------------------------------------------------------------------------------------
 int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, const int32_t *active_flags, double momentum_N,
                                   int restart_interval, double *const *send_dev, double *const *send_aux_dev, void *stream) {
-  DPGO_TRY(require_device());
-  DPGO_REQUIRE(agents && active_flags && send_dev && send_aux_dev, DPGO_ERR_INVALID_ARG,
-               "null agents, active flags or send buffers");
-  DPGO_REQUIRE(count > 0, DPGO_ERR_INVALID_ARG, "count must be positive");
+  DPGO_TRY(check_agents(agents, count, true));
+  DPGO_REQUIRE(active_flags && send_dev && send_aux_dev, DPGO_ERR_INVALID_ARG, "null active flags or send buffers");
   DPGO_REQUIRE(momentum_N >= 1.0 && restart_interval >= 1, DPGO_ERR_INVALID_ARG,
                "momentum_N must be >= 1 and restart_interval >= 1");
   dpgo_problem *lead = agents[0];
-  DPGO_REQUIRE(lead, DPGO_ERR_INVALID_ARG, "null problem handle");
-  DPGO_REQUIRE(handles_distinct(agents, count), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
-  std::vector<uint64_t> key;
-  key.reserve(5 * (size_t)count);
+  std::vector<uint64_t> key = call_key(0x6163620000ull, agents, count);   // "acb"
   for (int i = 0; i < count; ++i) {
     const dpgo_problem *p = agents[i];
-    DPGO_REQUIRE(p, DPGO_ERR_INVALID_ARG, "null problem handle");
-    DPGO_REQUIRE(p->device == lead->device && p->d == lead->d && p->r == lead->r, DPGO_ERR_INVALID_ARG,
-                 "the agents of one accelerated call must share the device, d and r");
     DPGO_ACC_READY(p);
     DPGO_REQUIRE(p->pub.slot && p->pub.slot_unique, DPGO_ERR_STATE,
                  "the agent needs a public pose list without duplicates (dpgo_agent_set_public_poses)");
     DPGO_REQUIRE(p->pub.num == 0 || (send_dev[i] && send_aux_dev[i]), DPGO_ERR_INVALID_ARG, "null send buffer");
-    key.push_back((uint64_t)(uintptr_t)p);
-    key.push_back(p->generation);
     key.push_back((uint64_t)(active_flags[i] != 0));
     key.push_back((uint64_t)(uintptr_t)send_dev[i]);
     key.push_back((uint64_t)(uintptr_t)send_aux_dev[i]);
   }
-  DPGO_CUDA(cudaSetDevice(lead->device));
-  cudaStream_t st = stream ? (cudaStream_t)stream : lead->stream;
+  const cudaStream_t st = call_stream(lead, stream);
   const dpgo_problem::JobTable<dpgo::AccelJob> *tab = nullptr;
   DPGO_TRY(job_table(lead->acc.tables, key, count, st, [&](std::vector<dpgo::AccelJob> &jobs) {
     int ctas = 0;
@@ -2203,13 +2187,8 @@ int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, cons
 
 static int issue_accel_round(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
                              const double *gathered_dev, const double *gathered_aux_dev, int64_t num_slots, cudaStream_t main) {
-  dpgo_problem *lead = agents[0];
-  DPGO_CUDA(cudaEventRecord(lead->ev_fork.get(), main));
-  for (int i = 0; i < num_active; ++i) {
-    dpgo_problem *p = agents[i];
-    StreamSwap swap(p, p->cluster ? p->own_stream.get() : main);   // cluster steps side by side, full-grid steps in order
+  return fan_out(agents, num_active, main, round_streams(main), [&](int, dpgo_problem *p) -> int {
     double *X = p->vec[dpgo::V_X0].get(), *Y = p->acc.vec[0].get(), *V = p->acc.vec[1].get(), *XP = p->acc.vec[2].get();
-    if (p->stream != main) DPGO_CUDA(cudaStreamWaitEvent(p->stream, lead->ev_fork.get(), 0));
     DPGO_TRY(dpgo_agent_build_G(p, gathered_aux_dev, num_slots));
     DPGO_CUDA(cudaMemcpyAsync(X, Y, p->vec_bytes(), cudaMemcpyDeviceToDevice, p->stream));
     DPGO_TRY(dpgo_optimize_resident_async(p, params));
@@ -2222,23 +2201,17 @@ static int issue_accel_round(dpgo_problem_t *const *agents, int num_active, cons
       DPGO_CUDA(dpgo::launch_accel_finish(p->r, p->dh, p->n, X, Y, V, XP, p->acc.state.get(), dpgo::ACCEL_FINISH_RESTART_END,
                                           p->acc.part.get(), p->acc.ticket.get() + 1, p->status.opt_record.get(), p->stream));
     }
-    if (p->stream != main) {
-      DPGO_CUDA(cudaEventRecord(p->ev_done.get(), p->stream));
-      DPGO_CUDA(cudaStreamWaitEvent(main, p->ev_done.get(), 0));
-    }
-  }
-  return DPGO_OK;
+    return DPGO_OK;
+  });
 }
 
 int dpgo_agents_accel_round_async(dpgo_problem_t *const *agents, int num_active, const dpgo_opt_params_t *params,
                                   const double *gathered_dev, const double *gathered_aux_dev, int64_t num_slots,
                                   void *main_stream) {
-  DPGO_TRY(require_device());
-  DPGO_REQUIRE(num_active >= 0 && (num_active == 0 || agents) && params, DPGO_ERR_INVALID_ARG, "bad arguments");
+  DPGO_REQUIRE(num_active >= 0 && params, DPGO_ERR_INVALID_ARG, "bad arguments");
   if (num_active == 0) return DPGO_OK;
-  DPGO_REQUIRE(handles_distinct(agents, num_active), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
+  DPGO_TRY(check_agents(agents, num_active, false));
   for (int i = 0; i < num_active; ++i) {
-    DPGO_CHECK_HANDLE(agents[i]);
     DPGO_ACC_READY(agents[i]);
     DPGO_REQUIRE(agents[i]->acc.state && agents[i]->acc.rounds > 0, DPGO_ERR_STATE,
                  "dpgo_agents_accel_begin_async has not been called");
@@ -2302,11 +2275,9 @@ struct GateSet {                           // every agent of a round reads its b
 int dpgo_agents_select_round_async(dpgo_problem_t *const *agents, int count, const int32_t *agent_index,
                                    const dpgo_opt_params_t *params, const double *records_dev, const double *gathered_dev,
                                    int64_t num_slots, double *const *send_dev, void *stream) {
-  DPGO_TRY(require_device());
-  DPGO_REQUIRE(count > 0 && agents && agent_index && params && records_dev && send_dev, DPGO_ERR_INVALID_ARG, "bad arguments");
+  DPGO_TRY(check_agents(agents, count, false));
+  DPGO_REQUIRE(agent_index && params && records_dev && send_dev, DPGO_ERR_INVALID_ARG, "bad arguments");
   dpgo_problem *lead = agents[0];
-  DPGO_CHECK_HANDLE(lead);
-  DPGO_REQUIRE(handles_distinct(agents, count), DPGO_ERR_INVALID_ARG, "an agent is listed twice");
   DPGO_REQUIRE(lead->sel.k > 0, DPGO_ERR_STATE, "dpgo_agents_set_agent_graph has not been called for the first agent");
   std::vector<char> seen((size_t)lead->sel.k, 0);
   for (int i = 0; i < count; ++i) {

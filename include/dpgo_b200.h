@@ -315,8 +315,6 @@ DPGO_API int dpgo_agent_accel_restart_begin(dpgo_problem_t *p);             /* X
 DPGO_API int dpgo_agent_accel_restart_end(dpgo_problem_t *p);               /* V = Y = X */
 /* public tiles of the auxiliary iterate Y (ref getAuxSharedPoseDict, :107-118) */
 DPGO_API int dpgo_agent_pack_public_aux(dpgo_problem_t *p, double *send_dev);
-/* X = Y, then optimise X in place (ref updateX(true, true): the step starts from the auxiliary iterate) */
-DPGO_API int dpgo_optimize_resident_from_aux_async(dpgo_problem_t *p, const dpgo_opt_params_t *params);
 /* One RBCD round of the active agents of one GPU with one call (ref: the body of the round loop,
  * examples/MultiRobotExample.cpp:229-334: updateNeighborPoses -> iterate() -> getSharedPoseDict per selected agent).
  * Per agent: G rebuild from gathered_dev -> RTR step -> pack of its public tiles into send_dev[i] (thread-block cluster
@@ -332,7 +330,8 @@ DPGO_API int dpgo_agents_round_async(dpgo_problem_t *const *agents, int num_acti
 /* The host boundary of a round with one call per direction (ref: the host matrices PGOAgent::setX / getX move,
  * src/PGOAgent.cpp:66-93): direction 0 = X of every listed agent from (pinned) host memory, then its public tiles packed
  * into send_dev[i] (send_dev may be NULL); direction 1 = X back to host memory.  Asynchronous on `stream` (NULL: the
- * stream the first handle is set to); a repeated call is replayed as a CUDA graph. */
+ * stream the first handle is set to); a repeated call is replayed as a CUDA graph.  A handle listed twice is refused with
+ * DPGO_ERR_INVALID_ARG. */
 DPGO_API int dpgo_agents_host_io_async(dpgo_problem_t *const *agents, int count, double *const *X_host,
                               double *const *send_dev, int direction, void *stream);
 /* ---- accelerated rounds with one call per GPU (ref src/PGOAgent.cpp:685-695,1033-1091; examples/MultiRobotExample.cpp:
@@ -344,7 +343,7 @@ DPGO_API int dpgo_agents_host_io_async(dpgo_problem_t *const *agents, int count,
  * restart_interval == 0) X = XPrev, V = Y = X, gamma = alpha = 0.  Then every agent's public tiles of X and Y go to
  * send_dev[i] and send_aux_dev[i].  One launch on `stream` (NULL: the first agent's).  Calls that share an agent must be
  * ordered (one ticket counter per agent), and a handle listed twice in one call is refused with DPGO_ERR_INVALID_ARG.
- * Job tables are kept per agent list and active set, as for dpgo_agents_status_async. */
+ * Job tables are kept per agent list, active set and send buffers, as for dpgo_agents_status_async. */
 DPGO_API int dpgo_agents_accel_begin_async(dpgo_problem_t *const *agents, int count, const int32_t *active_flags,
                                            double momentum_N, int restart_interval, double *const *send_dev,
                                            double *const *send_aux_dev, void *stream);
@@ -383,7 +382,9 @@ DPGO_API int dpgo_agent_set_align_candidates(dpgo_problem_t *p, int num_groups, 
  * 369-440: one call per GPU and wave aligns `count` agents of one device against the gathered public tiles.  Per agent
  * the groups whose neighbour has ready_host[neighbour] != 0 are tried in order (GNC-TLS rotation averaging at the
  * threshold 2 sqrt(2) sin(0.25), ~30 degrees, then the mean translation of the inliers); the first with inliers moves
- * the trajectory into the global frame: X = YLift (T_align T).  Asynchronous on `stream` (NULL: the first agent's). */
+ * the trajectory into the global frame: X = YLift (T_align T).  Asynchronous on `stream` (NULL: the first agent's).
+ * A handle listed twice is refused with DPGO_ERR_INVALID_ARG.  Job tables are kept per agent list, as for
+ * dpgo_agents_status_async; the ready flags are uploaded on every call. */
 DPGO_API int dpgo_agents_align_async(dpgo_problem_t *const *agents, int count, const double *gathered_dev, int64_t num_slots,
                                      const int32_t *ready_host, int num_agents, void *stream);
 /* the agent's last alignment (waits for the stream of the align call that included the agent): T_align (d x (d+1) column-major, nullable) and info4 =

@@ -362,12 +362,19 @@ def test_rotation_averaging(d, m):
 # a handle listed twice
 # ---------------------------------------------------------------------------------------------------------------------
 def test_duplicate_handles_refused():
-    """The five batched calls refuse one handle listed twice (two jobs would share its ticket counter); the agent's next
-    status record is bitwise the one before, so its ticket was not touched."""
+    """The seven batched calls refuse one handle listed twice (two jobs would share its ticket counter, or write its
+    alignment buffers and X at once) and enqueue nothing: the agent's iterate is unchanged and its next status record is
+    bitwise the one before, so its ticket was not touched."""
     import torch
     L, cp = lib(), capi()
     a = ac.Agent(3, 5, 1100, 3)                              # 35 status CTAs
     gp = handle(a)
+    T = np.asfortranarray(np.tile(np.hstack([np.eye(3), np.zeros((3, 1))]), (1, a.n)))
+    Y = np.asfortranarray(orc.fixed_stiefel_variable(3, 5))
+    # the align call's state is set, so only the duplicate can refuse it; X = Y T is then undone
+    cp.check(L.dpgo_agent_set_local_trajectory(gp._h, cp.dptr(T), cp.dptr(Y)))
+    cp.check(L.dpgo_agent_set_align_candidates(gp._h, 0, None, None, None, None, None, None))
+    gp.upload_X(a.X)
     pub = np.arange(4, dtype=np.int32)
     cp.check(L.dpgo_agent_set_public_poses(gp._h, len(pub), cp.iptr(pub)))
     cp.check(L.dpgo_agent_accel_init(gp._h))
@@ -387,6 +394,10 @@ def test_duplicate_handles_refused():
     cp.check(L.dpgo_agents_set_agent_graph(gp._h, 2, cp.iptr(ptr), cp.iptr(adj)))
     assert L.dpgo_agents_select_round_async(two, 2, cp.iptr(idx2), C.byref(prm), C.c_void_p(buf.data_ptr()), None, 0,
                                             ptrs(send), None) == ERR_INVALID_ARG
+    zeros = [np.zeros(a.r * (a.d + 1) * a.n) for _ in range(2)]          # an upload of either would change X
+    X_host = (C.c_void_p * 2)(*[z.ctypes.data for z in zeros])
+    assert L.dpgo_agents_host_io_async(two, 2, X_host, None, 0, None) == ERR_INVALID_ARG
+    assert L.dpgo_agents_align_async(two, 2, None, 0, cp.iptr(np.ones(1, dtype=np.int32)), 1, None) == ERR_INVALID_ARG
     torch.cuda.synchronize()
     assert np.isnan(buf.cpu().numpy()).all()
     assert np.array_equal(gp.download_X(), a.X)
