@@ -101,8 +101,6 @@ SIGNATURES = {
     "dpgo_nd_debug_emulate": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int64, _ip, _ip, _dp, C.c_double, C.c_int, C.c_int,
                                         C.c_int, _dp, _dp, C.POINTER(C.c_int64)]),
     "dpgo_debug_phase_latency": (C.c_int, [_vp, C.c_int, _dp, _dp]),
-    "dpgo_debug_phase_times": (C.c_int, [_vp, C.c_int, _dp]),
-    "dpgo_debug_phase_times32": (C.c_int, [_vp, C.c_int, _dp]),
     "dpgo_debug_phase_times64": (C.c_int, [_vp, C.c_int, _dp]),
     "dpgo_chordal_initialization": (C.c_int, [C.c_int, C.c_int, C.c_int64, _ip, _ip, _dp, _dp, _dp, _dp, C.c_int, C.c_double,
                                               C.c_int, _dp, _ip]),

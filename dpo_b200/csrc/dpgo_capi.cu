@@ -65,7 +65,7 @@ struct dpgo_problem {
   struct RoundGraph { std::vector<uint64_t> key; dpgo::GraphExec exec; int uses = 0; bool failed = false; };
   std::vector<RoundGraph> round_graphs;      // CUDA graphs of the batched round / host I/O calls, kept by the call's first agent
   template <class Job> struct JobTable { std::vector<uint64_t> key; DevBuf<Job> jobs; int ctas = 0; };
-  int launch_mode = -1;          // -1: by DPGO_CLUSTER_MAX_POSES (default off), 0: full cooperative grid, 1: one thread-block cluster
+  int launch_mode = 0;           // 0: full cooperative grid, 1: one thread-block cluster
   // Q in block-CSR, its launch tables and its host copy (lazy preconditioner setup): build_from_triplets
   struct BlockQ {
     int64_t nb = 0;
@@ -115,7 +115,7 @@ struct dpgo_problem {
   // vectors
   DevBuf<double> G, vec[dpgo::V_COUNT], S[2];
   DevBuf<unsigned> bar;          // [0] arrival counter, [1] epoch
-  DevBuf<unsigned long long> phase_ns;       // diagnostic phase clock (8 slots), allocated on request
+  DevBuf<unsigned long long> phase_ns;       // diagnostic phase clock (64 slots), allocated on request
   DevBuf<dpgo_opt_result_t> result;
   std::unique_ptr<dpgo_opt_result_t, dpgo::CudaFreeHost> h_result;   // pinned
   bool async_pending = false;
@@ -200,8 +200,6 @@ void fill_kparams(const dpgo_problem *p, dpgo::KParams &kp, int op, const dpgo_o
   const dpgo_problem::Nd &F = p->nd[nd_slot(prm.precond)];
   kp.nd = F.k;
   if (!F.ready) kp.nd.nphases = 0;
-  static const int strict = [] { const char *e = std::getenv("DPGO_STRICT_ACQUIRE"); return (e && e[0] == '1') ? 1 : 0; }();
-  kp.strict_acquire = strict;
   kp.cluster = p->cluster ? 1 : 0;
   kp.smem_doubles = 0;
   kp.phase_ns = p->phase_ns.get();
@@ -212,8 +210,7 @@ void fill_kparams(const dpgo_problem *p, dpgo::KParams &kp, int op, const dpgo_o
 }
 
 cudaError_t run_spmv(const dpgo_problem *p, const double *X, const double *G, double *out) {
-  static const bool force_gather = [] { const char *e = std::getenv("DPGO_SPMV_KERNEL"); return e && std::string(e) == "gather"; }();
-  if (p->bsr.ngroups > 0 && !force_gather)
+  if (p->bsr.ngroups > 0)
     return dpgo::launch_spmv_tma(p->r, p->dh, p->bsr.ngroups, p->bsr.groups.get(), p->bsr.rowptr.get(), p->bsr.bcol.get(),
                                  p->bsr.bval.get(), X, G, out, p->sms, p->stream);
   return dpgo::launch_spmv(p->r, p->dh, p->n, p->bsr.rowptr.get(), p->bsr.bcol.get(), p->bsr.bval.get(), X, G, out, p->stream);
@@ -249,10 +246,6 @@ dpgo::nd::Options nd_options(int grid, int r, bool cluster = false) {
   opt.ycap_tiles = dpgo::ND_YCAP_TILES;
   opt.slot_cap = dpgo::ND_SLOT_CAP;
   if (const char *e = std::getenv("DPGO_ND_CUTS")) opt.force_ncuts = std::atoi(e);
-  if (const char *e = std::getenv("DPGO_ND_LEAF")) opt.leaf_size = std::max(1, std::atoi(e));
-  if (const char *e = std::getenv("DPGO_ND_TPHASE_US")) opt.t_phase_us = std::atof(e);
-  if (const char *e = std::getenv("DPGO_ND_BW_GBS")) opt.bw_gbs = std::atof(e);
-  if (const char *e = std::getenv("DPGO_ND_TTILE_US")) opt.t_tile_us = std::atof(e);
   return opt;
 }
 
@@ -506,16 +499,14 @@ int build_from_triplets(dpgo_problem *p, std::vector<BlockTriplet> &trip, unsign
   int grid = p->max_grid;
   const bool dense = (precond_mask & ((1u << DPGO_PRECOND_DENSE_EXACT) | (1u << DPGO_PRECOND_SPARSE_EXACT))) != 0;
   if (!dense) grid = std::max(1, std::min(grid, (n + rows_per_pass - 1) / rows_per_pass));
-  // Launch mode 1 (dpgo_problem_set_launch_mode; or DPGO_CLUSTER_MAX_POSES=<n> for handles left at the default): the step
-  // kernel runs as ONE thread-block cluster (<= 16 CTAs) whose phase ends are hardware cluster barriers instead of the
-  // atomic-counter grid barrier.  For one agent alone this is SLOWER than the full grid (10-16 SMs stream the
-  // preconditioner blocks more slowly than all of them; scripts/phase_times.py --agents 8 / 16 compares the two); its
-  // point is that a cluster launch is not cooperative, so the agents of
-  // a colour class run side by side on one GPU and the round captures into a CUDA graph (dpgo_agents_round_async).
-  static const int cluster_max_poses = [] { const char *e = std::getenv("DPGO_CLUSTER_MAX_POSES"); return e ? std::atoi(e) : 0; }();
+  // Launch mode 1 (dpgo_problem_set_launch_mode): the step kernel runs as ONE thread-block cluster (<= 16 CTAs) whose
+  // phase ends are hardware cluster barriers instead of the atomic-counter grid barrier.  For one agent alone this is
+  // SLOWER than the full grid (10-16 SMs stream the preconditioner blocks more slowly than all of them;
+  // scripts/phase_times.py --agents 8 / 16 compares the two); its point is that a cluster launch is not cooperative, so
+  // the agents of a colour class run side by side on one GPU and the round captures into a CUDA graph
+  // (dpgo_agents_round_async).
   p->cluster = false;
-  const bool want_cluster = p->launch_mode == 1 || (p->launch_mode < 0 && n <= cluster_max_poses);
-  if (p->max_cluster >= 8 && want_cluster) {
+  if (p->max_cluster >= 8 && p->launch_mode == 1) {
     // (one CTA per 16 poses is enough: always taking 16 CTAs makes small agents slower)
     grid = std::max(1, std::min(p->max_cluster, (n + rows_per_pass - 1) / rows_per_pass));
     p->cluster = true;
@@ -1076,7 +1067,7 @@ int dpgo_debug_phase_latency(dpgo_problem_t *p, int phases, double *us_per_phase
   return DPGO_OK;
 }
 
-static int phase_times_impl(dpgo_problem_t *p, int enable, double *ms_by_kind, int nout) {
+int dpgo_debug_phase_times64(dpgo_problem_t *p, int enable, double *ms_by_kind) {
   DPGO_CHECK_HANDLE(p);
   if (enable && !p->phase_ns) {
     DPGO_CUDA(p->phase_ns.alloc(64));
@@ -1087,18 +1078,14 @@ static int phase_times_impl(dpgo_problem_t *p, int enable, double *ms_by_kind, i
     DPGO_CUDA(cudaStreamSynchronize(p->stream));
     DPGO_CUDA(cudaMemcpy(ns, p->phase_ns.get(), sizeof(ns), cudaMemcpyDeviceToHost));
     if (ms_by_kind)
-      for (int i = 0; i < nout; ++i) ms_by_kind[i] = 1e-6 * (double)ns[i];
+      for (int i = 0; i < 64; ++i) ms_by_kind[i] = 1e-6 * (double)ns[i];
     DPGO_CUDA(cudaMemset(p->phase_ns.get(), 0, sizeof(ns)));
     if (!enable) p->phase_ns = {};
   } else if (ms_by_kind) {
-    for (int i = 0; i < nout; ++i) ms_by_kind[i] = 0.0;
+    for (int i = 0; i < 64; ++i) ms_by_kind[i] = 0.0;
   }
   return DPGO_OK;
 }
-
-int dpgo_debug_phase_times(dpgo_problem_t *p, int enable, double *ms_by_kind) { return phase_times_impl(p, enable, ms_by_kind, 8); }
-int dpgo_debug_phase_times32(dpgo_problem_t *p, int enable, double *ms_by_kind) { return phase_times_impl(p, enable, ms_by_kind, 32); }
-int dpgo_debug_phase_times64(dpgo_problem_t *p, int enable, double *ms_by_kind) { return phase_times_impl(p, enable, ms_by_kind, 64); }
 
 int dpgo_spmv_device(dpgo_problem_t *p, const double *X_dev, double *out_dev, int add_G) {
   DPGO_CHECK_HANDLE(p);
@@ -1176,25 +1163,6 @@ int dpgo_nd_debug_emulate(int n, int d, int r, int64_t nb, const int32_t *brow, 
     nd::assign_residency(plan, opt.warps, budget);
     nd::emulate_apply(H, plan, blob, r, V_host, Z_host);
     if (info16) nd_fill_info(H, plan, info16);
-    if (const char *dump = std::getenv("DPGO_ND_DUMP_PLAN")) {            // per (phase, CTA) work statistics, CSV
-      if (FILE *fp = std::fopen(dump, "w")) {
-        std::fprintf(fp, "phase,dir,stage,cta,steps,gather_tiles,jobs,job_cols,max_warp_cols,epis\n");
-        for (size_t ph = 0; ph < plan.phases.size(); ++ph)
-          for (int c = 0; c < plan.grid; ++c) {
-            const nd::CtaPhase &cp = plan.cta_phase[(size_t)plan.phases[ph].cta0 + c];
-            long gt = 0, nj = 0, jc = 0, ne = 0, mw = 0;
-            for (int si = cp.s0; si < cp.s1; ++si) {
-              const nd::Step &st = plan.steps[(size_t)si];
-              gt += st.g1 - st.g0; nj += st.j1 - st.j0; ne += st.e1 - st.e0;
-              std::vector<long> w((size_t)opt.warps, 0);
-              for (int j = st.j0; j < st.j1; ++j) { jc += plan.jobs[(size_t)j].ncols; w[(size_t)((j - st.j0) % opt.warps)] += plan.jobs[(size_t)j].ncols + 40; }
-              mw += *std::max_element(w.begin(), w.end());
-            }
-            std::fprintf(fp, "%zu,%d,%d,%d,%d,%ld,%ld,%ld,%ld,%ld\n", ph, plan.phases[ph].dir, plan.phases[ph].stage, c, cp.s1 - cp.s0, gt, nj, jc, mw, ne);
-          }
-        std::fclose(fp);
-      }
-    }
     if (const char *dump = std::getenv("DPGO_ND_DUMP_JOBS")) {            // residency of every job, CSV
       if (FILE *fp = std::fopen(dump, "w")) {
         std::fprintf(fp, "phase,cta,step,warp,ncols,nres,soff,budget\n");

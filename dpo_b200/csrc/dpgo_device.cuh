@@ -212,11 +212,6 @@ __device__ __forceinline__ double jacobi_elem(const double *__restrict__ dinv, i
 
 // ---- grid-wide barrier for the persistent kernel ------------------------------------------------
 // Monotonic arrival counter (wrap-safe signed comparison); every CTA is resident (cooperative launch).
-__device__ __forceinline__ unsigned ld_acquire_u32(const unsigned *p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ unsigned ld_relaxed_u32(const unsigned *p) {
   unsigned v;
   asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -230,6 +225,5 @@ __device__ __forceinline__ unsigned ld_relaxed_u32(const unsigned *p) {
 // has none: every vector / workspace another CTA may have written is read with ld.global.cg (L2) or ld.relaxed.gpu,
 // never through L1, and read-only data is never rewritten during a launch.  Ordering of those L2 reads after the
 // poll: the poll loop's exit branch depends on the loaded value and the other threads wait at the bar.sync behind it.
-// KParams::strict_acquire != 0 restores the acquire poll (A/B: DPGO_STRICT_ACQUIRE=1).
 
 }  // namespace dpgo

@@ -68,8 +68,7 @@ __device__ __forceinline__ void phase_end(const KParams &kp, BlockCtx &bc, doubl
     }
     if (!kp.cluster) {
       if (lane == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(kp.bar_counter) : "memory");
-      if (kp.strict_acquire) { while ((int)(ld_acquire_u32(kp.bar_counter) - bc.epoch) < 0) { } }
-      else { while ((int)(ld_relaxed_u32(kp.bar_counter) - bc.epoch) < 0) { } }
+      while ((int)(ld_relaxed_u32(kp.bar_counter) - bc.epoch) < 0) { }
     }
   }
   if (kp.cluster) {
@@ -77,8 +76,7 @@ __device__ __forceinline__ void phase_end(const KParams &kp, BlockCtx &bc, doubl
     // publishes the CTA's global writes to the other CTAs of the cluster, which read them from L2) replaces the
     // atomic counter and its polling round trips, a fraction of the cost of a grid-wide phase end
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    if (kp.strict_acquire) asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-    else asm volatile("barrier.cluster.wait.aligned;" ::: "memory");
+    asm volatile("barrier.cluster.wait.aligned;" ::: "memory");
   }
   if (warp == 0) {
     if (NUSED > 0) {

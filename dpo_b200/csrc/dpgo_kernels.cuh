@@ -78,9 +78,8 @@ struct KParams {
   dpgo_opt_result_t *result;   // device copy of the result record
   KNd nd;                // the exact preconditioner prm.precond selects (nd.nphases == 0: not prepared)
   int cluster;           // 1: the whole grid is ONE thread-block cluster (<= 16 CTAs): phase ends use barrier.cluster
-  int strict_acquire;    // 1: the grid barrier polls with ld.acquire (L1 invalidated every phase); 0: relaxed poll (default)
   int smem_doubles;      // dynamic shared memory of this launch, in doubles
-  unsigned long long *phase_ns; // diagnostic (nullable): per phase kind, ns seen by CTA 0 (dpgo_debug_phase_times)
+  unsigned long long *phase_ns; // diagnostic (nullable): per phase kind, ns seen by CTA 0 (dpgo_debug_phase_times64)
   double *opt_record;    // 2 doubles: relative change of the last optimising call, optimising calls so far (OP_OPTIMIZE only)
   const unsigned char *gate;   // nullable: the agent's byte of a selection mask; 0 = the launch returns at entry
 };

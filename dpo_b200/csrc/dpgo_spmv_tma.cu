@@ -2,7 +2,7 @@
 //
 // Why: the measurement-block stream (128 B per block, contiguous for a contiguous range of pose tiles)
 // is >75 % of the algorithmic bytes; a per-row gather kernel serialises 5-8 dependent DRAM latencies per
-// row (rowptr -> indices -> blocks, batch after batch) and stays far below HBM peak (DPGO_SPMV_KERNEL=gather: A/B).
+// row (rowptr -> indices -> blocks, batch after batch) and stays far below HBM peak.
 // Here the row structure and the DRAM stream are decoupled:
 //   * the host cuts the pose tiles into "row groups" of <= BT blocks (consecutive rows);
 //   * each CTA walks its groups with an NSTAGE-deep ring of shared-memory stages; one elected thread

@@ -259,13 +259,10 @@ DPGO_API int dpgo_nd_debug_emulate(int n, int d, int r, int64_t nb, const int32_
 DPGO_API int dpgo_debug_phase_latency(dpgo_problem_t *p, int phases, double *us_per_phase, double *us_launch);
 /* diagnostic: phase clock of the persistent kernel.  enable != 0 switches it on (subsequent optimise calls
  * accumulate, per phase kind, the nanoseconds CTA 0 spent up to the closing grid barrier); every call returns the
- * accumulated milliseconds in ms_by_kind[8] (0 eval pass, 3 Hessian product, 4 tCG update, 5 retraction, 6 final;
- * 1, 2 and 7 unused) and resets them; enable == 0 switches it off. */
-DPGO_API int dpgo_debug_phase_times(dpgo_problem_t *p, int enable, double *ms_by_kind);
-/* same with 32 slots: 0..7 as above, 8 + k = phase k of an exact preconditioner's application (k < 16; DENSE_EXACT
- * has phase 0 only), 24 / 25 / 26 = gathers / panel jobs / epilogues of those phases as seen by CTA 0, others unused */
-DPGO_API int dpgo_debug_phase_times32(dpgo_problem_t *p, int enable, double *ms_by_kind);
-/* same with 64 slots: 32 + 3 k + {0, 1, 2} = gathers / panel jobs / epilogues of phase k (k < 10) as seen by CTA 0 */
+ * accumulated milliseconds in ms_by_kind[64] and resets them; enable == 0 switches it off.  Slots: 0 eval pass,
+ * 3 Hessian product, 4 tCG update, 5 retraction, 6 final; 8 + k = phase k of an exact preconditioner's application
+ * (k < 16; DENSE_EXACT has phase 0 only), 24 / 25 / 26 = gathers / panel jobs / epilogues of those phases as seen by
+ * CTA 0; 32 + 3 k + {0, 1, 2} = gathers / panel jobs / epilogues of phase k (k < 10) as seen by CTA 0; others unused. */
 DPGO_API int dpgo_debug_phase_times64(dpgo_problem_t *p, int enable, double *ms_by_kind);
 
 /* ---- chordal initialisation on the GPU ------------------------------------------------------------------------

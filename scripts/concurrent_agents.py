@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Experiment: the RTR steps of one colour class of small agents on ONE GPU, (a) one after the other as full-grid
-cooperative kernels on one stream, (b) concurrently on per-agent streams.  With DPGO_CLUSTER_MAX_POSES=<n> the agents
-run as single thread-block clusters (non-cooperative launches that can share the GPU)."""
+cooperative kernels on one stream, (b) concurrently on per-agent streams.  When the runner steps a colour class side by
+side, the agents run as single thread-block clusters (non-cooperative launches that can share the GPU)."""
 import argparse, json, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -21,8 +21,7 @@ run = DistributedPGO(edges, n, args.agents, r=5, schedule="coloured")
 for _ in range(4):
     run.step(evaluate=False)
 torch.cuda.synchronize()
-out = {"dataset": args.dataset, "agents": args.agents, "colours": run.ncolours,
-       "cluster_max_poses": os.environ.get("DPGO_CLUSTER_MAX_POSES"), "nd": run.agents[0].mProblem.nd_info()}
+out = {"dataset": args.dataset, "agents": args.agents, "colours": run.ncolours, "nd": run.agents[0].mProblem.nd_info()}
 main = torch.cuda.current_stream().cuda_stream
 for mode in ("one_stream", "own_streams"):
     for a in run.local_ids:

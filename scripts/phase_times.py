@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Phase clock of k_optimize on the bench workload (sphere2500, 1 agent, r = 5, exact preconditioner): where one
 RTR step spends its time, per phase kind, as seen by CTA 0 up to each closing grid barrier
-(dpgo_debug_phase_times).  Prints one JSON line; --dataset / --rank / --precond select other workloads."""
+(dpgo_debug_phase_times64).  Prints one JSON line; --dataset / --rank / --precond select other workloads."""
 import argparse
 import ctypes as C
 import json

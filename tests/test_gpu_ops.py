@@ -89,7 +89,7 @@ def test_preconditioners(ds, r, data_dir):
 
 def test_dense_exact_bytes_and_phase_clock(data_dir):
     """dpgo_precond_algorithmic_bytes reports the bytes of the operator's blocks once it is prepared (the dense inverse
-    of the connected sphere2500 graph); dpgo_debug_phase_times32 accumulates per-phase time of the persistent kernel."""
+    of the connected sphere2500 graph); dpgo_debug_phase_times64 accumulates per-phase time of the persistent kernel."""
     import ctypes as C
     import dpo_b200 as dp
     from dpo_b200 import _capi
@@ -99,19 +99,19 @@ def test_dense_exact_bytes_and_phase_clock(data_dir):
     assert gp.precond_algorithmic_bytes(dp.PRECOND_DENSE_EXACT) == 0                         # nothing prepared yet
     gp.PreConditioner(X, rng.standard_normal(X.shape), dp.PRECOND_DENSE_EXACT)
     assert gp.precond_algorithmic_bytes(dp.PRECOND_DENSE_EXACT) == 8 * N * N + 2 * vec
-    ms = (C.c_double * 32)()
-    _capi.check(gp._lib.dpgo_debug_phase_times32(gp._h, 1, ms))
+    ms = (C.c_double * 64)()
+    _capi.check(gp._lib.dpgo_debug_phase_times64(gp._h, 1, ms))
     opt = dp.QuadraticOptimizer(gp)
     opt.setTrustRegionIterations(1)
     opt.setTrustRegionMaxInnerIterations(5)
     opt.setPreconditioner(dp.PRECOND_DENSE_EXACT)
     opt.optimize(X)
     res = opt.getOptResult()
-    _capi.check(gp._lib.dpgo_debug_phase_times32(gp._h, 0, ms))
+    _capi.check(gp._lib.dpgo_debug_phase_times64(gp._h, 0, ms))
     assert ms[0] > 0 and ms[8] > 0 and ms[3] > 0                                              # eval, dense apply, Hessian
     assert ms[1] == 0 and ms[2] == 0 and ms[9] == 0                                           # one phase per application
     assert sum(ms[:24]) <= res.elapsed_ms * 1.5 + 1.0
-    _capi.check(gp._lib.dpgo_debug_phase_times32(gp._h, 0, ms))                               # switched off: zeros
+    _capi.check(gp._lib.dpgo_debug_phase_times64(gp._h, 0, ms))                               # switched off: zeros
     assert all(v == 0.0 for v in ms)
 
 
