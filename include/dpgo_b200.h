@@ -88,12 +88,14 @@ typedef struct dpgo_opt_params {
 /* ref: include/DPGO/DPGO_types.h:40-59 (ROPTResult) + bookkeeping counters. */
 typedef struct dpgo_opt_result {
   int32_t success;
-  int32_t tcg_status;        /* status of the last tCG solve */
+  int32_t tcg_status;        /* status of the last tCG solve (after a give-up: that of the last rejected attempt;
+                                the reference returns before recording one) */
   int32_t tcg_iterations;    /* inner iterations summed over all attempts */
   int32_t outer_iterations;  /* RTR attempts executed (accepted + rejected) */
   int32_t rejections;        /* rejected attempts */
   int32_t spmv_passes;       /* passes over Q executed inside the call */
-  int32_t precond_applies;   /* applications of the tCG preconditioner M^-1 */
+  int32_t precond_applies;   /* applications of the tCG preconditioner M^-1: one z0 per attempt, a z0 reused
+                                after a rejection included, plus one per inner iteration that did not stop */
   int32_t reserved0;
   double f_init, gradnorm_init, f_opt, gradnorm_opt, relative_change, elapsed_ms;
   double quad_init, lin_init; /* <XQ,X> and <X,G> at the input point: f = quad/2 + lin; summed over agents,

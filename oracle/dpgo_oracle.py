@@ -475,6 +475,25 @@ class QuadraticOptimizer:
         self.precond = precond                       # "exact" (reference) | "jacobi" | "none"
         self.result = OptResult()
         self._jacobi = None
+        # Decision trace: when a list, every comparison that picks a branch of the trust region appends
+        # ("cmp", what, lhs, rhs, scale, taken) -- both sides, and the magnitude the computed lhs is accurate relative to
+        # (0: its own) -- and every RTR attempt appends ("attempt", status, inner, rho, Delta, accepted).
+        self.trace: Optional[list] = None
+        # A deliberately wrong variant of one branch, for tests that check a comparison can tell it from the right one:
+        # "no_cap" (no 5 Delta0 cap), "shrink_half" (shrink by 0.5), "accept_positive" (accept at rho > 0),
+        # "giveup_11" (give up after 11 rejections), "stale_z0" (z0 of the previous point reused after an acceptance),
+        # "wrong_root" (tau of the other root of the boundary equation).  None is the algorithm.
+        self.mutation: Optional[str] = None
+
+    def _cmp(self, what, lhs, op, rhs, scale=0.0):
+        taken = {"<=": lhs <= rhs, ">=": lhs >= rhs, "<": lhs < rhs, ">": lhs > rhs}[op]
+        if self.trace is not None:
+            self.trace.append(("cmp", what, float(lhs), float(rhs), float(scale), bool(taken)))
+        return taken
+
+    def _attempt_done(self, status, inner, rho, Delta, accepted):
+        if self.trace is not None:
+            self.trace.append(("attempt", int(status), int(inner), float(rho), float(Delta), bool(accepted)))
 
     # -- preconditioner variants -------------------------------------------------------
     def _apply_precond(self, X, V):
@@ -529,11 +548,11 @@ class QuadraticOptimizer:
         return retract(Y, -self.rgd_stepsize * g, p.d)
 
     # -- one tCG solve (ROPTLIB SolversTR::tCG_TR; theta=1, kappa=0.1, Min_Inner_Iter=0) ----
-    def _tcg(self, X, EG, g, Delta, max_inner):
+    def _tcg(self, X, EG, g, Delta, max_inner, z0=None):
         p = self.problem
         eta = np.zeros_like(X)
         res = g.copy()
-        z = self._apply_precond(X, res)
+        z = self._apply_precond(X, res) if z0 is None else z0
         delta = -z
         z_r = float(np.sum(z * res))
         d_Pd = z_r
@@ -550,17 +569,32 @@ class QuadraticOptimizer:
             d_Hd = float(np.sum(delta * Hd))
             alpha = z_r / d_Hd if d_Hd != 0.0 else float("inf")
             e_new = e_Pe + 2.0 * alpha * e_Pd + alpha * alpha * d_Pd
-            if d_Hd <= 0.0 or e_new >= Delta * Delta:
-                tau = (-e_Pd + math.sqrt(e_Pd * e_Pd + d_Pd * (Delta * Delta - e_Pe))) / d_Pd
+            dH_scale = float(np.linalg.norm(delta) * np.linalg.norm(Hd))
+            e_scale = abs(e_Pe) + abs(2.0 * alpha * e_Pd) + alpha * alpha * abs(d_Pd)
+            if self._cmp("d_Hd <= 0", d_Hd, "<=", 0.0, dH_scale) or \
+                    self._cmp("e_new >= Delta^2", e_new, ">=", Delta * Delta, e_scale):
+                # Boundary point eta + tau delta, tau the positive root of |eta + tau delta|_P = Delta.  An exactly
+                # stationary start (g = 0, so z = delta = 0 and d_Pd = 0) has no direction to follow: tau = 0 keeps
+                # eta = 0, whose model decrease is 0, so the attempt is rejected and the step returns its input, as the
+                # kernel does (its tau is NaN there, and so is its rho).
+                disc = e_Pd * e_Pd + d_Pd * (Delta * Delta - e_Pe)     # >= 0 unless a mutation broke CG's invariants
+                sq = math.sqrt(disc) if disc >= 0.0 else math.nan
+                if d_Pd == 0.0:
+                    tau = 0.0
+                elif self.mutation == "wrong_root":
+                    tau = (-e_Pd - sq) / d_Pd
+                else:
+                    tau = (-e_Pd + sq) / d_Pd
                 eta = eta + tau * delta
                 status = TCG_NEGCURV if d_Hd <= 0.0 else TCG_EXCREGION
                 break
             e_Pe = e_new
             eta = eta + alpha * delta
+            res_scale = float(np.linalg.norm(res) + abs(alpha) * np.linalg.norm(Hd))
             res = res + alpha * Hd
             nr = float(np.linalg.norm(res))
-            if nr <= n0 * min(n0 ** theta, kappa):
-                status = TCG_LCON if kappa < n0 ** theta else TCG_SCON
+            if self._cmp("nr <= n0 min(n0, 0.1)", nr, "<=", n0 * min(n0 ** theta, kappa), res_scale):
+                status = TCG_LCON if self._cmp("n0 > 0.1", n0 ** theta, ">", kappa) else TCG_SCON
                 break
             z = self._apply_precond(X, res)
             zr_new = float(np.sum(z * res))
@@ -571,10 +605,10 @@ class QuadraticOptimizer:
             d_Pd = z_r + beta * beta * d_Pd
         return eta, status, inner
 
-    def _rtr_attempt(self, X, f1, EG, g, Delta):
+    def _rtr_attempt(self, X, f1, EG, g, Delta, z0=None):
         """One RTRNewton iteration from X with radius Delta: returns (X2, f2, rho, status, inner)."""
         p = self.problem
-        eta, status, inner = self._tcg(X, EG, g, Delta, self.tr_max_inner)
+        eta, status, inner = self._tcg(X, EG, g, Delta, self.tr_max_inner, z0)
         X2 = retract(X, eta, p.d)
         f2 = p.f(X2)
         Heta = p.rie_hess(X, EG, eta)
@@ -586,9 +620,12 @@ class QuadraticOptimizer:
     def trust_region(self, Yinit: np.ndarray) -> np.ndarray:
         """ref: src/QuadraticOptimizer.cpp:61-122 (+ ROPTLIB SolversTR::Run radius rules)."""
         p, res = self.problem, self.result
+        mut = self.mutation
+        accept_rho = 0.0 if mut == "accept_positive" else 0.1
+        shrink = 0.5 if mut == "shrink_half" else 0.25
         gn0 = p.rie_grad_norm(Yinit)
         res.spmv += 5
-        if gn0 < self.tr_tolerance:                              # ref :67-70
+        if self._cmp("gradnorm < tol", gn0, "<", self.tr_tolerance):          # ref :67-70
             return Yinit
         X = Yinit
         if self.tr_iterations == 1:                              # ref :92-110
@@ -603,37 +640,47 @@ class QuadraticOptimizer:
                 res.tcg_iterations += inner
                 res.tcg_status = status
                 res.outer_iterations += 1
-                if rho > 0.1:
+                accepted = self._cmp("rho > 0.1", rho, ">", accept_rho)
+                self._attempt_done(status, inner, rho, radius, accepted)
+                if accepted:
                     return X2
-                if total_steps > 10:
-                    return Yinit
-                radius /= 4.0
-                total_steps += 1
+                # every rejected attempt counts, the last one before the give-up included (the reference returns
+                # before its own counter sees that one)
                 res.rejections += 1
+                if total_steps > (9 if mut == "giveup_11" else 10):
+                    return Yinit
+                radius *= shrink
+                total_steps += 1
         # multi-iteration mode (ROPTLIB's own loop): Delta0, maximum_Delta = 5 Delta0
         Delta = self.tr_initial_radius
-        Delta_max = 5.0 * self.tr_initial_radius
+        Delta_max = math.inf if mut == "no_cap" else 5.0 * self.tr_initial_radius
         f1 = p.f(X)
         EG = p.euc_grad(X)
         g = tangent_project(X, EG, p.d)
+        z0 = self._apply_precond(X, g)
         res.spmv += 2
         for _ in range(self.tr_iterations):
-            X2, f2, rho, status, inner = self._rtr_attempt(X, f1, EG, g, Delta)
+            X2, f2, rho, status, inner = self._rtr_attempt(X, f1, EG, g, Delta, z0)
             res.tcg_iterations += inner
             res.tcg_status = status
             res.outer_iterations += 1
-            if rho < 0.25:
-                Delta *= 0.25
-            elif rho > 0.75 and status in (TCG_NEGCURV, TCG_EXCREGION):
+            Delta_used = Delta
+            if self._cmp("rho < 0.25", rho, "<", 0.25):
+                Delta *= shrink
+            elif self._cmp("rho > 0.75", rho, ">", 0.75) and status in (TCG_NEGCURV, TCG_EXCREGION):
                 Delta = min(2.0 * Delta, Delta_max)
-            if rho > 0.1:
+            accepted = self._cmp("rho > 0.1", rho, ">", accept_rho)
+            self._attempt_done(status, inner, rho, Delta_used, accepted)
+            if accepted:
                 X, f1 = X2, f2
                 EG = p.euc_grad(X)
                 g = tangent_project(X, EG, p.d)
+                if mut != "stale_z0":
+                    z0 = self._apply_precond(X, g)
                 res.spmv += 1
             else:
                 res.rejections += 1
-            if float(np.linalg.norm(g)) < self.tr_tolerance:
+            if self._cmp("gradnorm < tol", float(np.linalg.norm(g)), "<", self.tr_tolerance):
                 break
         return X
 
