@@ -1,4 +1,4 @@
-// dpgo_kernels.cuh -- kernel-side parameter block shared by dpgo_kernels.cu and dpgo_capi.cu
+// dpgo_kernels.cuh -- kernel-side parameter block shared by dpgo_kernels.cu and the C API (dpgo_capi*.cu)
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -159,7 +159,7 @@ struct KRefactor {
 // Every stage of R (deepest first): assemble the fronts, sweep them, pack the panels.  Ordinary launches on `stream`, none
 // synchronising; the sequence captures into a CUDA graph.
 cudaError_t launch_nd_refactor(const KRefactor &k, const nd::Refactor &R, cudaStream_t stream);
-// block-Jacobi inverse blocks (Q_jj + shift I)^-1 of every pose, 4x4 padded (the host's jacobi_blocks in dpgo_capi.cu);
+// block-Jacobi inverse blocks (Q_jj + shift I)^-1 of every pose, 4x4 padded (the host's jacobi_blocks in dpgo_capi_precond.cu);
 // a non-positive pivot sets *fail (nullable)
 cudaError_t launch_jacobi_blocks(int n, int dh, const int *rowptr, const int *bcol, const double *bval, double shift, double *dinv,
                                  int *fail, cudaStream_t stream);

@@ -18,7 +18,7 @@ import numpy as np
 import structure_cases as sc
 from oracle import dpgo_oracle as orc
 
-# mirrored from dpgo_kernels.cuh / dpgo_capi.cu
+# mirrored from dpgo_kernels.cuh / dpgo_capi_agents.cu
 STATUS_ROWS = 32             # rows of an agent's Q per status CTA
 ACCEL_THREADS = 128          # poses per momentum CTA
 SELECT_MAX_AGENTS = 1024     # agents one selection CTA ranks

@@ -181,7 +181,7 @@ def make_case(name: str, d: int, seed: int = 0) -> Case:
 # host facts: which branch a case reaches
 # ---------------------------------------------------------------------------------------------------------------------
 def tma_groups(row_blocks, bt=SPMV_GROUP_BLOCKS):
-    """Row groups of the TMA-fed product as the library cuts them (dpgo_capi.cu build_from_triplets): consecutive rows,
+    """Row groups of the TMA-fed product as the library cuts them (build_from_triplets in dpgo_capi.cu): consecutive rows,
     <= bt rows and <= bt blocks each.  [(row0, row1, block0, block1)], or None when a row exceeds bt blocks or Q has
     no block (the gather kernel runs then)."""
     rowptr = np.concatenate([[0], np.cumsum(row_blocks)])
