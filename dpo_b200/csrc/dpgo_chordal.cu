@@ -44,21 +44,23 @@ __global__ void k_dot(int len, const double *__restrict__ a, const double *__res
 __global__ void k_mask_anchor(double *q) {
   if (threadIdx.x < TS9) q[threadIdx.x] = 0.0;
 }
-// x += alpha p; r -= alpha q; z = r / diag      (alpha = rz / pq)
+// x += alpha p; r -= alpha q; z = r / diag      (alpha = rz / pq, 0 unless pq > 0)
+// Between two host checks the loop keeps iterating after convergence; once rz reaches exactly 0, p = 0 and pq = 0, and
+// alpha = 0 / 0 would put NaN into x.  alpha = 0 (and beta = 0 below) make a converged solve a fixed point instead.
 __global__ void k_update_xrz(int len, const double *__restrict__ sc, const double *__restrict__ p, const double *__restrict__ q,
                              const double *__restrict__ dinv, double *x, double *r, double *z) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= len) return;
-  const double alpha = sc[0] / sc[1];
+  const double alpha = (sc[1] > 0.0) ? sc[0] / sc[1] : 0.0;
   x[i] = fma(alpha, p[i], x[i]);
   const double rr = fma(-alpha, q[i], r[i]);
   r[i] = rr;
   z[i] = rr * dinv[i / 3];            // element (a, k) of tile t sits at 9 t + 3 k + a: column index = i / 3
 }
-// p = z + beta p  (beta = rz_new / rz); the last thread rotates the scalars
+// p = z + beta p  (beta = rz_new / rz, 0 unless rz > 0)
 __global__ void k_update_p(int len, double *sc, const double *__restrict__ z, double *p) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const double beta = sc[2] / sc[0];
+  const double beta = (sc[0] > 0.0) ? sc[2] / sc[0] : 0.0;
   if (i < len) p[i] = fma(beta, p[i], z[i]);
 }
 __global__ void k_rotate_scalars(double *sc) { sc[0] = sc[2]; }
@@ -100,7 +102,8 @@ struct ProblemGuard {
   } while (0)
 
 // Solve X Q = B on the free tiles (tile 0 anchored to zero in X) by Jacobi-preconditioned CG; B comes in `b` (anchored tile
-// already zero), the solution is left in `x`.  Everything runs on `st` (also the problem's stream).
+// already zero), the solution is left in `x`.  Everything runs on `st` (also the problem's stream).  Stops when
+// rz = r D^-1 r^T <= tol^2 rz0; DPGO_ERR_CUDA when rz turns NaN or max_iter iterations do not get there.
 int pcg(dpgo_problem_t *h, int n, const double *diag_host, double *x, const double *b, double tol, int max_iter, int *iters,
         cudaStream_t st, std::string &err) {
   const int len = TS9 * n;
@@ -121,6 +124,7 @@ int pcg(dpgo_problem_t *h, int n, const double *diag_host, double *x, const doub
   *iters = 0;
   if (!(rz0 > 0.0)) return DPGO_OK;
   const int CHECK = 25;
+  bool converged = false;
   for (int it = 0; it < max_iter; ++it) {
     CH_TRY(dpgo_spmv_device(h, p.get(), q.get(), 0));                           // q = p Q  (k_spmv_tma)
     k_mask_anchor<<<1, 32, 0, st>>>(q.get());
@@ -135,7 +139,17 @@ int pcg(dpgo_problem_t *h, int n, const double *diag_host, double *x, const doub
       CH_CUDA(cudaMemcpyAsync(&rz, sc.get(), sizeof(double), cudaMemcpyDeviceToHost, st));
       CH_CUDA(cudaStreamSynchronize(st));
       if (!(rz == rz)) { err = "chordal initialisation: conjugate gradients broke down"; return DPGO_ERR_CUDA; }
-      if (rz <= tol * tol * rz0) break;
+      if (rz <= tol * tol * rz0) { converged = true; break; }
+    }
+  }
+  if (!converged) {                                  // the last check was not on convergence (or max_iter % CHECK != 0)
+    double rz = 0.0;
+    CH_CUDA(cudaMemcpyAsync(&rz, sc.get(), sizeof(double), cudaMemcpyDeviceToHost, st));
+    CH_CUDA(cudaStreamSynchronize(st));
+    if (!(rz == rz)) { err = "chordal initialisation: conjugate gradients broke down"; return DPGO_ERR_CUDA; }
+    if (rz > tol * tol * rz0) {
+      err = "chordal initialisation: conjugate gradients did not reach tol in max_iter iterations (" + std::to_string(max_iter) + ")";
+      return DPGO_ERR_CUDA;
     }
   }
   CH_CUDA(cudaStreamSynchronize(st));

@@ -44,7 +44,8 @@ enum {
   DPGO_ERR_INVALID_ARG = 1, /* shape / pointer / range violation (ref: assert() on shapes,
                                src/QuadraticProblem.cpp:32-33,51-52) */
   DPGO_ERR_NO_DEVICE = 2,   /* no CUDA device / device index out of range */
-  DPGO_ERR_CUDA = 3,        /* a CUDA runtime call or kernel failed */
+  DPGO_ERR_CUDA = 3,        /* a CUDA runtime call or kernel failed, or a numerical solve failed (the chordal
+                               initialisation's conjugate gradients broke down or did not converge in max_iter) */
   DPGO_ERR_STATE = 4,       /* call order violation (e.g. optimise before set_Q) */
   DPGO_ERR_UNSUPPORTED = 5, /* d not in {2,3}; r outside the compiled set (d=3: 3..5, d=2: 2,3,5); an exact
                                preconditioner whose blocks would exceed 24 GB (DENSE_EXACT: N above about 54k) */
@@ -272,8 +273,11 @@ DPGO_API int dpgo_debug_phase_times64(dpgo_problem_t *p, int enable, double *ms_
  * t_0 = 0) + projectToRotationGroup :463-477.  Both normal systems are 3 x 3-block connection Laplacians, solved by
  * Jacobi-preconditioned conjugate gradients whose product is the TMA-fed block-CSR kernel of the hot path.
  * m edges p1 -> p2 (pose ids), R: m x d x d row-major, t: m x d, kappa / tau: m.  T_host: d x (d+1)n column-major
- * ([R_p t_p] per pose, the layout of the reference's Matrix).  tol: relative residual (<= 0: 1e-11); iterations2[2]
- * (nullable) receives the CG iteration counts of the two solves.  dpgo_chordal_last_error() for the message. */
+ * ([R_p t_p] per pose, the layout of the reference's Matrix).  tol: relative residual in the Jacobi-scaled norm (<= 0:
+ * 1e-11); max_iter: CG iteration cap per solve (<= 0: 50000).  A solve that does not reach tol within max_iter iterations,
+ * or whose residual turns NaN, fails with DPGO_ERR_CUDA; poses outside the connected component of pose 0 get R = I.
+ * iterations2[2] (nullable) receives the CG iteration counts of the two solves.  Arguments are checked before any device
+ * call; n = 1 needs no device.  dpgo_chordal_last_error() for the message. */
 DPGO_API int dpgo_chordal_initialization(int n, int d, int64_t m, const int32_t *p1, const int32_t *p2, const double *R,
                                          const double *t, const double *kappa, const double *tau, int device, double tol,
                                          int max_iter, double *T_host, int32_t *iterations2);

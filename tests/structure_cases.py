@@ -1,5 +1,6 @@
 """Pose graphs whose shape reaches the kernels' host-chosen branches, and componentwise comparators against a
-high-precision reference.  Helper module of test_structure_cases.py (CPU) and test_gpu_structures.py (GPU); no fixtures.
+high-precision reference.  Helper module of test_structure_cases.py (CPU) and test_gpu_structures.py (GPU), whose graphs
+the chordal-initialisation tests (test_chordal_cpu.py, test_gpu_chordal.py) reuse; no fixtures.
 
 The shipped datasets have small, even degrees and no empty rows, so several branches of the library are never taken on
 them.  Each case below names the branch it is built for (`Case.target`); test_structure_cases.py checks from host facts
@@ -94,6 +95,34 @@ def edge_set(rng, d, pairs):
     z = np.zeros(m, dtype=np.int64)
     return pg.EdgeSet(d, z, z, pairs[:, 0], pairs[:, 1], random_rotations(rng, m, d), rng.standard_normal((m, d)),
                       rng.uniform(1.0, 100.0, m), rng.uniform(0.5, 10.0, m))
+
+
+def noise_free_graph(d, pairs, n, seed=0, kappa=None, tau=None):
+    """Random ground-truth poses and the exact relative measurements of `pairs` between them; weights as edge_set draws
+    them unless given.  Returns (n, edges, ground-truth T of shape (d, (d+1) n))."""
+    rng = np.random.default_rng([seed, d, n])
+    Rp = random_rotations(rng, n, d)
+    tp = rng.uniform(-10.0, 10.0, (n, d))
+    e = edge_set(rng, d, pairs)
+    i, j = e.p1, e.p2
+    e.R[:] = np.einsum("mba,mbc->mac", Rp[i], Rp[j])                  # R_i^T R_j
+    e.t[:] = np.einsum("mba,mb->ma", Rp[i], tp[j] - tp[i])            # R_i^T (t_j - t_i)
+    if kappa is not None:
+        e.kappa[:] = kappa
+    if tau is not None:
+        e.tau[:] = tau
+    T = np.concatenate([Rp, tp[:, :, None]], axis=2)                  # (n, d, d+1)
+    return n, e, np.transpose(T, (1, 0, 2)).reshape(d, (d + 1) * n)
+
+
+def in_gauge_of_pose_zero(T, d):
+    """T expressed in the frame of its pose 0 (R_0 = I, t_0 = 0)."""
+    n = T.shape[1] // (d + 1)
+    Tt = np.asarray(T).reshape(d, n, d + 1)
+    R0, t0 = Tt[:, 0, :d], Tt[:, 0, d]
+    out = np.einsum("ba,bnc->anc", R0, Tt)
+    out[:, :, d] = np.einsum("ba,bn->an", R0, Tt[:, :, d] - t0[:, None])
+    return out.reshape(d, (d + 1) * n)
 
 
 def chain(poses):

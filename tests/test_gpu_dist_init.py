@@ -266,3 +266,37 @@ def test_two_ranks_bit_equal_to_one_process(tmp_path, data_dir):
         assert np.array_equal(np.load(os.path.join(str(tmp_path), f"X_{a}.npy")), run.agents[a].mProblem.download_X()), a
     with open(os.path.join(str(tmp_path), "report.json")) as fh:
         assert json.load(fh) == run.init_report
+
+
+def tiny_agent_owner(n):
+    """smallGrid3D in 4 agents, agent 1 owning exactly 2 consecutive poses and agent 2 exactly 3 (joined by odometry, and
+    sharing odometry edges with agents 0 and 3): their local chordal solves converge before CG's first residual check."""
+    owner = np.full(n, 3, dtype=np.int64)
+    owner[:60] = 0
+    owner[60:62] = 1
+    owner[62:65] = 2
+    return owner
+
+
+def test_agents_of_two_and_three_poses(tmp_path, data_dir):
+    """The distributed start with agents of 2 and 3 poses, in the Python runner against the oracle and in the C++ device
+    runner (examples/MultiAgentPGO --resident --init distributed --partition FILE): the same per-agent records."""
+    import subprocess
+    from dpo_b200 import posegraph as pg
+    path = os.path.join(data_dir, "smallGrid3D.g2o")
+    edges, n = pg.read_g2o_file(path)
+    meas, _ = orc.read_g2o(path)
+    owner = tiny_agent_owner(n)
+    parts, counts, _ = orc.split_measurements(meas, owner, 4)
+    assert list(counts[1:3]) == [2, 3] and all(len(parts[a][2]) > 0 for a in range(4))
+    run = start(edges, n, 4, owner=owner)
+    _, _, rep = check_against_oracle(run, meas, n, 4, owner=owner)
+    assert all(r["wave"] >= 0 for r in rep)
+    part = os.path.join(str(tmp_path), "owner.txt")
+    np.savetxt(part, owner, fmt="%d")
+    exe = os.path.join(ROOT, "build", "examples", "MultiAgentPGO")
+    res = subprocess.run([exe, path, "--robots", "4", "--iters", "1", "--stop", "0", "--resident", "--init", "distributed",
+                          "--partition", part], capture_output=True, text=True, timeout=600)
+    assert res.returncode == 0, res.stderr[-2000:]
+    rec = [[int(v) for v in ln.split()[2:]] for ln in res.stdout.splitlines() if ln.startswith("init ")]
+    assert rec == [[r["wave"], r["neighbor"], r["candidates"], r["inliers"], r["iterations"]] for r in rep]
