@@ -10,7 +10,9 @@
 #include <algorithm>
 #include <cmath>
 #include <map>
+#include <memory>
 #include <stdexcept>
+#include <type_traits>
 
 #include "dpgo_b200.h"
 
@@ -32,57 +34,109 @@ unsigned greedySelection(unsigned selected, const DeviceRBCDStatus &st, unsigned
     if (std::sqrt(st.at(a, 2)) > std::sqrt(st.at(arg, 2))) arg = a;
   return arg;
 }
+
+// Owners of the runner's resources, as in dpo_b200/csrc/dpgo_devbuf.cuh but over the C ABI (this library does not link
+// the CUDA runtime).  Dropping one releases what it holds, so a constructor that throws half way leaks nothing.
+struct DeviceFree {
+  int device = 0;
+  void operator()(double *p) const { dpgo_device_free(device, p); }
+};
+struct StreamDestroy {
+  int device = 0;
+  void operator()(void *s) const { dpgo_stream_destroy(device, s); }
+};
+struct PinnedFree { void operator()(double *p) const { dpgo_host_free_pinned(p); } };
+struct CommDestroy { void operator()(ncclComm_t c) const { ncclCommDestroy(c); } };
+using DeviceBuffer = std::unique_ptr<double, DeviceFree>;
+using Stream = std::unique_ptr<void, StreamDestroy>;
+using PinnedBuffer = std::unique_ptr<double, PinnedFree>;
+using Comm = std::unique_ptr<std::remove_pointer_t<ncclComm_t>, CommDestroy>;
+
+DeviceBuffer deviceBuffer(int device, size_t count) {   // zero-initialised
+  void *p = nullptr;
+  check(dpgo_device_malloc(device, sizeof(double) * count, &p), "dpgo_device_malloc");
+  return DeviceBuffer(static_cast<double *>(p), DeviceFree{device});
+}
+
+// An array of `part` doubles per agent that every GPU holds for all K agents (`all`), each GPU writing the parts of its
+// own agents into `own()` and one all-gather filling every `all` from them.  One GPU writes straight into `all`.
+struct Gathered {
+  DeviceBuffer all, ownParts;      // ownParts: more than one GPU only
+  double *own() const { return ownParts ? ownParts.get() : all.get(); }
+};
+Gathered gathered(int device, size_t part, unsigned K, unsigned perGpu) {
+  Gathered b;
+  b.all = deviceBuffer(device, K * part);
+  if (perGpu < K) b.ownParts = deviceBuffer(device, perGpu * part);
+  return b;
+}
+
+// One GPU: its stream, buffers and communicator (released in reverse order: communicator, buffers, stream), and the
+// fixed arguments of the calls that take every agent of its contiguous block first .. first + perGpu - 1.
+struct Gpu {
+  Stream stream;
+  Gathered tiles;                  // the agents' padded public tiles of X (slotElems doubles each)
+  Gathered auxTiles;               // accelerated rounds: the public tiles of Y
+  Gathered records;                // status records, DPGO_STATUS_DOUBLES each
+  Comm comm;                       // more than one GPU only
+  unsigned first = 0;
+  std::vector<dpgo_problem *> handles;
+  std::vector<int32_t> ids;        // first, first + 1, ...
+  std::vector<double *> tileDst, auxTileDst;   // each agent's slot in tiles.own() / auxTiles.own()
+};
 }  // namespace
 
 struct DeviceRBCD::Impl {
   unsigned d = 3, r = 5, dh = 4, ts = 20, K = 1, N = 1, perGpu = 1, pmax = 1;
   size_t n = 0;
+  size_t slotElems = 0;            // one agent's padded public tiles: pmax * ts doubles
+  int64_t numSlots = 0;            // the slots of a gathered tile buffer: K * pmax
   std::string schedule;
   std::vector<std::unique_ptr<PGOAgent>> agents;
   std::vector<size_t> count;
   std::vector<std::vector<size_t>> globalOf;      // agent -> global pose ids in local order
   std::vector<dpgo_problem *> h;
-  std::vector<int> gpuOf;
-  std::vector<void *> stream;
-  std::vector<double *> send, gathered;
-  std::vector<double *> sendAux, gatheredAux;      // accelerated rounds: the public tiles of Y
+  std::vector<Gpu> gpu;
+  std::vector<int32_t> slots;      // 0 .. perGpu - 1: a GPU's agents' places in its status records
+  PinnedBuffer statusHost;         // all agents' records in agent order
   bool acceleration = false;
   unsigned restartInterval = 30;
   double momentumN = 1;
   bool colourMomentum = false;     // momentumBlocks == "colours"
-  std::vector<ncclComm_t> comm;
   std::vector<std::vector<unsigned>> neighbors;
   dpgo_opt_params_t prm;
   unsigned selected = 0;
   bool concurrent = false;         // active agents of a GPU side by side (cluster launches, own streams)
   bool gatheredCurrent = false;    // the gathered buffers hold every agent's current public tiles
-  std::vector<double *> statusDev; // per GPU: its agents' status records
-  std::vector<double *> statusAll; // per GPU: every agent's record (N == 1: statusDev), the greedy_set selection's input
-  double *statusHost = nullptr;    // pinned, all agents' records in agent order
-  bool recordsCurrent = false;     // statusAll holds the records of the current iterates
+  bool recordsCurrent = false;     // records.all holds the records of the current iterates
 
-  // one ncclAllGather group: every GPU's send buffer into every GPU's gathered buffer (one GPU packs straight into it)
-  void allGather(const std::vector<double *> &sendBuf, const std::vector<double *> &gatheredBuf) {
+  // also when the constructor throws: the agents' problems run on the GPU streams, so they go before the members
+  ~Impl() {
+    for (unsigned g = 0; g < gpu.size(); ++g)
+      if (gpu[g].stream) dpgo_stream_synchronize((int)g, gpu[g].stream.get());   // errors ignored
+    agents.clear();
+  }
+
+  double *tileDst(unsigned a) const {
+    const Gpu &G = gpu[a / perGpu];
+    return G.tileDst[a - G.first];
+  }
+  // one ncclAllGather group: every GPU's own parts of `buf` (`part` doubles per agent) into every GPU's copy of all
+  void allGather(Gathered Gpu::*buf, size_t part) {
     if (N == 1) return;
     checkNccl(ncclGroupStart(), "ncclGroupStart");
     for (unsigned g = 0; g < N; ++g) {
       check(dpgo_device_set((int)g), "dpgo_device_set");
-      checkNccl(ncclAllGather(sendBuf[g], gatheredBuf[g], (size_t)perGpu * pmax * ts, ncclDouble, comm[g], (cudaStream_t)stream[g]),
+      const Gathered &b = gpu[g].*buf;
+      checkNccl(ncclAllGather(b.own(), b.all.get(), (size_t)perGpu * part, ncclDouble, gpu[g].comm.get(),
+                              (cudaStream_t)gpu[g].stream.get()),
                 "ncclAllGather");
     }
     checkNccl(ncclGroupEnd(), "ncclGroupEnd");
   }
-  // one ncclAllGather group of the status records: every GPU's agents' records into every GPU's copy of all of them
-  void allGatherRecords() {
-    if (N == 1) return;
-    checkNccl(ncclGroupStart(), "ncclGroupStart");
-    for (unsigned g = 0; g < N; ++g) {
-      check(dpgo_device_set((int)g), "dpgo_device_set");
-      checkNccl(ncclAllGather(statusDev[g], statusAll[g], (size_t)perGpu * DPGO_STATUS_DOUBLES, ncclDouble, comm[g],
-                              (cudaStream_t)stream[g]),
-                "ncclAllGather");
-    }
-    checkNccl(ncclGroupEnd(), "ncclGroupEnd");
+  void buildG() {                  // every agent's G from the gathered tiles
+    for (unsigned a = 0; a < K; ++a)
+      check(dpgo_agent_build_G(h[a], gpu[a / perGpu].tiles.all.get(), numSlots), "dpgo_agent_build_G");
   }
 };
 
@@ -210,18 +264,22 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
     }
 
   // ---- streams, agents (Q on the agent's GPU), resident iterates ----
-  I.stream.assign(I.N, nullptr);
-  for (unsigned g = 0; g < I.N; ++g) check(dpgo_stream_create((int)g, &I.stream[g]), "dpgo_stream_create");
+  I.gpu.resize(I.N);
+  for (unsigned g = 0; g < I.N; ++g) {
+    void *s = nullptr;
+    check(dpgo_stream_create((int)g, &s), "dpgo_stream_create");
+    I.gpu[g].stream = Stream(s, StreamDestroy{(int)g});
+    I.gpu[g].first = g * I.perGpu;
+  }
   I.h.assign(K, nullptr);
-  I.gpuOf.assign(K, 0);
   Matrix lift;
   for (unsigned a = 0; a < K; ++a) {
+    Gpu &G = I.gpu[a / I.perGpu];
     PGOAgentParameters prm(d, r, K);
     prm.algorithm = opt.algorithm;
     prm.preconditioner = opt.preconditioner;
     prm.device = (int)(a / I.perGpu);
     prm.cluster = I.concurrent;
-    I.gpuOf[a] = prm.device;
     I.agents.emplace_back(new PGOAgent(a, prm));
     if (a == 0) I.agents[0]->getLiftingMatrix(lift);
     else I.agents[a]->setLiftingMatrix(lift);
@@ -230,7 +288,9 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
     I.agents[a]->setPoseGraph(odo[a], priv[a], shared[a], Matrix::Zero(d, dh * I.count[a]));
     I.h[a] = I.agents[a]->problem()->handle();
     if (!I.h[a]) throw std::runtime_error("DeviceRBCD: agent without a device problem");
-    check(dpgo_problem_set_stream(I.h[a], I.stream[(size_t)I.gpuOf[a]]), "dpgo_problem_set_stream");
+    check(dpgo_problem_set_stream(I.h[a], G.stream.get()), "dpgo_problem_set_stream");
+    G.handles.push_back(I.h[a]);
+    G.ids.push_back((int32_t)a);
     if (!distributed) {
       Matrix Xa0(r, dh * I.count[a]);
       for (size_t q = 0; q < I.count[a]; ++q) Xa0.block(0, q * dh, r, dh) = Matrix(XInit).block(0, I.globalOf[a][q] * dh, r, dh);
@@ -257,7 +317,7 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
           kap.push_back(m.weight * m.kappa); tau.push_back(m.weight * m.tau);
         }
       if (dpgo_chordal_initialization((int)na, (int)d, (int64_t)p1.size(), p1.data(), p2.data(), R.data(), t.data(), kap.data(),
-                                      tau.data(), I.gpuOf[a], 0.0, 0, T.data(), nullptr) != DPGO_OK)
+                                      tau.data(), prm.device, 0.0, 0, T.data(), nullptr) != DPGO_OK)
         throw std::runtime_error(std::string("dpgo_chordal_initialization: ") + dpgo_chordal_last_error());
     }
     check(dpgo_agent_set_local_trajectory(I.h[a], T.data(), lift.data()), "dpgo_agent_set_local_trajectory");
@@ -296,26 +356,30 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
     check(dpgo_agent_set_shared_edges(I.h[a], (int)m, loc.data(), slot.data(), outg.data(), T.data(), om.data()),
           "dpgo_agent_set_shared_edges");
   }
-  // ---- exchange buffers and communicators ----
-  const size_t slotElems = (size_t)I.pmax * I.ts;
-  I.send.assign(I.N, nullptr);
-  I.gathered.assign(I.N, nullptr);
+  // ---- exchange and status buffers, communicators ----
+  constexpr unsigned S = DPGO_STATUS_DOUBLES;
+  I.slotElems = (size_t)I.pmax * I.ts;
+  I.numSlots = (int64_t)K * I.pmax;
   for (unsigned g = 0; g < I.N; ++g) {
-    void *p = nullptr;
-    check(dpgo_device_malloc((int)g, sizeof(double) * K * slotElems, &p), "dpgo_device_malloc");
-    I.gathered[g] = static_cast<double *>(p);
-    if (I.N == 1) {
-      I.send[g] = I.gathered[g];                       // a single GPU packs straight into the gathered layout
-    } else {
-      check(dpgo_device_malloc((int)g, sizeof(double) * I.perGpu * slotElems, &p), "dpgo_device_malloc");
-      I.send[g] = static_cast<double *>(p);
+    Gpu &G = I.gpu[g];
+    G.tiles = gathered((int)g, I.slotElems, K, I.perGpu);
+    if (I.acceleration) G.auxTiles = gathered((int)g, I.slotElems, K, I.perGpu);
+    G.records = gathered((int)g, S, K, I.perGpu);
+    for (unsigned i = 0; i < I.perGpu; ++i) {
+      G.tileDst.push_back(G.tiles.own() + i * I.slotElems);
+      if (I.acceleration) G.auxTileDst.push_back(G.auxTiles.own() + i * I.slotElems);
     }
   }
+  for (unsigned i = 0; i < I.perGpu; ++i) I.slots.push_back((int32_t)i);
+  void *hp = nullptr;
+  check(dpgo_host_alloc_pinned(sizeof(double) * S * K, &hp), "dpgo_host_alloc_pinned");
+  I.statusHost.reset(static_cast<double *>(hp));
   if (I.N > 1) {
     std::vector<int> devs(I.N);
+    std::vector<ncclComm_t> comm(I.N, nullptr);
     for (unsigned g = 0; g < I.N; ++g) devs[g] = (int)g;
-    I.comm.assign(I.N, nullptr);
-    checkNccl(ncclCommInitAll(I.comm.data(), (int)I.N, devs.data()), "ncclCommInitAll");
+    checkNccl(ncclCommInitAll(comm.data(), (int)I.N, devs.data()), "ncclCommInitAll");
+    for (unsigned g = 0; g < I.N; ++g) I.gpu[g].comm.reset(comm[g]);
   }
   if (distributed) {
     // candidate tables (ref computeNeighborTransform / findSharedLoopClosureWithNeighbor, src/PGOAgent.cpp:250-288,922-934):
@@ -353,19 +417,6 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
   if (I.acceleration) {
     I.momentumN = opt.momentumBlocks == "colours" ? (double)mNumColours : (double)K;
     for (unsigned a = 0; a < K; ++a) check(dpgo_agent_accel_init(I.h[a]), "dpgo_agent_accel_init");
-    I.sendAux.assign(I.N, nullptr);
-    I.gatheredAux.assign(I.N, nullptr);
-    for (unsigned g = 0; g < I.N; ++g) {
-      void *p = nullptr;
-      check(dpgo_device_malloc((int)g, sizeof(double) * K * slotElems, &p), "dpgo_device_malloc");
-      I.gatheredAux[g] = static_cast<double *>(p);
-      if (I.N == 1) {
-        I.sendAux[g] = I.gatheredAux[g];
-      } else {
-        check(dpgo_device_malloc((int)g, sizeof(double) * I.perGpu * slotElems, &p), "dpgo_device_malloc");
-        I.sendAux[g] = static_cast<double *>(p);
-      }
-    }
   }
   if (I.schedule == "greedy_set") {                     // the agent graph in CSR form, with each GPU's first agent
     std::vector<int32_t> ptr{0}, adj;
@@ -373,9 +424,8 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
       for (unsigned b : I.neighbors[a]) adj.push_back((int32_t)b);
       ptr.push_back((int32_t)adj.size());
     }
-    for (unsigned g = 0; g < I.N; ++g)
-      check(dpgo_agents_set_agent_graph(I.h[(size_t)g * I.perGpu], (int)K, ptr.data(), adj.data()),
-            "dpgo_agents_set_agent_graph");
+    for (const Gpu &G : I.gpu)
+      check(dpgo_agents_set_agent_graph(G.handles[0], (int)K, ptr.data(), adj.data()), "dpgo_agents_set_agent_graph");
   }
   dpgo_opt_params_default(&I.prm);
   I.prm.algorithm = (opt.algorithm == ROPTALG::RTR) ? DPGO_ALG_RTR : DPGO_ALG_RGD;
@@ -386,26 +436,7 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
   I.prm.tr_initial_radius = 100;
 }
 
-DeviceRBCD::~DeviceRBCD() {
-  if (!impl) return;
-  Impl &I = *impl;
-  try { sync(); } catch (...) {}
-  for (ncclComm_t c : I.comm)
-    if (c) ncclCommDestroy(c);
-  I.agents.clear();                                    // problems first: they use the streams
-  for (unsigned g = 0; g < I.N; ++g) {
-    if (I.N > 1 && I.send[g]) dpgo_device_free((int)g, I.send[g]);
-    if (I.gathered[g]) dpgo_device_free((int)g, I.gathered[g]);
-    if (g < I.gatheredAux.size()) {
-      if (I.N > 1 && I.sendAux[g]) dpgo_device_free((int)g, I.sendAux[g]);
-      if (I.gatheredAux[g]) dpgo_device_free((int)g, I.gatheredAux[g]);
-    }
-    if (g < I.statusDev.size() && I.statusDev[g]) dpgo_device_free((int)g, I.statusDev[g]);
-    if (I.N > 1 && g < I.statusAll.size() && I.statusAll[g]) dpgo_device_free((int)g, I.statusAll[g]);
-    if (I.stream[g]) dpgo_stream_destroy((int)g, I.stream[g]);
-  }
-  dpgo_host_free_pinned(I.statusHost);
-}
+DeviceRBCD::~DeviceRBCD() = default;
 
 // Wave w >= 1 (ref src/PGOAgent.cpp:369-440, examples/MultiRobotExample.cpp:245-256): one exchange of the public tiles;
 // every agent that is not initialised and has a neighbour initialised before the wave tries those neighbours in increasing
@@ -428,10 +459,10 @@ void DeviceRBCD::alignWaves() {
     for (unsigned g = 0; g < I.N; ++g) {
       std::vector<dpgo_problem *> hs;
       for (unsigned a : todo)
-        if ((unsigned)I.gpuOf[a] == g) hs.push_back(I.h[a]);
+        if (a / I.perGpu == g) hs.push_back(I.h[a]);
       if (!hs.empty())
-        check(dpgo_agents_align_async(hs.data(), (int)hs.size(), I.gathered[g], (int64_t)I.K * I.pmax, ready.data(), (int)I.K,
-                                      I.stream[g]),
+        check(dpgo_agents_align_async(hs.data(), (int)hs.size(), I.gpu[g].tiles.all.get(), I.numSlots, ready.data(), (int)I.K,
+                                      I.gpu[g].stream.get()),
               "dpgo_agents_align_async");
     }
     std::vector<unsigned> newly;
@@ -458,24 +489,18 @@ void DeviceRBCD::alignWaves() {
   }
 }
 
-size_t DeviceRBCD::allGatherBytesPerGpu() const { return sizeof(double) * impl->perGpu * impl->pmax * impl->ts; }
+size_t DeviceRBCD::allGatherBytesPerGpu() const { return sizeof(double) * impl->perGpu * impl->slotElems; }
 
 void DeviceRBCD::exchange() {
   Impl &I = *impl;
-  const size_t slotElems = (size_t)I.pmax * I.ts;
-  for (unsigned a = 0; a < I.K; ++a) {
-    const size_t g = (size_t)I.gpuOf[a];
-    double *dst = (I.N == 1) ? I.gathered[g] + a * slotElems : I.send[g] + (a % I.perGpu) * slotElems;
-    check(dpgo_agent_pack_public(I.h[a], dst), "dpgo_agent_pack_public");
-  }
-  I.allGather(I.send, I.gathered);
-  for (unsigned a = 0; a < I.K; ++a)
-    check(dpgo_agent_build_G(I.h[a], I.gathered[(size_t)I.gpuOf[a]], (int64_t)I.K * I.pmax), "dpgo_agent_build_G");
+  for (unsigned a = 0; a < I.K; ++a) check(dpgo_agent_pack_public(I.h[a], I.tileDst(a)), "dpgo_agent_pack_public");
+  I.allGather(&Gpu::tiles, I.slotElems);
+  I.buildG();
 }
 
 void DeviceRBCD::sync() {
   Impl &I = *impl;
-  for (unsigned g = 0; g < I.N; ++g) check(dpgo_stream_synchronize((int)g, I.stream[g]), "dpgo_stream_synchronize");
+  for (unsigned g = 0; g < I.N; ++g) check(dpgo_stream_synchronize((int)g, I.gpu[g].stream.get()), "dpgo_stream_synchronize");
 }
 
 static std::vector<unsigned> activeSet(const std::string &schedule, unsigned K, unsigned selected, unsigned round,
@@ -494,31 +519,22 @@ bool DeviceRBCD::concurrent() const { return impl->concurrent; }
 // one all-gather group per buffer, per GPU one call for the active agents (G from the Y tiles, step from Y, V, restart)
 void DeviceRBCD::roundAccelerated(const std::vector<unsigned> &active) {
   Impl &I = *impl;
-  const size_t slotElems = (size_t)I.pmax * I.ts;
-  for (unsigned g = 0; g < I.N; ++g) {
-    std::vector<dpgo_problem *> hs;
+  for (Gpu &G : I.gpu) {
     std::vector<int32_t> flags;
-    std::vector<double *> sx, sy;
-    for (unsigned a = g * I.perGpu; a < (g + 1) * I.perGpu; ++a) {
-      const size_t off = (I.N == 1 ? a : a % I.perGpu) * slotElems;
-      hs.push_back(I.h[a]);
-      flags.push_back(std::find(active.begin(), active.end(), a) != active.end() ? 1 : 0);
-      sx.push_back(I.send[g] + off);
-      sy.push_back(I.sendAux[g] + off);
-    }
-    check(dpgo_agents_accel_begin_async(hs.data(), (int)hs.size(), flags.data(), I.momentumN, (int)I.restartInterval, sx.data(),
-                                        sy.data(), I.stream[g]),
+    for (int32_t a : G.ids) flags.push_back(std::find(active.begin(), active.end(), (unsigned)a) != active.end() ? 1 : 0);
+    check(dpgo_agents_accel_begin_async(G.handles.data(), (int)G.handles.size(), flags.data(), I.momentumN,
+                                        (int)I.restartInterval, G.tileDst.data(), G.auxTileDst.data(), G.stream.get()),
           "dpgo_agents_accel_begin_async");
   }
-  I.allGather(I.send, I.gathered);
-  I.allGather(I.sendAux, I.gatheredAux);
+  I.allGather(&Gpu::tiles, I.slotElems);
+  I.allGather(&Gpu::auxTiles, I.slotElems);
   for (unsigned g = 0; g < I.N; ++g) {
     std::vector<dpgo_problem *> hs;
     for (unsigned a : active)
-      if ((unsigned)I.gpuOf[a] == g) hs.push_back(I.h[a]);
+      if (a / I.perGpu == g) hs.push_back(I.h[a]);
     if (hs.empty()) continue;
-    check(dpgo_agents_accel_round_async(hs.data(), (int)hs.size(), &I.prm, I.gathered[g], I.gatheredAux[g], (int64_t)I.K * I.pmax,
-                                        I.stream[g]),
+    check(dpgo_agents_accel_round_async(hs.data(), (int)hs.size(), &I.prm, I.gpu[g].tiles.all.get(), I.gpu[g].auxTiles.all.get(),
+                                        I.numSlots, I.gpu[g].stream.get()),
           "dpgo_agents_accel_round_async");
   }
   I.gatheredCurrent = false;                           // the gathered X tiles predate the active agents' steps
@@ -539,21 +555,20 @@ std::vector<unsigned> DeviceRBCD::issueRound() {
     roundAccelerated(active);
   } else {
     if (!I.gatheredCurrent) { exchange(); I.gatheredCurrent = true; }
-    const size_t slotElems = (size_t)I.pmax * I.ts;
     for (unsigned g = 0; g < I.N; ++g) {
       std::vector<dpgo_problem *> hs;
       std::vector<double *> dst;
       for (unsigned a : active)
-        if ((unsigned)I.gpuOf[a] == g) {
+        if (a / I.perGpu == g) {
           hs.push_back(I.h[a]);
-          dst.push_back((I.N == 1) ? I.gathered[g] + a * slotElems : I.send[g] + (a % I.perGpu) * slotElems);
+          dst.push_back(I.tileDst(a));
         }
       if (hs.empty()) continue;
-      check(dpgo_agents_round_async(hs.data(), (int)hs.size(), &I.prm, I.gathered[g], (int64_t)I.K * I.pmax, dst.data(),
-                                    I.stream[g], I.schedule == "parallel"),
+      check(dpgo_agents_round_async(hs.data(), (int)hs.size(), &I.prm, I.gpu[g].tiles.all.get(), I.numSlots, dst.data(),
+                                    I.gpu[g].stream.get(), I.schedule == "parallel"),
             "dpgo_agents_round_async");
     }
-    I.allGather(I.send, I.gathered);
+    I.allGather(&Gpu::tiles, I.slotElems);
   }
   ++mRound;
   return active;
@@ -567,21 +582,11 @@ void DeviceRBCD::selectRound() {
   Impl &I = *impl;
   if (!I.gatheredCurrent) { exchange(); I.gatheredCurrent = true; }
   if (!I.recordsCurrent) statusDevice();
-  const size_t slotElems = (size_t)I.pmax * I.ts;
-  for (unsigned g = 0; g < I.N; ++g) {
-    std::vector<dpgo_problem *> hs;
-    std::vector<int32_t> idx;
-    std::vector<double *> dst;
-    for (unsigned a = g * I.perGpu; a < (g + 1) * I.perGpu; ++a) {
-      hs.push_back(I.h[a]);
-      idx.push_back((int32_t)a);
-      dst.push_back((I.N == 1) ? I.gathered[g] + a * slotElems : I.send[g] + (a % I.perGpu) * slotElems);
-    }
-    check(dpgo_agents_select_round_async(hs.data(), (int)hs.size(), idx.data(), &I.prm, I.statusAll[g], I.gathered[g],
-                                         (int64_t)I.K * I.pmax, dst.data(), I.stream[g]),
+  for (Gpu &G : I.gpu)
+    check(dpgo_agents_select_round_async(G.handles.data(), (int)G.handles.size(), G.ids.data(), &I.prm, G.records.all.get(),
+                                         G.tiles.all.get(), I.numSlots, G.tileDst.data(), G.stream.get()),
           "dpgo_agents_select_round_async");
-  }
-  I.allGather(I.send, I.gathered);
+  I.allGather(&Gpu::tiles, I.slotElems);
   I.recordsCurrent = false;
   ++mRound;
 }
@@ -635,12 +640,12 @@ DeviceRBCDStatus DeviceRBCD::status() {
   constexpr unsigned S = DPGO_STATUS_DOUBLES;
   statusDevice();
   for (unsigned g = 0; g < I.N; ++g)
-    check(dpgo_copy_to_host_async((int)g, I.statusHost + (size_t)g * I.perGpu * S, I.statusDev[g], sizeof(double) * S * I.perGpu,
-                                  I.stream[g]),
+    check(dpgo_copy_to_host_async((int)g, I.statusHost.get() + (size_t)g * I.perGpu * S, I.gpu[g].records.own(),
+                                  sizeof(double) * S * I.perGpu, I.gpu[g].stream.get()),
           "dpgo_copy_to_host_async");
   sync();
   DeviceRBCDStatus st;
-  st.records.assign(I.statusHost, I.statusHost + (size_t)S * I.K);
+  st.records.assign(I.statusHost.get(), I.statusHost.get() + (size_t)S * I.K);
   double gn2 = 0;
   for (unsigned a = 0; a < I.K; ++a) {
     st.cost += st.at(a, 0) + st.at(a, 1);
@@ -653,40 +658,16 @@ DeviceRBCDStatus DeviceRBCD::status() {
 // every agent's status record on the device (G first, from the current tiles), N > 1: all-gathered; no synchronisation
 void DeviceRBCD::statusDevice() {
   Impl &I = *impl;
-  constexpr unsigned S = DPGO_STATUS_DOUBLES;
   if (I.gatheredCurrent) {
-    for (unsigned a = 0; a < I.K; ++a)
-      check(dpgo_agent_build_G(I.h[a], I.gathered[(size_t)I.gpuOf[a]], (int64_t)I.K * I.pmax), "dpgo_agent_build_G");
+    I.buildG();
   } else {
     exchange();
     I.gatheredCurrent = true;
   }
-  if (I.statusDev.empty()) {
-    I.statusDev.assign(I.N, nullptr);
-    for (unsigned g = 0; g < I.N; ++g) {
-      void *p = nullptr;
-      check(dpgo_device_malloc((int)g, sizeof(double) * S * I.perGpu, &p), "dpgo_device_malloc");
-      I.statusDev[g] = static_cast<double *>(p);
-    }
-    I.statusAll = I.statusDev;
-    if (I.N > 1)
-      for (unsigned g = 0; g < I.N; ++g) {
-        void *p = nullptr;
-        check(dpgo_device_malloc((int)g, sizeof(double) * S * I.K, &p), "dpgo_device_malloc");
-        I.statusAll[g] = static_cast<double *>(p);
-      }
-    void *hp = nullptr;
-    check(dpgo_host_alloc_pinned(sizeof(double) * S * I.K, &hp), "dpgo_host_alloc_pinned");
-    I.statusHost = static_cast<double *>(hp);
-  }
-  std::vector<int32_t> slots(I.perGpu);
-  for (unsigned i = 0; i < I.perGpu; ++i) slots[i] = (int32_t)i;
-  for (unsigned g = 0; g < I.N; ++g) {                  // a GPU hosts the contiguous block of agents g * perGpu ...
-    std::vector<dpgo_problem *> hs(I.h.begin() + (size_t)g * I.perGpu, I.h.begin() + (size_t)(g + 1) * I.perGpu);
-    check(dpgo_agents_status_async(hs.data(), (int)hs.size(), slots.data(), I.statusDev[g], I.stream[g]),
+  for (Gpu &G : I.gpu)
+    check(dpgo_agents_status_async(G.handles.data(), (int)G.handles.size(), I.slots.data(), G.records.own(), G.stream.get()),
           "dpgo_agents_status_async");
-  }
-  I.allGatherRecords();
+  I.allGather(&Gpu::records, DPGO_STATUS_DOUBLES);
   I.recordsCurrent = true;
 }
 

@@ -1,7 +1,7 @@
 """Setup calls repeated on live problem handles.  Every setup path (set_edges with its preconditioners, the public poses,
 the shared edges, the alignment candidates, accel_init, the agent graph) replaces the device buffers it owns; a second
 pass of the same calls on the same handles must give the same rounds bit for bit.  Handles destroyed and re-created in
-one process must keep working."""
+one process must keep working.  The C++ runner releases every resource it creates, also when its constructor throws."""
 import os
 
 import numpy as np
@@ -91,3 +91,45 @@ def test_handles_destroyed_and_recreated():
             ag.mProblem.close()
         del run
         gc.collect()
+
+
+@pytest.fixture(scope="module")
+def runner_lifetime_check():
+    from dpo_b200 import build
+    return build.build_cpp_program([os.path.join(ROOT, "tests", "cpp", "runner_lifetime_check.cpp")],
+                                   os.path.join(ROOT, "build", "tests", "runner_lifetime_check"))
+
+
+def _device_count():
+    import ctypes
+    from dpo_b200 import _capi
+    c = ctypes.c_int(0)
+    _capi.load_library().dpgo_device_count(ctypes.byref(c))
+    return c.value
+
+
+@pytest.mark.parametrize("gpus", [1, 2])
+def test_cpp_runner_releases_its_resources(gpus, runner_lifetime_check):
+    """DPGO::DeviceRBCD releases every stream, device buffer, pinned buffer and NCCL communicator it creates: when its
+    constructor throws (the distributed initialisation of a disconnected agent graph), and after solve() / status() with
+    accelerated coloured rounds and after step() / selectionLog() with greedy_set rounds."""
+    import subprocess
+    if gpus > _device_count():
+        pytest.skip(f"needs {gpus} GPUs")
+    res = subprocess.run([runner_lifetime_check, os.path.join(DATA, "smallGrid3D.g2o"), str(gpus)], capture_output=True,
+                         text=True, timeout=600)
+    assert res.returncode == 0, res.stderr[-2000:]
+    lines = res.stdout.splitlines()
+    assert any(ln.startswith("error a ") and "agents [3]" in ln for ln in lines), res.stdout
+    counts = {}
+    for ln in lines:
+        w = ln.split()
+        if w[0] == "counts":
+            counts[w[1]] = dict(zip(w[2::2], map(int, w[3::2])))
+    assert sorted(counts) == ["a", "b", "c"], res.stdout
+    for case, c in counts.items():
+        assert c["dpgo_stream_create"] == gpus and c["dpgo_device_malloc"] > 0, (case, c)
+        assert c["ncclCommInitAll"] == (gpus if gpus > 1 else 0), (case, c)
+        for create, release in [("dpgo_stream_create", "dpgo_stream_destroy"), ("dpgo_device_malloc", "dpgo_device_free"),
+                                ("dpgo_host_alloc_pinned", "dpgo_host_free_pinned"), ("ncclCommInitAll", "ncclCommDestroy")]:
+            assert c[create] == c[release], (case, create, c)
