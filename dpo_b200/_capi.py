@@ -105,6 +105,10 @@ SIGNATURES = {
     "dpgo_chordal_initialization": (C.c_int, [C.c_int, C.c_int, C.c_int64, _ip, _ip, _dp, _dp, _dp, _dp, C.c_int, C.c_double,
                                               C.c_int, _dp, _ip]),
     "dpgo_chordal_last_error": (C.c_char_p, []),
+    "dpgo_pose_covariances": (C.c_int, [C.c_int, C.c_int, C.c_int64, _ip, _ip, _dp, _dp, _dp, _dp, _dp, _dp, C.c_int, C.c_int,
+                                        C.c_int64, _ip, _dp, _dp, C.POINTER(C.c_int64)]),
+    "dpgo_pose_covariances_debug_emulate": (C.c_int, [C.c_int, C.c_int, C.c_int64, _ip, _ip, _dp, _dp, _dp, _dp, _dp, _dp, C.c_int,
+                                                      C.c_int, C.c_int, C.c_int64, _ip, _dp, _dp, C.POINTER(C.c_int64)]),
     "dpgo_device_set": (C.c_int, [C.c_int]),
     "dpgo_device_malloc": (C.c_int, [C.c_int, C.c_size_t, C.POINTER(_vp)]),
     "dpgo_device_free": (C.c_int, [C.c_int, _vp]),

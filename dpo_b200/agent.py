@@ -607,6 +607,7 @@ class DistributedPGO:
         self.torch = torch
         self.dist = dist
         self.k, self.n, self.r, self.d = k, n, r, edges.d
+        self.edges = edges
         self.rank = rank
         self.distributed = dist is not None and world is not None and world > 1
         self.world = world if self.distributed else 1
@@ -1132,3 +1133,13 @@ class DistributedPGO:
             cols = (self.glob[a][:, None] * dh + np.arange(dh)[None, :]).ravel()
             T[:, cols] = out
         return T
+
+    def pose_covariances(self, anchor: Optional[int] = None, pairs=None):
+        """Marginal covariances of the rounded trajectory() (pg.poseCovariancesGPU on this process's GPU), anchored at
+        agent 0's pose 0, the gauge of trajectory(), unless `anchor` names another global pose.  Single-process runs only:
+        the whole graph and trajectory must be on this process."""
+        if self.distributed:
+            raise ValueError("pose_covariances() needs the whole pose graph in one process: a multi-rank run holds only its "
+                             "own agents' poses (call pg.poseCovariancesGPU on a gathered trajectory instead)")
+        a = int(self.glob[0][0]) if anchor is None else int(anchor)
+        return pg.poseCovariancesGPU(self.edges, self.n, self.trajectory(), anchor=a, pairs=pairs, device=self.dev.index or 0)

@@ -16,9 +16,10 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdpgo_b200.so")
 SOURCES = ["dpgo_kernels.cu", "dpgo_spmv_tma.cu", "dense_inverse.cu", "dpgo_capi.cu", "dpgo_capi_precond.cu",
            "dpgo_capi_edges.cu", "dpgo_capi_agents.cu", "dpgo_chordal.cu", "dpgo_align.cu", "dpgo_status.cu",
-           "dpgo_accel.cu", "dpgo_select.cu", "nd_refactor.cu"]
+           "dpgo_accel.cu", "dpgo_select.cu", "nd_refactor.cu", "dpgo_covariance.cu", "dpgo_capi_covariance.cu"]
 HOST_ONLY_SOURCES = ["nd_precond.cpp"]          # host planning code inside libdpgo_b200.so (g++, OpenMP)
-HEADERS = ["dpgo_device.cuh", "dpgo_devbuf.cuh", "dpgo_handle.cuh", "dpgo_kernels.cuh", "dpgo_rotation.cuh", "nd_precond.h", os.path.join("..", "..", "include", "dpgo_b200.h")]
+HEADERS = ["dpgo_device.cuh", "dpgo_devbuf.cuh", "dpgo_handle.cuh", "dpgo_kernels.cuh", "dpgo_rotation.cuh", "nd_precond.h",
+           "dpgo_covariance.cuh", os.path.join("..", "..", "include", "dpgo_b200.h")]
 HOST_ONLY_FLAGS = ["-O3", "-std=c++17", "-fPIC", "-fvisibility=hidden", "-fopenmp", "-mavx2", "-mfma", "-Wall"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # Hopper with the architecture-specific features the kernels use (bulk TMA copies, mbarrier transaction counts,

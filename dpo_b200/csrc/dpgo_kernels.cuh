@@ -164,6 +164,37 @@ cudaError_t launch_nd_refactor(const KRefactor &k, const nd::Refactor &R, cudaSt
 cudaError_t launch_jacobi_blocks(int n, int dh, const int *rowptr, const int *bcol, const double *bval, double shift, double *dinv,
                                  int *fail, cudaStream_t stream);
 
+// ---- pose covariances (dpgo_covariance.cu) ----
+// The Gauss-Newton information H of a trajectory in block-CSR form over 3-scalar nodes (d = 2: one per pose; d = 3: two,
+// w_i then v_i), blocks padded to 4 x 4 as the factorisation reads them: bval[b][k][c] = H[3 node.x + k, 3 node.y + c].
+// Block b sums its contributions contrib[cptr[b] .. cptr[b+1]) = {edge, role of node.x | role of node.y << 1} in that
+// order; the anchor's nodes are identity blocks without coupling.
+struct KPoseInfo {
+  int d, anchor;
+  int64_t nb;
+  const int *cptr;
+  const int2 *contrib, *bnode;       // bnode[b] = {column node, row node}
+  const int *p1, *p2;
+  const double *T, *R, *t, *kappa, *tau, *w;   // T: d x (d+1)n column-major; R, t, kappa, tau as in dpgo_pose_covariances; w nullable
+  double *bval;
+};
+cudaError_t launch_assemble_pose_info(const KPoseInfo &k, cudaStream_t stream);
+// One 3 x 3 block of a front inverse: rows ra.., columns rc.. of refactor node `node`'s front -> out[x * ld + y].
+struct CovItem { int node, ra, rc, pad; long long out; };
+// Selected inversion over the fronts of a factorisation with shift 0 (nd::Selinv), root stage first; the items of stage st
+// are items[item0[st] .. item0[st+1]).
+struct KSelinv {
+  const nd::RefactorNode *nodes;
+  const int *parent, *pmap0, *pmap;
+  const double *blob;
+  double *arena;                     // front inverses, in the refactorisation's arena layout
+  const CovItem *items;
+  double *out;
+  int ld;
+};
+cudaError_t launch_nd_selinv(const KSelinv &k, const nd::Refactor &R, const nd::Selinv &S, const std::vector<int> &item0,
+                             cudaStream_t stream);
+
 // ---- frame alignment of the distributed initialisation (dpgo_align.cu) ----
 // One aligning agent.  Its candidates are grouped per neighbour (group g = candidates [grp_ptr[g], grp_ptr[g+1]) against
 // agent grp_nbr[g], groups in increasing neighbour id); candidate q pairs local pose cand_local[q] with the gathered tile

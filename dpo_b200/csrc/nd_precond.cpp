@@ -677,6 +677,81 @@ void build_refactor(const Hierarchy &H, Refactor &R) {
   R.ws_doubles = std::max<int64_t>(ws, 1);
 }
 
+void build_selinv(const Hierarchy &H, const Refactor &R, Selinv &S) {
+  const size_t nn = R.nodes.size();
+  S = Selinv();
+  std::vector<int> order(H.nodes.size());
+  std::iota(order.begin(), order.end(), 0);
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return H.nodes[(size_t)a].stage < H.nodes[(size_t)b].stage; });
+  std::vector<int> idx(H.nodes.size());
+  for (size_t q = 0; q < nn; ++q) idx[(size_t)order[q]] = (int)q;
+  S.macro = order;
+  S.parent.assign(nn, -1);
+  S.pmap0.assign(nn, 0);
+  S.max_b.assign((size_t)H.nstages, 0);
+  std::vector<int> where((size_t)H.n, -1);
+  for (size_t q = 0; q < nn; ++q) {
+    const MacroNode &mn = H.nodes[(size_t)order[q]];
+    S.max_b[(size_t)mn.stage] = std::max(S.max_b[(size_t)mn.stage], H.dh * (int)mn.bnd.size());
+    S.pmap0[q] = (int)S.pmap.size();
+    if (mn.parent < 0) {
+      if (!mn.bnd.empty()) throw std::runtime_error("nd: a root node with boundary poses");
+      continue;
+    }
+    const int pq = idx[(size_t)mn.parent];
+    S.parent[q] = pq;
+    const RefactorNode &pn = R.nodes[(size_t)pq];
+    for (int k = 0; k < pn.no + pn.nb; ++k) where[(size_t)R.poses[(size_t)pn.pose0 + k]] = k;
+    for (int p : mn.bnd) {
+      if (where[(size_t)p] < 0) throw std::runtime_error("nd: boundary pose outside the parent front");
+      S.pmap.push_back(where[(size_t)p]);
+    }
+    for (int k = 0; k < pn.no + pn.nb; ++k) where[(size_t)R.poses[(size_t)pn.pose0 + k]] = -1;
+  }
+  if (S.pmap.empty()) S.pmap.push_back(0);
+}
+
+void emulate_selinv(const Hierarchy &H, const Refactor &R, const Selinv &S, const std::vector<double> &blob,
+                    std::vector<std::vector<double>> &front) {
+  const int dh = H.dh;
+  const size_t nn = R.nodes.size();
+  front.assign(nn, {});
+  for (size_t qq = nn; qq-- > 0;) {                       // root stage first (R is ordered deepest first)
+    const RefactorNode &rn = R.nodes[qq];
+    const int64_t s = (int64_t)dh * rn.no, b = (int64_t)dh * rn.nb, M = s + b;
+    std::vector<double> &F = front[qq];
+    F.assign((size_t)(M * M), 0.0);
+    const double *gf = blob.data() + rn.gf, *gb = blob.data() + rn.gb;
+    auto W = [&](int64_t r, int64_t j) { return gf[(r / dh / 2) * PANEL_ROWS * s + j * PANEL_ROWS + (r / dh % 2) * dh + r % dh]; };
+    auto Fm = [&](int64_t i, int64_t k) { return gb[(i / dh / 2) * PANEL_ROWS * b + k * PANEL_ROWS + (i / dh % 2) * dh + i % dh]; };
+    for (int64_t c = 0; c < s; ++c)
+      for (int64_t r = 0; r < s; ++r) F[(size_t)(r + M * c)] = W(r, c);
+    if (b > 0) {
+      const std::vector<double> &Pf = front[(size_t)S.parent[qq]];
+      const RefactorNode &pn = R.nodes[(size_t)S.parent[qq]];
+      const int64_t Mp = (int64_t)dh * (pn.no + pn.nb);
+      const int *pm = S.pmap.data() + S.pmap0[qq];
+      for (int64_t c = 0; c < b; ++c)
+        for (int64_t r = 0; r < b; ++r) {
+          const int64_t pr = pm[r / dh] * dh + r % dh, pc = pm[c / dh] * dh + c % dh;
+          F[(size_t)(s + r + M * (s + c))] = pr <= pc ? Pf[(size_t)(pr + Mp * pc)] : Pf[(size_t)(pc + Mp * pr)];
+        }
+      for (int64_t j = 0; j < b; ++j)                     // Sigma_ob = -Fm Sigma_bb
+        for (int64_t i = 0; i < s; ++i) {
+          double acc = 0.0;
+          for (int64_t k = 0; k < b; ++k) acc = std::fma(Fm(i, k), F[(size_t)(s + k + M * (s + j))], acc);
+          F[(size_t)(i + M * (s + j))] = -acc;
+        }
+      for (int64_t j = 0; j < s; ++j)                     // Sigma_oo = W - Sigma_ob Fm^T (upper triangle)
+        for (int64_t i = 0; i <= j; ++i) {
+          double acc = 0.0;
+          for (int64_t k = 0; k < b; ++k) acc = std::fma(F[(size_t)(i + M * (s + k))], Fm(j, k), acc);
+          F[(size_t)(i + M * j)] -= acc;
+        }
+    }
+  }
+}
+
 // =================================================================================================================
 // 3. plan
 // =================================================================================================================

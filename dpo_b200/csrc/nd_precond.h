@@ -153,5 +153,24 @@ struct Refactor {
 // Throws std::runtime_error when a child is not exactly one stage below its parent (the arena parity relies on it).
 void build_refactor(const Hierarchy &H, Refactor &R);
 
+// ---- selected inversion over the same fronts (dpgo_covariance.cu): with W = Foo^-1 and Fm = W Fob of every node (the
+// panels a factorisation with shift 0 leaves), the front inverse  Sigma_front = (A^-1) restricted to the node's front poses
+// follows from the parent's, root to leaves:
+//     Sigma_bb = parent's Sigma_front at the node's boundary poses,   Sigma_ob = -Fm Sigma_bb,   Sigma_oo = W - Sigma_ob Fm^T.
+// Fronts are M x M column-major (M = dh (own + bnd), own then bnd) and only their upper triangle (row <= col) is read.
+// pmap: per refactor node (R's order), the position of each of its boundary poses in its parent's front; pmap0 / parent.
+struct Selinv {
+  std::vector<int> parent;    // refactor index of the parent, -1 at a root
+  std::vector<int> pmap0;     // offset into pmap (nb entries per node)
+  std::vector<int> pmap;
+  std::vector<int> macro;     // refactor index -> macro node (H.nodes index)
+  std::vector<int> max_b;     // per stage: largest boundary (scalars)
+};
+void build_selinv(const Hierarchy &H, const Refactor &R, Selinv &S);
+// HOST ONLY, verification: the sweep of the device selected inversion, with the same recurrence and the same summation
+// order, over the panels of build_numeric (Options::shift = 0).  front[q] (refactor order) receives node q's front inverse.
+void emulate_selinv(const Hierarchy &H, const Refactor &R, const Selinv &S, const std::vector<double> &blob,
+                    std::vector<std::vector<double>> &front);
+
 }  // namespace nd
 }  // namespace dpgo

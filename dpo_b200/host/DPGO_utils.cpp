@@ -7,6 +7,7 @@
 
 #include "dpgo_b200.h"
 
+#include <algorithm>
 #include <cmath>
 #include <fstream>
 #include <sstream>
@@ -328,6 +329,45 @@ Matrix chordalInitializationGPU(size_t dimension, size_t num_poses, const std::v
                                   device, tol, 0, T.data(), nullptr) != DPGO_OK)
     throw std::runtime_error(std::string("dpgo_chordal_initialization: ") + dpgo_chordal_last_error());
   return T;
+}
+
+PoseCovariances poseCovariancesGPU(size_t dimension, size_t num_poses, const std::vector<RelativeSEMeasurement> &measurements,
+                                   const Matrix &T, size_t anchor, const std::vector<std::pair<size_t, size_t>> &pairs,
+                                   int device) {
+  const size_t d = dimension, m = measurements.size(), n = num_poses, b = d == 3 ? 6 : 3;
+  if ((size_t)T.rows() != d || (size_t)T.cols() != (d + 1) * n)
+    throw std::runtime_error("poseCovariancesGPU: the trajectory must be d x (d+1)n");
+  std::vector<int32_t> p1(m), p2(m), pr(2 * pairs.size());
+  std::vector<double> R(m * d * d), t(m * d), kappa(m), tau(m), weight(m);
+  for (size_t e = 0; e < m; ++e) {
+    const RelativeSEMeasurement &ms = measurements[e];
+    p1[e] = (int32_t)ms.p1;
+    p2[e] = (int32_t)ms.p2;
+    for (size_t a = 0; a < d; ++a) {
+      for (size_t c = 0; c < d; ++c) R[e * d * d + a * d + c] = ms.R(a, c);
+      t[e * d + a] = ms.t(a);
+    }
+    kappa[e] = ms.kappa;
+    tau[e] = ms.tau;
+    weight[e] = ms.weight;
+  }
+  for (size_t q = 0; q < pairs.size(); ++q) { pr[2 * q] = (int32_t)pairs[q].first; pr[2 * q + 1] = (int32_t)pairs[q].second; }
+  if (device < 0) { const char *ev = std::getenv("DPGO_DEVICE"); device = ev ? std::atoi(ev) : 0; }
+  std::vector<double> cov(n * b * b), pcov(std::max<size_t>(pairs.size(), 1) * b * b);
+  if (dpgo_pose_covariances((int)n, (int)d, (int64_t)m, p1.data(), p2.data(), R.data(), t.data(), kappa.data(), tau.data(),
+                            weight.data(), T.data(), (int)anchor, device, (int64_t)pairs.size(), pr.data(), cov.data(),
+                            pcov.data(), nullptr) != DPGO_OK)
+    throw std::runtime_error(std::string("dpgo_pose_covariances: ") + dpgo_last_error());
+  auto block = [&](const double *src) {                  // row-major b x b
+    Matrix M((Eigen::Index)b, (Eigen::Index)b);
+    for (size_t a = 0; a < b; ++a)
+      for (size_t c = 0; c < b; ++c) M((Eigen::Index)a, (Eigen::Index)c) = src[a * b + c];
+    return M;
+  };
+  PoseCovariances out;
+  for (size_t p = 0; p < n; ++p) out.pose.push_back(block(cov.data() + p * b * b));
+  for (size_t q = 0; q < pairs.size(); ++q) out.pair.push_back(block(pcov.data() + q * b * b));
+  return out;
 }
 
 Matrix chordalInitialization(size_t dimension, size_t num_poses, const std::vector<RelativeSEMeasurement> &measurements) {

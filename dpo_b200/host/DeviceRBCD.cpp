@@ -89,6 +89,7 @@ struct Gpu {
 struct DeviceRBCD::Impl {
   unsigned d = 3, r = 5, dh = 4, ts = 20, K = 1, N = 1, perGpu = 1, pmax = 1;
   size_t n = 0;
+  std::vector<RelativeSEMeasurement> graph;       // the global pose graph (poseCovariances)
   size_t slotElems = 0;            // one agent's padded public tiles: pmax * ts doubles
   int64_t numSlots = 0;            // the slots of a gathered tile buffer: K * pmax
   std::string schedule;
@@ -146,6 +147,7 @@ DeviceRBCD::DeviceRBCD(const std::vector<RelativeSEMeasurement> &graph, size_t n
   Impl &I = *impl;
   if (graph.empty()) throw std::runtime_error("DeviceRBCD: empty pose graph");
   I.d = (unsigned)graph[0].t.size();
+  I.graph = graph;
   I.r = opt.r;
   I.dh = I.d + 1;
   I.ts = I.r * I.dh;
@@ -718,6 +720,13 @@ Matrix DeviceRBCD::trajectory() {
     for (size_t q = 0; q < I.count[a]; ++q) T.block(0, I.globalOf[a][q] * I.dh, I.d, I.dh) = Ta.block(0, q * I.dh, I.d, I.dh);
   }
   return T;
+}
+
+PoseCovariances DeviceRBCD::poseCovariances(long anchor, const std::vector<std::pair<size_t, size_t>> &pairs) {
+  Impl &I = *impl;
+  const Matrix T = trajectory();
+  const size_t a = anchor < 0 ? I.globalOf[0][0] : (size_t)anchor;
+  return poseCovariancesGPU(I.d, I.n, I.graph, T, a, pairs, 0);
 }
 
 }  // namespace DPGO

@@ -297,6 +297,43 @@ def chordalInitializationGPU(d: int, n: int, edges: EdgeSet, device: int = 0, to
     return (T, (int(its[0]), int(its[1]))) if return_iterations else T
 
 
+def _covariance_args(edges: EdgeSet, n: int, T: np.ndarray, pairs):
+    d = edges.d
+    T = np.asfortranarray(np.asarray(T, dtype=np.float64))
+    if T.shape != (d, (d + 1) * n):
+        raise ValueError(f"expected a trajectory of shape {(d, (d + 1) * n)}, got {T.shape}")
+    pr = np.zeros((0, 2), dtype=np.int32) if pairs is None else np.ascontiguousarray(np.asarray(pairs, dtype=np.int32).reshape(-1, 2))
+    arrays = [np.ascontiguousarray(a, dtype=dt) for a, dt in ((edges.p1, np.int32), (edges.p2, np.int32), (edges.R, np.float64),
+                                                            (edges.t, np.float64), (edges.kappa, np.float64),
+                                                            (edges.tau, np.float64), (edges.weight, np.float64))]
+    b = 6 if d == 3 else 3
+    return T, pr, arrays, b
+
+
+def poseCovariancesGPU(edges: EdgeSet, n: int, T: np.ndarray, anchor: int = 0, pairs=None, device: int = 0,
+                       return_info: bool = False):
+    """Marginal covariances of the poses of trajectory T (d x (d+1)n, e.g. a rounded solution) under the Gauss-Newton
+    information of `edges`, with pose `anchor` fixed (dpgo_pose_covariances; the model is in include/dpgo_b200.h).
+
+    Returns cov (n, b, b), b = 6 (SE(3): rotation then translation) or 3 (SE(2): angle then translation), the anchor's
+    block 0; with pairs (k, 2) also the cross blocks Sigma[x_i, x_j] (k, b, b); with return_info also info16.
+    The graph is assembled, factored and selectively inverted on the GPU; edge weights are honoured."""
+    import ctypes as C
+    from . import _capi as capi
+    lib = capi.load_library()
+    T, pr, (p1, p2, R, t, kappa, tau, w), b = _covariance_args(edges, n, T, pairs)
+    cov = np.zeros((n, b, b))
+    pcov = np.zeros((max(len(pr), 1), b, b))
+    info = (C.c_int64 * 16)()
+    capi.check(lib.dpgo_pose_covariances(n, edges.d, len(p1), capi.iptr(p1), capi.iptr(p2), capi.dptr(R), capi.dptr(t),
+                                         capi.dptr(kappa), capi.dptr(tau), capi.dptr(w), capi.dptr(T), int(anchor), device,
+                                         len(pr), capi.iptr(pr), capi.dptr(cov), capi.dptr(pcov), info))
+    out = (cov,) if pairs is None else (cov, pcov[:len(pr)])
+    if return_info:
+        out = out + (list(info),)
+    return out[0] if len(out) == 1 else out
+
+
 def synthetic_grid_graph(nx: int, ny: int, nz: int, edges_per_pose: float = 4.0, seed: int = 0,
                          rot_sigma: float = 0.05, trans_sigma: float = 0.1, kappa: float = 200.0,
                          tau: float = 100.0) -> Tuple[EdgeSet, int, np.ndarray]:

@@ -26,6 +26,17 @@ Matrix chordalInitialization(size_t dimension, size_t num_poses, const std::vect
 // kernel, dpgo_chordal_initialization); device < 0: env DPGO_DEVICE or 0.  Throws std::runtime_error on failure.
 Matrix chordalInitializationGPU(size_t dimension, size_t num_poses, const std::vector<RelativeSEMeasurement> &measurements,
                                 int device = -1, double tol = 1e-11);
+// GPU extension: marginal covariances of the poses of trajectory T (d x (d+1)n, e.g. DeviceRBCD::trajectory()) under the
+// Gauss-Newton information of the measurements (weights honoured), pose `anchor` fixed (dpgo_pose_covariances; the model
+// is in dpgo_b200.h).  pose[p]: b x b, b = 6 (3D: rotation then translation) or 3 (2D: angle then translation), the
+// anchor's block 0; pair[q]: the cross block Sigma[x_i, x_j] of pairs[q] = (i, j).  device < 0: env DPGO_DEVICE or 0.
+// Throws std::runtime_error on failure.
+struct PoseCovariances {
+  std::vector<Matrix> pose, pair;
+};
+PoseCovariances poseCovariancesGPU(size_t dimension, size_t num_poses, const std::vector<RelativeSEMeasurement> &measurements,
+                                   const Matrix &T, size_t anchor = 0,
+                                   const std::vector<std::pair<size_t, size_t>> &pairs = {}, int device = -1);
 Matrix odometryInitialization(size_t dimension, size_t num_poses, const std::vector<RelativeSEMeasurement> &odometry);
 
 // projections; ref src/DPGO_utils.cpp:463-492

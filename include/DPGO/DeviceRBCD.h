@@ -22,6 +22,7 @@
 #define DPGO_DEVICE_RBCD_H
 
 #include <DPGO/DPGO_types.h>
+#include <DPGO/DPGO_utils.h>
 #include <DPGO/PGOAgent.h>
 #include <DPGO/RelativeSEMeasurement.h>
 
@@ -131,6 +132,10 @@ class DeviceRBCD {
   // d x (d+1)n trajectory in global pose order, rounded on the device against agent 0's pose 0
   // (ref getTrajectoryInGlobalFrame, src/PGOAgent.cpp:500-519)
   Matrix trajectory();
+  // marginal covariances of trajectory() (poseCovariancesGPU on GPU 0), anchored at agent 0's pose 0 -- the gauge of
+  // trajectory() -- unless `anchor` names another global pose.  The runner holds the whole pose graph in this process
+  // (its GPUs are one process's), which is what the call needs.
+  PoseCovariances poseCovariances(long anchor = -1, const std::vector<std::pair<size_t, size_t>> &pairs = {});
   // greedy_set: the agents of rounds first .. first + count - 1 (those issued so far), each sorted; synchronises the GPUs
   std::vector<std::vector<unsigned>> selectionLog(unsigned first = 0, unsigned count = ~0u);
 

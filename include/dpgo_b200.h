@@ -283,6 +283,48 @@ DPGO_API int dpgo_chordal_initialization(int n, int d, int64_t m, const int32_t 
                                          int max_iter, double *T_host, int32_t *iterations2);
 DPGO_API const char *dpgo_chordal_last_error(void);
 
+/* ---- pose marginal covariances on the GPU ----------------------------------------------------------------------
+ * The uncertainty of a trajectory T (d x (d+1)n column-major, [R_p t_p] per pose: a rounded solution) under the
+ * Gauss-Newton information of the edges (p1, p2, R, t, kappa, tau as in dpgo_chordal_initialization; weight: m, nullable =
+ * all 1; every edge joins two different poses):
+ *   perturbation   right (body frame), R_p exp([w_p]x) and t_p + R_p v_p; tangent x_p = (w_p, v_p) of dimension
+ *                  b = 6 (d = 3) or b = 3 (d = 2, w_p the angle), in that order;
+ *   residuals      R_j - R_i R_ij (weight kappa) and t_j - t_i - R_i t_ij (weight tau) of every edge i -> j, scaled so
+ *                  that sum_e 1/2 r^T Om_e r (Om_e = weight diag(kappa .., tau ..)) is f = 1/2 <Q, T^T T> with Q the
+ *                  connection Laplacian;
+ *   information    H = sum_e J_e^T Om_e J_e at T (Gauss-Newton: positive semidefinite at any trajectory, with a null
+ *                  space of dimension b on a connected graph: the gauge);
+ *   covariance     Sigma = H_anchored^-1, the anchor pose's b rows and columns dropped (its blocks are reported as 0).
+ * cov_host receives the b x b diagonal block of every pose (n b b doubles, row-major blocks); pair_cov_host the b x b
+ * block Sigma[x_i, x_j] of each of the num_pairs pairs (i, j) = (pairs[2q], pairs[2q+1]).  Nothing dense: H is assembled,
+ * factored and selectively inverted on the device over the nested-dissection fronts of its block pattern, in fixed
+ * summation orders (two calls are bitwise equal).  The requested pairs join that pattern as structural blocks, so both
+ * poses of a pair share a front and every pair block is read from one.  That has a cost: each pair is an extra edge for
+ * the dissection, so many long-range pairs (loop-closure gating over a whole map) enlarge the separators, and the
+ * factorisation's work and device memory (info16[4]) grow with them, up to dense fronts; requesting pairs also changes
+ * the hierarchy, so the diagonal blocks of a call with pairs may differ in the last bits from one without.  Arguments
+ * (ranges, finite non-negative precisions and weights, a finite trajectory, every pose connected to the anchor by edges
+ * of positive weight and a positive kappa or tau) are checked before any device call (DPGO_ERR_INVALID_ARG).  That
+ * check is on the graph only: information that is still singular (a pose whose edges all have tau = 0, so its
+ * translation is free) fails in the factorisation with a pivot that is not positive (DPGO_ERR_CUDA), and information
+ * that is merely ill-conditioned returns its (large, fp64-accurate to about cond(H) eps) inverse.  info16 (nullable): 0 macro levels, 1 macro nodes, 2 3-scalar nodes of H (d = 2: n, d = 3: 2n),
+ * 3 blocks of H, 4 device bytes of H + factor + fronts, 5 largest own block (scalars), 6 largest boundary (scalars),
+ * 7 dissection depth, 8 3 x 3 output blocks, 9 stages (factor + sweep), 10 / 11 / 12 assembly / factorisation /
+ * selected-inversion nanoseconds (device events), others 0.  n = 1 needs no device.  Messages: dpgo_last_error(). */
+DPGO_API int dpgo_pose_covariances(int n, int d, int64_t m, const int32_t *p1, const int32_t *p2, const double *R,
+                                   const double *t, const double *kappa, const double *tau, const double *weight,
+                                   const double *T_host, int anchor, int device, int64_t num_pairs, const int32_t *pairs,
+                                   double *cov_host, double *pair_cov_host, int64_t *info16);
+/* HOST ONLY, verification on machines without a GPU (never used by a product path): the same pattern, hierarchy and
+ * output blocks as dpgo_pose_covariances, the assembly kernel's arithmetic on the host, the host factorisation
+ * (nd build_numeric, shift 0) and a host emulation of the selected-inversion sweep.  force_cuts < 0 lets the cost model
+ * choose the macro levels, leaf_size <= 0 keeps the default.  info16 as above without the times. */
+DPGO_API int dpgo_pose_covariances_debug_emulate(int n, int d, int64_t m, const int32_t *p1, const int32_t *p2,
+                                                 const double *R, const double *t, const double *kappa, const double *tau,
+                                                 const double *weight, const double *T_host, int anchor, int force_cuts,
+                                                 int leaf_size, int64_t num_pairs, const int32_t *pairs, double *cov_host,
+                                                 double *pair_cov_host, int64_t *info16);
+
 /* ---- plain device helpers for hosts that drive several GPUs without linking the CUDA runtime themselves (the C++
  *      multi-GPU runner: exchange buffers + one stream per GPU, NCCL calls on those streams) ---------------------- */
 DPGO_API int dpgo_device_set(int device);                                /* cudaSetDevice for the calling thread */
