@@ -151,13 +151,16 @@ __global__ void __launch_bounds__(256) k_gj_update(GjJob one, const GjJob *jobs,
 
 cudaError_t gj_sweep_batch(const GjJob *jobs_dev, int njobs, int max_M, int max_s, int *fail, cudaStream_t stream) {
   if (njobs <= 0 || max_s <= 0) return cudaSuccess;
-  if (njobs > 65535) return cudaErrorInvalidValue;
   const GjJob none = {};
   const int tiles = (max_M + GJT - 1) / GJT;
-  for (int k0 = 0; k0 < max_s; k0 += GJB) {
-    k_gj_pivot<<<dim3(1, njobs), dim3(GJB, GJB), 0, stream>>>(none, jobs_dev, k0, fail);
-    k_gj_panels<<<dim3((max_M + 255) / 256, njobs), 256, 0, stream>>>(none, jobs_dev, k0);
-    k_gj_update<<<dim3(tiles, tiles, njobs), 256, 0, stream>>>(none, jobs_dev, k0);
+  for (int j0 = 0; j0 < njobs; j0 += MAX_GRID_YZ) {          // the jobs are independent: slices run one after another
+    const GjJob *jobs = jobs_dev + j0;
+    const unsigned nj = (unsigned)(njobs - j0 < MAX_GRID_YZ ? njobs - j0 : MAX_GRID_YZ);
+    for (int k0 = 0; k0 < max_s; k0 += GJB) {
+      k_gj_pivot<<<dim3(1, nj), dim3(GJB, GJB), 0, stream>>>(none, jobs, k0, fail);
+      k_gj_panels<<<dim3((max_M + 255) / 256, nj), 256, 0, stream>>>(none, jobs, k0);
+      k_gj_update<<<dim3(tiles, tiles, nj), 256, 0, stream>>>(none, jobs, k0);
+    }
   }
   return cudaGetLastError();
 }

@@ -185,6 +185,7 @@ void fill_info(const CovProblem &P, const CovSetup &C, int64_t *info) {
   info[5] = smax; info[6] = bmax; info[7] = C.H.nd_depth;
   info[8] = (int64_t)C.item0.back();
   info[9] = 2 * (int64_t)C.H.nstages;                  // factor + sweep stages
+  for (size_t st = 0; st + 1 < C.R.stage0.size(); ++st) info[13] = std::max(info[13], (int64_t)(C.R.stage0[st + 1] - C.R.stage0[st]));
 }
 
 nd::Options cov_options(int force_cuts, int leaf_size) {

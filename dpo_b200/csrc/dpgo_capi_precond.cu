@@ -78,8 +78,6 @@ int ensure_refactor(dpgo_problem *p, int slot) {
   } catch (const std::exception &e) {
     return fail(DPGO_ERR_UNSUPPORTED, what + ": " + e.what());
   }
-  for (size_t st = 0; st + 1 < R->stage0.size(); ++st)
-    if (R->stage0[st + 1] - R->stage0[st] > 65535) return fail(DPGO_ERR_UNSUPPORTED, what + ": more than 65535 nodes in one stage");
   if (R->child.empty()) R->child.push_back({0, 0});        // one macro level: no children, nothing reads these
   if (R->cmap.empty()) R->cmap.push_back(-1);
   DPGO_CUDA(F.rnodes.assign(R->nodes.data(), R->nodes.size(), p->stream));

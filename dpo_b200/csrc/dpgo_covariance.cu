@@ -159,15 +159,18 @@ cudaError_t launch_nd_selinv(const KSelinv &k, const nd::Refactor &R, const nd::
   const int ns = (int)R.stage0.size() - 1;
   for (int st = ns - 1; st >= 0; --st) {
     const int n0 = R.stage0[(size_t)st], nn = R.stage0[(size_t)st + 1] - n0;
-    if (nn <= 0) continue;
-    if (nn > 65535) return cudaErrorInvalidValue;
+    if (nn <= 0 || R.max_nfr[(size_t)st] == 0) continue;     // no node of the stage holds a pose (an empty separator)
     const int64_t Mx = (int64_t)COV_DH * R.max_nfr[(size_t)st];
-    k_nd_selinv_gather<<<dim3((unsigned)((Mx * Mx + SEL_THREADS - 1) / SEL_THREADS), nn), SEL_THREADS, 0, stream>>>(k, n0);
     const int64_t smax = R.max_s[(size_t)st], bmax = S.max_b[(size_t)st];
-    if (bmax > 0) {
-      const unsigned ts = (unsigned)((smax + SEL_T - 1) / SEL_T), tb = (unsigned)((bmax + SEL_T - 1) / SEL_T);
-      k_nd_selinv_gemm<0><<<dim3(tb, ts, nn), SEL_THREADS, 0, stream>>>(k, n0);
-      k_nd_selinv_gemm<1><<<dim3(ts, ts, nn), SEL_THREADS, 0, stream>>>(k, n0);
+    const unsigned ts = (unsigned)((smax + SEL_T - 1) / SEL_T), tb = (unsigned)((bmax + SEL_T - 1) / SEL_T);
+    // the nodes of one stage are independent: a stage of more than MAX_GRID_YZ nodes runs in consecutive slices
+    for (int c0 = n0; c0 < n0 + nn; c0 += MAX_GRID_YZ) {
+      const unsigned nc = (unsigned)(n0 + nn - c0 < MAX_GRID_YZ ? n0 + nn - c0 : MAX_GRID_YZ);
+      k_nd_selinv_gather<<<dim3((unsigned)((Mx * Mx + SEL_THREADS - 1) / SEL_THREADS), nc), SEL_THREADS, 0, stream>>>(k, c0);
+      if (bmax > 0) {
+        k_nd_selinv_gemm<0><<<dim3(tb, ts, nc), SEL_THREADS, 0, stream>>>(k, c0);
+        k_nd_selinv_gemm<1><<<dim3(ts, ts, nc), SEL_THREADS, 0, stream>>>(k, c0);
+      }
     }
     const int a = item0[(size_t)st], z = item0[(size_t)st + 1];
     if (z > a) k_nd_selinv_extract<<<(unsigned)(((int64_t)(z - a) * 9 + 255) / 256), 256, 0, stream>>>(k, a, z);

@@ -137,8 +137,11 @@ struct GjJob {
   double *A, *piv, *Rw, *C;
   int M, s;
 };
-// Sweeps every job of jobs_dev (njobs <= 65535; max_M / max_s bound the jobs' sizes): 3 launches per 32 pivots, no
-// synchronisation.  A non-positive pivot sets *fail (nullable).
+// gridDim.y and gridDim.z are at most 65535: the batched launches that put one CTA set per matrix or per node there
+// (gj_sweep_batch, launch_nd_refactor, launch_nd_selinv) take a longer batch in consecutive slices of this many.
+constexpr int MAX_GRID_YZ = 65535;
+// Sweeps every job of jobs_dev (max_M / max_s bound the jobs' sizes): 3 launches per 32 pivots and slice of
+// MAX_GRID_YZ jobs, no synchronisation.  A non-positive pivot sets *fail (nullable).
 cudaError_t gj_sweep_batch(const GjJob *jobs_dev, int njobs, int max_M, int max_s, int *fail, cudaStream_t stream);
 
 // ---- numeric refactorisation of the exact preconditioners on the device (nd_refactor.cu) ----

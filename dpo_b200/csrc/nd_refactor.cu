@@ -142,14 +142,21 @@ cudaError_t launch_nd_refactor(const KRefactor &k, const nd::Refactor &R, cudaSt
   const int ns = (int)R.stage0.size() - 1;
   for (int st = 0; st < ns; ++st) {
     const int n0 = R.stage0[(size_t)st], nn = R.stage0[(size_t)st + 1] - n0;
-    if (nn <= 0) continue;
-    if (nn > 65535) return cudaErrorInvalidValue;
+    if (nn <= 0 || R.max_nfr[(size_t)st] == 0) continue;     // no node of the stage holds a pose: nothing to launch
+    // the nodes of one stage are independent: a stage of more than MAX_GRID_YZ nodes runs in consecutive slices
     const int64_t fb = (int64_t)R.max_nfr[(size_t)st] * R.max_nfr[(size_t)st];
-    k_nd_front<<<dim3((unsigned)((fb + REF_THREADS - 1) / REF_THREADS), nn), REF_THREADS, 0, stream>>>(k, n0);
+    for (int c0 = n0; c0 < n0 + nn; c0 += MAX_GRID_YZ) {
+      const unsigned nc = (unsigned)(n0 + nn - c0 < MAX_GRID_YZ ? n0 + nn - c0 : MAX_GRID_YZ);
+      k_nd_front<<<dim3((unsigned)((fb + REF_THREADS - 1) / REF_THREADS), nc), REF_THREADS, 0, stream>>>(k, c0);
+    }
     const cudaError_t e = gj_sweep_batch(k.jobs + n0, nn, k.dh * R.max_nfr[(size_t)st], R.max_s[(size_t)st], k.fail, stream);
     if (e != cudaSuccess) return e;
     const int64_t pb = R.max_blob[(size_t)st];
-    if (pb > 0) k_nd_pack<<<dim3((unsigned)((pb + REF_THREADS - 1) / REF_THREADS), nn), REF_THREADS, 0, stream>>>(k, n0);
+    if (pb > 0)
+      for (int c0 = n0; c0 < n0 + nn; c0 += MAX_GRID_YZ) {
+        const unsigned nc = (unsigned)(n0 + nn - c0 < MAX_GRID_YZ ? n0 + nn - c0 : MAX_GRID_YZ);
+        k_nd_pack<<<dim3((unsigned)((pb + REF_THREADS - 1) / REF_THREADS), nc), REF_THREADS, 0, stream>>>(k, c0);
+      }
   }
   return cudaGetLastError();
 }

@@ -310,7 +310,8 @@ DPGO_API const char *dpgo_chordal_last_error(void);
  * that is merely ill-conditioned returns its (large, fp64-accurate to about cond(H) eps) inverse.  info16 (nullable): 0 macro levels, 1 macro nodes, 2 3-scalar nodes of H (d = 2: n, d = 3: 2n),
  * 3 blocks of H, 4 device bytes of H + factor + fronts, 5 largest own block (scalars), 6 largest boundary (scalars),
  * 7 dissection depth, 8 3 x 3 output blocks, 9 stages (factor + sweep), 10 / 11 / 12 assembly / factorisation /
- * selected-inversion nanoseconds (device events), others 0.  n = 1 needs no device.  Messages: dpgo_last_error(). */
+ * selected-inversion nanoseconds (device events), 13 largest number of macro nodes in one stage (a stage of more than
+ * 65535 runs in several launches), others 0.  n = 1 needs no device.  Messages: dpgo_last_error(). */
 DPGO_API int dpgo_pose_covariances(int n, int d, int64_t m, const int32_t *p1, const int32_t *p2, const double *R,
                                    const double *t, const double *kappa, const double *tau, const double *weight,
                                    const double *T_host, int anchor, int device, int64_t num_pairs, const int32_t *pairs,

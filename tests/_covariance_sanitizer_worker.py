@@ -19,4 +19,10 @@ e2 = edges2.take(keep)
 T2 = pg.chordalInitialization(2, 200, e2)
 cov2 = pg.poseCovariancesGPU(e2, 200, T2, pairs=[[3, 150]])[0]
 assert np.all(np.isfinite(cov2))
+# a 2D star anchored at its hub: non-root macro nodes whose boundary is empty, so the sweep runs no product
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import covariance_cases as cc  # noqa: E402
+hub = cc.make_case("hub2100_anchor_hub", 2)
+code, cov3, _, info3 = cc.call_device(hub)
+assert code == 0 and info3[6] == 0 and info3[1] > 1 and np.all(np.isfinite(cov3))
 print("ok")

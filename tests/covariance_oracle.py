@@ -62,7 +62,8 @@ def jacobians(T, edges):
     R, _ = poses(T, d)
     i, j = edges.p1, edges.p2
     m = len(edges)
-    Ji, Jj = np.zeros((m, d * d + d, b)), np.zeros((m, d * d + d, b))
+    dt = np.result_type(T, edges.R)                      # long double in, long double Jacobians out
+    Ji, Jj = np.zeros((m, d * d + d, b), dtype=dt), np.zeros((m, d * d + d, b), dtype=dt)
     for k, G in enumerate(generators(d)):
         Jj[:, :d * d, k] = (R[j] @ G).reshape(m, d * d)
         RG = R[i] @ G
@@ -135,16 +136,23 @@ def _columns(lu, n, b, anchor, cols_of):
 
 def refine(lu, A, E, X, steps: int = 2):
     """Iterative refinement of the solves X ~ A^-1 E with the residual E - A X in extended precision (np.longdouble):
-    the forward error then no longer carries splu's cond(A) eps, which matters on ill-conditioned graphs."""
-    A = A.tocsr()
-    data, idx, ptr = A.data.astype(np.longdouble), A.indices, A.indptr
-    assert np.all(np.diff(ptr) > 0)
+    the forward error then no longer carries splu's cond(A) eps, which matters on ill-conditioned graphs.  A is a SciPy
+    sparse matrix, or a function returning the long-double product A X of a long-double block of columns X: for a
+    matrix whose values are themselves long double, so that the residuals come from those values rather than from the
+    doubles lu factored."""
+    if callable(A):
+        product = A
+    else:
+        A = A.tocsr()
+        data, idx, ptr = A.data.astype(np.longdouble), A.indices, A.indptr
+        assert np.all(np.diff(ptr) > 0)
+        product = lambda Xc: np.add.reduceat(data[:, None] * Xc[idx], ptr[:-1], axis=0)
     Xl = X.astype(np.longdouble)
     for _ in range(steps):
         Rs = np.empty(X.shape)
         for c0 in range(0, X.shape[1], 16):
             c1 = min(X.shape[1], c0 + 16)
-            AX = np.add.reduceat(data[:, None] * Xl[idx, c0:c1], ptr[:-1], axis=0)
+            AX = product(Xl[:, c0:c1])
             Rs[:, c0:c1] = (E[:, c0:c1].astype(np.longdouble) - AX).astype(np.float64)
         Xl += lu.solve(Rs).astype(np.longdouble)
     return Xl.astype(np.float64)
