@@ -295,11 +295,13 @@ cudaError_t launch_frame_lift(int d, int r, int njobs, int max_poses, const Alig
   if (njobs <= 0 || max_poses <= 0) return cudaSuccess;
   const int elems = max_poses * r * (d + 1);
   const dim3 grid((elems + 255) / 256, njobs);
-#define DPGO_LIFT(R_, D_) \
-  if (r == R_ && d == D_) { k_apply_frame_lift<R_, D_><<<grid, 256, 0, stream>>>(jobs); return cudaGetLastError(); }
-  DPGO_LIFT(3, 3) DPGO_LIFT(4, 3) DPGO_LIFT(5, 3) DPGO_LIFT(2, 2) DPGO_LIFT(3, 2) DPGO_LIFT(5, 2)
-#undef DPGO_LIFT
-  return cudaErrorInvalidValue;
+  bool ok = false;
+  DPGO_DISPATCH(r, d + 1, {
+    k_apply_frame_lift<R, DH - 1><<<grid, 256, 0, stream>>>(jobs);
+    ok = true;
+  });
+  if (!ok) return cudaErrorInvalidValue;
+  return cudaGetLastError();
 }
 
 }  // namespace dpgo

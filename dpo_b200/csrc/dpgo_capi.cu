@@ -319,8 +319,8 @@ int dpgo_problem_create(int n, int d, int r, int device, dpgo_problem_t **out) {
   DPGO_REQUIRE(n <= 100000000, DPGO_ERR_UNSUPPORTED, "n above 1e8 poses: element offsets are 32-bit in the kernels");
   DPGO_REQUIRE(d == 2 || d == 3, DPGO_ERR_UNSUPPORTED, "d must be 2 or 3");
   DPGO_REQUIRE(r >= d, DPGO_ERR_INVALID_ARG, "r must be >= d (ref: assert(r >= d), src/QuadraticProblem.cpp:19)");
-  DPGO_REQUIRE((d == 3 && r <= 5) || (d == 2 && (r <= 3 || r == 5)), DPGO_ERR_UNSUPPORTED,
-               "unsupported rank (compiled instantiations: d=3: r in 3..5; d=2: r in {2,3,5})");
+  DPGO_REQUIRE(r <= DPGO_MAX_RANK, DPGO_ERR_UNSUPPORTED,
+               "r must be <= 8 (DPGO_MAX_RANK: the lifted rows of a pose tile are the 8 rows of an fp64 MMA fragment)");
   DPGO_TRY(require_device(device));
   DPGO_CUDA(cudaSetDevice(device));
   dpgo_problem *p = new (std::nothrow) dpgo_problem();

@@ -32,7 +32,7 @@ void nd_kernel_sizes(const dpgo::nd::Plan &plan, dpgo::KNd &K) {
   K.resident_doubles = 0;
 }
 
-dpgo::nd::Options nd_options(int grid, int r, bool cluster = false) {
+dpgo::nd::Options nd_options(int grid, int r, int dh, bool cluster = false) {
   dpgo::nd::Options opt;
   opt.grid = grid;
   opt.r = r;
@@ -41,8 +41,8 @@ dpgo::nd::Options nd_options(int grid, int r, bool cluster = false) {
   // 3.5 us, and 1.0 us is no faster; sphere2500's 156-pose agents are best with 2.0 us as well)
   if (cluster) opt.t_phase_us = 2.0;
   opt.warps = dpgo::OPT_THREADS / 32;
-  opt.ycap_tiles = dpgo::ND_YCAP_TILES;
-  opt.slot_cap = dpgo::ND_SLOT_CAP;
+  opt.ycap_tiles = dpgo::nd_ycap_tiles(r, dh);
+  opt.slot_cap = dpgo::nd_slot_cap(r);
   if (const char *e = std::getenv("DPGO_ND_CUTS")) opt.force_ncuts = std::atoi(e);
   return opt;
 }
@@ -140,7 +140,7 @@ int ensure_nd(dpgo_problem *p, int slot) {
   std::vector<double> blob;
   auto H = std::make_unique<nd::Hierarchy>();
   try {
-    nd::Options opt = nd_options(p->grid, p->r, p->cluster);
+    nd::Options opt = nd_options(p->grid, p->r, p->dh, p->cluster);
     if (dense) opt.force_ncuts = 0;
     nd::BsrView Q{p->n, p->dh, p->bsr.h_rowptr.data(), p->bsr.h_bcol.data(), p->bsr.h_bval.data()};
     nd::build_hierarchy(Q, opt, *H);
@@ -149,7 +149,7 @@ int ensure_nd(dpgo_problem *p, int slot) {
   } catch (const std::exception &e) {
     return fail(DPGO_ERR_UNSUPPORTED, what + " setup: " + e.what());
   }
-  if (plan.max_ytiles > dpgo::ND_YCAP_TILES || plan.max_slots > dpgo::ND_SLOT_CAP)
+  if (plan.max_ytiles > dpgo::nd_ycap_tiles(p->r, p->dh) || plan.max_slots > dpgo::nd_slot_cap(p->r))
     return fail(DPGO_ERR_UNSUPPORTED, what + ": plan exceeds the shared-memory capacities");
   if ((int)plan.phases.size() > dpgo::nd::MAX_PHASES)
     return fail(DPGO_ERR_UNSUPPORTED, what + ": too many phases");
@@ -270,7 +270,7 @@ int dpgo_nd_debug_emulate(int n, int d, int r, int64_t nb, const int32_t *brow, 
   assemble_bsr(n, trip, rowptr, bc, bv);
   namespace nd = dpgo::nd;
   try {
-    nd::Options opt = nd_options(grid, r);
+    nd::Options opt = nd_options(grid, r, dh);
     opt.force_ncuts = force_cuts;
     opt.shift = shift;
     if (leaf_size > 0) opt.leaf_size = leaf_size;

@@ -1126,8 +1126,8 @@ template <int R, int DH> static cudaError_t launch_optimize_t(const KParams &kp_
   KParams kp = kp_in;
   const bool clock = kp.phase_ns != nullptr;
   const void *kern = optimize_kernel<R, DH>(clock);
-  static_assert((OPT_SMEM_BASE_DOUBLES + (size_t)ND_YCAP_TILES * R * DH + (size_t)(ND_SLOT_CAP + 1) * nd::PANEL_ROWS * R +
-                 4 * (size_t)ND_YCAP_TILES + 8) * sizeof(double) <= (size_t)OPT_SMEM_LIMIT,
+  static_assert((OPT_SMEM_BASE_DOUBLES + (size_t)nd_ycap_tiles(R, DH) * R * DH + (size_t)(nd_slot_cap(R) + 1) * nd::PANEL_ROWS * R +
+                 4 * (size_t)nd_ycap_tiles(R, DH) + 8) * sizeof(double) <= (size_t)OPT_SMEM_LIMIT,
                 "what a plan at the shared-memory capacities stages must fit the kernel's maximum shared memory");
   kp.smem_doubles = (int)optimize_smem_doubles<R, DH>(kp);
   const size_t smem = (size_t)kp.smem_doubles * sizeof(double);

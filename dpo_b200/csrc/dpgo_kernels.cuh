@@ -34,8 +34,13 @@ enum OpCode {
 constexpr int NRED = 4;            // scalars reduced per phase
 constexpr int OPT_THREADS = 512;   // persistent kernel block size
 constexpr int SPMV_GROUP_BLOCKS = 192;  // blocks per row group of the TMA-fed SpMV (24 KB of Q per smem stage)
-constexpr int ND_YCAP_TILES = 600;  // sparse exact preconditioner: pose tiles of a phase's input vector staged in shared memory per step
-constexpr int ND_SLOT_CAP = 240;    // ... and partial-sum slots (8 rows x r doubles) per step
+// Shared-memory capacities of one step of the block solve (sparse and dense exact preconditioners): pose tiles of a phase's
+// input vector staged per step (r x (d+1) doubles each), and partial-sum slots (8 rows x r doubles each).  Both areas grow
+// with r, so above r (d+1) = 20 and r = 5 the counts shrink in proportion: a plan at the capacities never stages more than
+// one at (r, d+1) = (5, 4) does, and what it leaves to the resident panel columns stays above 30 KB.  The planner honours
+// smaller capacities with smaller steps (more of them, or column-chunked ones).
+constexpr int nd_ycap_tiles(int r, int dh) { return r * dh <= 20 ? 600 : 12000 / (r * dh); }
+constexpr int nd_slot_cap(int r) { return r <= 5 ? 240 : 1200 / r; }
 constexpr int OPT_SMEM_LIMIT = 227 * 1024;  // dynamic shared memory one CTA of an H100 may ask for (checked by optimize_max_grid)
 constexpr int SP_CACHE_INTS = 2048;  // shared-memory copy of a CTA's block-CSR structure (row pointers + block columns), 8 KB
 
@@ -84,7 +89,8 @@ struct KParams {
   const unsigned char *gate;   // nullable: the agent's byte of a selection mask; 0 = the launch returns at entry
 };
 
-// Instantiations of the compiled (r, d+1) pairs (every pair dpgo_problem_create accepts); R and DH are constexpr in the body.
+// Instantiations of the compiled (r, d+1) pairs, every d <= r <= DPGO_MAX_RANK (the pairs dpgo_problem_create accepts); R and
+// DH are constexpr in the body.
 #define DPGO_DISPATCH(R_, DH_, ...)                                    \
   do {                                                                   \
     if ((DH_) == 4) {                                                    \
@@ -92,13 +98,20 @@ struct KParams {
         case 3: { constexpr int R = 3, DH = 4; __VA_ARGS__; } break;     \
         case 4: { constexpr int R = 4, DH = 4; __VA_ARGS__; } break;     \
         case 5: { constexpr int R = 5, DH = 4; __VA_ARGS__; } break;     \
+        case 6: { constexpr int R = 6, DH = 4; __VA_ARGS__; } break;     \
+        case 7: { constexpr int R = 7, DH = 4; __VA_ARGS__; } break;     \
+        case 8: { constexpr int R = 8, DH = 4; __VA_ARGS__; } break;     \
         default: break;                                                  \
       }                                                                  \
     } else if ((DH_) == 3) {                                             \
       switch (R_) {                                                      \
         case 2: { constexpr int R = 2, DH = 3; __VA_ARGS__; } break;     \
         case 3: { constexpr int R = 3, DH = 3; __VA_ARGS__; } break;     \
+        case 4: { constexpr int R = 4, DH = 3; __VA_ARGS__; } break;     \
         case 5: { constexpr int R = 5, DH = 3; __VA_ARGS__; } break;     \
+        case 6: { constexpr int R = 6, DH = 3; __VA_ARGS__; } break;     \
+        case 7: { constexpr int R = 7, DH = 3; __VA_ARGS__; } break;     \
+        case 8: { constexpr int R = 8, DH = 3; __VA_ARGS__; } break;     \
         default: break;                                                  \
       }                                                                  \
     }                                                                    \

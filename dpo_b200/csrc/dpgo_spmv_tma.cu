@@ -275,15 +275,7 @@ cudaError_t launch_spmv_tma(int r, int dh, int ngroups, const int2 *gi, const in
                             const double *bval, const double *X, const double *G, double *out, int sms,
                             cudaStream_t stream) {
   cudaError_t e = cudaErrorInvalidValue;
-  if (dh == 4) {
-    if (r == 3) e = launch_tma_t<3, 4>(ngroups, gi, rowptr, bcol, bval, X, G, out, sms, stream);
-    else if (r == 4) e = launch_tma_t<4, 4>(ngroups, gi, rowptr, bcol, bval, X, G, out, sms, stream);
-    else if (r == 5) e = launch_tma_t<5, 4>(ngroups, gi, rowptr, bcol, bval, X, G, out, sms, stream);
-  } else if (dh == 3) {
-    if (r == 2) e = launch_tma_t<2, 3>(ngroups, gi, rowptr, bcol, bval, X, G, out, sms, stream);
-    else if (r == 3) e = launch_tma_t<3, 3>(ngroups, gi, rowptr, bcol, bval, X, G, out, sms, stream);
-    else if (r == 5) e = launch_tma_t<5, 3>(ngroups, gi, rowptr, bcol, bval, X, G, out, sms, stream);
-  }
+  DPGO_DISPATCH(r, dh, e = (launch_tma_t<R, DH>(ngroups, gi, rowptr, bcol, bval, X, G, out, sms, stream)));
   return e;
 }
 

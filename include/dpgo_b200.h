@@ -32,6 +32,10 @@ extern "C" {
 
 #define DPGO_B200_ABI_VERSION 1
 
+/* Largest relaxation rank r: a pose tile's r lifted rows are the rows of the 8 x 4 A fragment of the fp64 tensor op
+   (mma.sync m8n8k4) in the product with Q and in the block solve. */
+#define DPGO_MAX_RANK 8
+
 #if defined(__GNUC__)
 #define DPGO_API __attribute__((visibility("default")))
 #else
@@ -47,7 +51,7 @@ enum {
   DPGO_ERR_CUDA = 3,        /* a CUDA runtime call or kernel failed, or a numerical solve failed (the chordal
                                initialisation's conjugate gradients broke down or did not converge in max_iter) */
   DPGO_ERR_STATE = 4,       /* call order violation (e.g. optimise before set_Q) */
-  DPGO_ERR_UNSUPPORTED = 5, /* d not in {2,3}; r outside the compiled set (d=3: 3..5, d=2: 2,3,5); an exact
+  DPGO_ERR_UNSUPPORTED = 5, /* d not in {2,3}; r above DPGO_MAX_RANK (every d <= r <= 8 is compiled); an exact
                                preconditioner whose blocks would exceed 24 GB (DENSE_EXACT: N above about 54k) */
   DPGO_ERR_ALLOC = 6
 };
