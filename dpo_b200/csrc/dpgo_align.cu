@@ -216,7 +216,7 @@ __global__ void __launch_bounds__(ALIGN_THREADS) k_robust_rotation_average(const
         double nc[1] = {0.0};
         for (int q = q0 + tid; q < q1; q += ALIGN_THREADS) {
           const double rr = sqrt(residual2(q, R));     // the reference passes r = sqrt(r^2) to RobustCost::weight
-          const double wq = gnc_tls_weight(rr * rr, mu, cbar);
+          const double wq = gnc_tls_weight(rr, mu, cbar);
           J.w[q] = wq;
           if (wq < W_TOL || wq > 1.0 - W_TOL) nc[0] += 1.0;
         }

@@ -1075,13 +1075,14 @@ __global__ void k_edge_weights(int64_t m, const int *__restrict__ p1, const int 
   const double r2 = om[0] * rot + om[D] * tra;
   if (resid) resid[e] = r2;
   if (fixed && fixed[e]) return;
+  // the reference passes r = sqrt(r^2) to RobustCost::weight, which squares it again: every weight is a function of r
   const double r = sqrt(r2);
   double wt = 1.0;
   if (cost == 1) wt = 1.0 / r;
   else if (cost == 2) wt = (r < param) ? 1.0 : param / r;
   else if (cost == 3) wt = (r < param) ? 1.0 : 0.0;
-  else if (cost == 4) { const double s = 1.0 + r2; wt = 1.0 / (s * s); }
-  else if (cost == 5) wt = gnc_tls_weight(r2, mu, param);
+  else if (cost == 4) { const double s = 1.0 + __dmul_rn(r, r); wt = 1.0 / (s * s); }    // r*r rounded, not fused
+  else if (cost == 5) wt = gnc_tls_weight(r, mu, param);
   w[e] = wt;
   // the counts of the reference's computeConvergedLoopClosureRatio (src/PGOAgent.cpp:1247-1289); integers, so deterministic
   if (gnc) atomicAdd(gnc + (wt == 1.0 ? 0 : (wt == 0.0 ? 1 : 2)), 1ULL);

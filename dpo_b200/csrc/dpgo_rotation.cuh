@@ -189,13 +189,14 @@ template <int R, int DH, class In, class Out> __device__ __forceinline__ void st
   for (int a = 0; a < R; ++a) out(D * R + a, in(D * R + a));
 }
 
-// GNC-TLS weight of a squared residual r2 at control parameter mu and threshold cbar (Yang et al., eq. 14; ref
+// GNC-TLS weight of a residual r at control parameter mu and threshold cbar (Yang et al., eq. 14; ref
 // RobustCost::weight, src/DPGO_robust.cpp:49-61): 0 above (mu+1)/mu cbar^2, 1 below mu/(mu+1) cbar^2, in between
-// cbar sqrt(mu (mu+1)) / r - mu.
-__device__ __forceinline__ double gnc_tls_weight(double r2, double mu, double cbar) {
-  const double c2 = cbar * cbar;
-  if (r2 >= c2 * (mu + 1.0) / mu) return 0.0;
-  if (r2 <= c2 * mu / (mu + 1.0)) return 1.0;
+// cbar sqrt(mu (mu+1)) / r - mu.  Every operation in the reference's order, so that the weights that are exactly 0 or 1
+// (which the GNC stop counts) are the reference's: r is squared again, and the bounds are (mu+1)/mu c^2 and mu/(mu+1) c^2.
+__device__ __forceinline__ double gnc_tls_weight(double r, double mu, double cbar) {
+  const double r2 = r * r, c2 = cbar * cbar;
+  if (r2 >= (mu + 1.0) / mu * c2) return 0.0;
+  if (r2 <= mu / (mu + 1.0) * c2) return 1.0;
   return sqrt(c2 * mu * (mu + 1.0) / r2) - mu;
 }
 

@@ -30,8 +30,9 @@ inline double geman_mcclure_weight(double r) {
 
 inline double gnc_tls_weight(double r, double mu, double cbar) {
   const double r2 = r * r, c2 = cbar * cbar;
-  if (r2 >= c2 * (mu + 1) / mu) return 0.0;     // certainly an outlier at this stage of the schedule
-  if (r2 <= c2 * mu / (mu + 1)) return 1.0;     // certainly an inlier
+  // the bounds in the reference's order: a different order rounds differently, and the 0 / 1 weights are counted exactly
+  if (r2 >= (mu + 1) / mu * c2) return 0.0;     // certainly an outlier at this stage of the schedule
+  if (r2 <= mu / (mu + 1) * c2) return 1.0;     // certainly an inlier
   return std::sqrt(c2 * mu * (mu + 1) / r2) - mu;
 }
 

@@ -4,6 +4,7 @@
 // gpu-marked tests.)
 #include <cmath>
 #include <cstdio>
+#include <cstdlib>
 #include <string>
 #include <vector>
 
@@ -20,9 +21,29 @@ static void print_matrix(const char *key, const Matrix &M) {
   std::printf("\n");
 }
 
+// `host_check --weights <file>`: one line `cost r mu c` per probe (cost as in RobustCostNames, the numbers in any strtod
+// form, hex floats included), RobustCost::weight(r) printed as `weight %a` per line, exactly.  mu and c enter through
+// RobustCostParameters (GNCInitMu, GNCBarc, Huber and TLS thresholds), as a caller sets them.
+static int robust_weights(const char *path) {
+  FILE *f = std::fopen(path, "r");
+  if (!f) { std::fprintf(stderr, "cannot open %s\n", path); return 2; }
+  char name[32], rs[64], mus[64], cs[64];
+  while (std::fscanf(f, "%31s %63s %63s %63s", name, rs, mus, cs) == 4) {
+    const double r = std::strtod(rs, nullptr), mu = std::strtod(mus, nullptr), c = std::strtod(cs, nullptr);
+    int t = 0;
+    while (t < (int)RobustCostNames.size() && RobustCostNames[t] != name) ++t;
+    if (t == (int)RobustCostNames.size()) { std::fprintf(stderr, "unknown cost %s\n", name); return 2; }
+    RobustCost cost((RobustCostType)t, RobustCostParameters(100, c, 1.4, mu, c, c));
+    std::printf("weight %a\n", cost.weight(r));
+  }
+  std::fclose(f);
+  return 0;
+}
+
 int main(int argc, char **argv) {
+  if (argc == 3 && std::string(argv[1]) == "--weights") return robust_weights(argv[2]);
   if (argc < 3) {
-    std::fprintf(stderr, "usage: host_check <file.g2o> <chordal_out.txt>\n");
+    std::fprintf(stderr, "usage: host_check <file.g2o> <chordal_out.txt> | host_check --weights <probes.txt>\n");
     return 2;
   }
   size_t n = 0;

@@ -12,6 +12,8 @@ lengths, times u.  Such a bound holds for any summation order, so it does not de
 """
 from __future__ import annotations
 
+import os
+import re
 from dataclasses import dataclass
 from typing import Optional
 
@@ -23,11 +25,29 @@ from dpo_b200 import posegraph as pg
 # mirrored from dpgo_kernels.cuh / nd_precond.h
 SPMV_GROUP_BLOCKS = 192      # blocks per row group of the TMA-fed Q.X product; a longer row sends it to the gather kernel
 SP_CACHE_INTS = 2048         # a CTA's block-CSR slice (rows + 1 + blocks) beyond this is read from global memory
-ND_YCAP_TILES = 600          # shared-memory tile capacity of one nested-dissection step (larger leaves: column chunks)
 DENSE_MAX_N = 12000          # the dense exact preconditioner (one macro level) is exercised up to this N ((d+1) n)
 U = 2.0 ** -53               # unit roundoff of float64
 
-RANKS = {3: (3, 4, 5), 2: (2, 3, 5)}   # every compiled relaxation rank per d
+
+def _max_rank():
+    """DPGO_MAX_RANK of the C header: every d <= r <= DPGO_MAX_RANK is compiled"""
+    hdr = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "dpgo_b200.h")
+    with open(hdr) as fh:
+        return int(re.search(r"^#define DPGO_MAX_RANK (\d+)", fh.read(), re.M).group(1))
+
+
+MAX_RANK = _max_rank()
+RANKS = {d: tuple(range(d, MAX_RANK + 1)) for d in (3, 2)}   # every compiled relaxation rank per d: d <= r <= DPGO_MAX_RANK
+
+
+def nd_ycap_tiles(r, dh):
+    """shared-memory tile capacity of one nested-dissection step at rank r (larger leaves: column chunks)"""
+    return 600 if r * dh <= 20 else 12000 // (r * dh)
+
+
+def nd_slot_cap(r):
+    """partial-sum slots of one nested-dissection step at rank r"""
+    return 240 if r <= 5 else 1200 // r
 
 
 @dataclass
@@ -160,7 +180,12 @@ def _multi_edges(rng):
 
 CASE_NAMES = ("single", "single_prior", "pair", "triple", "hub191", "hub192", "hub2100", "tail_isolated", "components",
               "clique700", "multi_edges", "long_chain")
-LARGE = ("hub2100", "long_chain")             # run with r in {d, 5} only
+LARGE = ("hub2100", "long_chain")             # run with r in large_ranks(d) only, as clique700
+
+
+def large_ranks(d):
+    """the ranks the largest cases run at: d, the largest rank of the fixed capacities (5) and DPGO_MAX_RANK"""
+    return (d, 5, MAX_RANK)
 
 
 def make_case(name: str, d: int, seed: int = 0) -> Case:
@@ -192,7 +217,7 @@ def make_case(name: str, d: int, seed: int = 0) -> Case:
     elif name == "clique700":
         n = 700 if d == 3 else 701
         pairs = _clique(n)
-        target = "ND leaf > ND_YCAP_TILES; n even (N = 2800) and odd (N = 2103: the last panel half used)"
+        target = "ND leaf > nd_ycap_tiles at every rank; n even (N = 2800) and odd (N = 2103: the last panel half used)"
     elif name == "multi_edges":
         (n, pairs), target = _multi_edges(rng), "duplicated and reversed edges, both directions, random sparse part"
     elif name == "long_chain":

@@ -27,9 +27,9 @@ def host_weight(cost, r, mu, c):
     if cost == "GM":
         return 1.0 / (1.0 + r * r) ** 2
     r2, c2 = r * r, c * c
-    if r2 >= c2 * (mu + 1) / mu:
+    if r2 >= (mu + 1) / mu * c2:
         return 0.0
-    if r2 <= c2 * mu / (mu + 1):
+    if r2 <= mu / (mu + 1) * c2:
         return 1.0
     return np.sqrt(c2 * mu * (mu + 1) / r2) - mu
 

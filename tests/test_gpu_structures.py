@@ -11,7 +11,7 @@ from oracle import dpgo_oracle as orc
 pytestmark = pytest.mark.gpu
 
 PARAMS = [(name, d, r) for name in sc.CASE_NAMES for d in (2, 3) for r in sc.RANKS[d]
-          if not (name in sc.LARGE + ("clique700",) and r not in (d, 5))]
+          if not (name in sc.LARGE + ("clique700",) and r not in sc.large_ranks(d))]
 _CASES = {}
 
 

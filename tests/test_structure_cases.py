@@ -75,7 +75,7 @@ def test_clique_reaches_its_branch(d, cases):
     rb = c.row_blocks()
     assert c.n == len(rb) and c.Q().shape == (c.N, c.N)
     assert c.N == {3: 2800, 2: 2103}[d] and rb.min() == c.n
-    assert c.n > sc.ND_YCAP_TILES and c.n % 2 == {3: 0, 2: 1}[d]
+    assert all(c.n > sc.nd_ycap_tiles(r, c.dh) for r in sc.RANKS[d]) and c.n % 2 == {3: 0, 2: 1}[d]
     assert c.N <= sc.DENSE_MAX_N
 
 
@@ -88,14 +88,15 @@ def test_emulated_plan_on_structure_cases(name, d, cases):
     if len(brow) == 0:                       # an empty Q: one zero block keeps the triplet arrays non-empty
         brow, bcol, blocks = np.array([0]), np.array([0]), np.zeros((1, c.dh, c.dh))
     rng = np.random.default_rng(7)
-    for r in (d, 5):
+    for r in sc.large_ranks(d):
         V = rng.standard_normal((r, c.N))
         ref = dense_reference(c.n, c.dh, brow, bcol, blocks, V)
         for grid in (132, 16):
             Z, info = emulate(c.n, d, r, brow, bcol, blocks, V, grid=grid)
             assert relerr(Z, ref) <= 1e-11, (name, d, r, grid, info)
             if name == "clique700":
-                assert info["max_own"] == c.N and info["max_ytiles"] == sc.ND_YCAP_TILES     # one leaf, column-chunked
+                assert info["max_own"] == c.N and info["max_ytiles"] == sc.nd_ycap_tiles(r, c.dh)   # one leaf, chunked
+            assert info["max_ytiles"] <= sc.nd_ycap_tiles(r, c.dh) and info["max_slots"] <= sc.nd_slot_cap(r), (r, info)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
