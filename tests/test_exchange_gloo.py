@@ -123,6 +123,57 @@ def test_exchange_plan_four_agents_on_two_ranks_gloo():
         assert ret[rk][0] <= 1e-12, ret[rk]
 
 
+def _gathered_worker(rank, world, port, ret):
+    sys.path.insert(0, ROOT)
+    import torch
+    import torch.distributed as dist
+    from dpo_b200.agent import _Gathered
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    try:
+        mine = [2 * rank, 2 * rank + 1]
+        g = _Gathered(torch, torch.device("cpu"), 4, mine, 3, True)
+        assert g.own.numel() == 2 * 3 and g.own.data_ptr() != g.all.data_ptr()
+        for a in mine:
+            g.part[a].copy_(10.0 * a + torch.arange(3, dtype=torch.float64))
+        g.gather(dist)
+        ret[rank] = g.all.tolist()
+    finally:
+        dist.destroy_process_group()
+
+
+def test_gathered_buffer_four_agents_on_two_ranks_gloo():
+    """The runner's gathered buffers over world = 2 ranks with two agents each: after the all-gather every rank holds agent
+    a's part at a * part, in agent order."""
+    import torch.multiprocessing as mp
+    port = 29500 + (os.getpid() % 90)
+    mgr = mp.Manager()
+    ret = mgr.dict()
+    procs = [mp.get_context("spawn").Process(target=_gathered_worker, args=(rk, 2, port, ret)) for rk in range(2)]
+    for p in procs:
+        p.start()
+    for p in procs:
+        p.join(180)
+        assert p.exitcode == 0
+    expect = [10.0 * a + i for a in range(4) for i in range(3)]
+    assert ret[0] == expect and ret[1] == expect
+
+
+def test_gathered_buffer_one_rank_writes_in_place():
+    """With one rank each agent's part is a view of `all` (no copy, nothing to gather)."""
+    import torch
+    sys.path.insert(0, ROOT)
+    from dpo_b200.agent import _Gathered
+    g = _Gathered(torch, torch.device("cpu"), 4, [0, 1, 2, 3], 3, False)
+    for a in range(4):
+        assert g.part[a].untyped_storage().data_ptr() == g.all.untyped_storage().data_ptr()
+        assert g.part[a].data_ptr() == g.all.data_ptr() + a * 3 * 8
+        g.part[a].fill_(a)
+    g.gather(None)
+    assert g.all.tolist() == [float(a) for a in range(4) for _ in range(3)]
+
+
 def test_partition_and_colouring():
     sys.path.insert(0, ROOT)
     from dpo_b200 import posegraph as pg

@@ -59,8 +59,8 @@ def test_batched_begin_equals_per_agent_calls(data_dir):
     lib = new.agents[0].mProblem._lib
     ids = new.local_ids
     hs = (C.c_void_p * 5)(*[new.agents[a].mProblem._h for a in ids])
-    sx = (C.c_void_p * 5)(*[C.c_void_p(new.send[a].data_ptr()) for a in ids])
-    sy = (C.c_void_p * 5)(*[C.c_void_p(new.send_aux[a].data_ptr()) for a in ids])
+    sx = (C.c_void_p * 5)(*[C.c_void_p(new.tiles.part[a].data_ptr()) for a in ids])
+    sy = (C.c_void_p * 5)(*[C.c_void_p(new.aux_tiles.part[a].data_ptr()) for a in ids])
     flags = np.zeros(5, dtype=np.int32)
     trace = ao.momentum_trace(5.0, 32, 30)
     import torch
@@ -77,10 +77,10 @@ def test_batched_begin_equals_per_agent_calls(data_dir):
             if (i + 2) % 30 == 0:
                 _capi.check(lib.dpgo_agent_accel_restart_begin(h))
                 _capi.check(lib.dpgo_agent_accel_restart_end(h))
-            old.agents[a].pack_public(old.send[a].data_ptr())
-            _capi.check(lib.dpgo_agent_pack_public_aux(h, C.c_void_p(old.send_aux[a].data_ptr())))
+            old.agents[a].pack_public(old.tiles.part[a].data_ptr())
+            _capi.check(lib.dpgo_agent_pack_public_aux(h, C.c_void_p(old.aux_tiles.part[a].data_ptr())))
         torch.cuda.synchronize()
-        assert torch.equal(new.gathered, old.gathered) and torch.equal(new.gathered_aux, old.gathered_aux), i
+        assert torch.equal(new.tiles.all, old.tiles.all) and torch.equal(new.aux_tiles.all, old.aux_tiles.all), i
         for a in ids:
             assert np.array_equal(new.agents[a].mProblem.download_X(), old.agents[a].mProblem.download_X()), (i, a)
 

@@ -192,7 +192,7 @@ def test_align_call_with_an_agent_without_shared_edges(data_dir):
     ready = np.zeros(8, dtype=np.int32)
     ready[0] = 1
     hs = (C.c_void_p * 2)(run.agents[1].mProblem._h, lone._h)
-    capi.check(lib.dpgo_agents_align_async(hs, 2, C.c_void_p(run.gathered.data_ptr()), 8 * run.plan.pmax, capi.iptr(ready), 8,
+    capi.check(lib.dpgo_agents_align_async(hs, 2, C.c_void_p(run.tiles.all.data_ptr()), 8 * run.plan.pmax, capi.iptr(ready), 8,
                                            None))
     info = np.zeros(4, dtype=np.int32)
     capi.check(lib.dpgo_agent_align_result(lone._h, None, capi.iptr(info)))

@@ -22,27 +22,12 @@ def make(schedule, acceleration):
 
 
 def setup_calls(run, X0):
-    """The setup sequence of the runner's constructor, issued again on its live handles."""
-    from dpo_b200 import _capi as capi
-    from dpo_b200.agent import alignment_candidates
+    """The setup sequence of the runner's constructor, issued again on its live handles, with the alignment candidates of
+    the distributed start too."""
     for a in run.local_ids:
-        ag = run.agents[a]
-        lib, h = ag.mProblem._lib, ag.mProblem._h
-        ag.constructQMatrix()                       # dpgo_problem_set_edges: build_from_triplets, then reassemble_Q
-        ag.attach_exchange(run.plan)                # public poses, shared edges
-        ct = alignment_candidates(a, ag.sharedLoopClosures, run.plan)
-        capi.check(lib.dpgo_agent_set_align_candidates(h, len(ct["neighbor"]), capi.iptr(ct["neighbor"]),
-                                                       capi.iptr(ct["ptr"]), capi.iptr(ct["local"]), capi.iptr(ct["slot"]),
-                                                       capi.iptr(ct["outgoing"]), capi.dptr(ct["T"])))
-        ag.mProblem.upload_X(X0[a])
-        if run.acceleration:
-            capi.check(lib.dpgo_agent_accel_init(h))
-    if run.schedule == "greedy_set":
-        nb = [run.plan.tables[a]["neighbors"] for a in range(run.k)]
-        ptr = np.concatenate([[0], np.cumsum([len(x) for x in nb])]).astype(np.int32)
-        adj = np.array([b for x in nb for b in x] or [0], dtype=np.int32)
-        lead = run.agents[run.local_ids[0]].mProblem
-        capi.check(lead._lib.dpgo_agents_set_agent_graph(lead._h, run.k, capi.iptr(ptr), capi.iptr(adj)))
+        run.agents[a].constructQMatrix()            # dpgo_problem_set_edges: build_from_triplets, then reassemble_Q
+        run.agents[a].mProblem.upload_X(X0[a])
+    run._setup_agents(candidates=True)              # public poses, shared edges, candidates, accel_init, agent graph
     run.round = 0
     run.selected = [0]
     run._gathered_current = False
